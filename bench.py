@@ -55,12 +55,12 @@ def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.isfile(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1405.3), d.get("bf16_tflops", 1652.1), d.get("hbm_gbs", 6560.6), "measured"
-    return 1400.0, 1590.0, 6650.0, "fallback"
+        return d.get("bf16_tflops_sustained", 989.0), d.get("bf16_tflops", 989.0), d.get("hbm_gbs", 3350.0), "measured"
+    return 989.0, 989.0, 3350.0, "fallback: H100 SXM data sheet (dense fp16 / bf16, HBM3), not reached"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     def __init__(self, gpu_index):
         self.rows = []
@@ -107,21 +107,6 @@ class ClockSampler:
         sm.sort()
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": smax, "reasons": sorted(reasons),
                 "samples": len(sm), "power_w_max": max(power) if power else None}
-
-
-def ncu_traffic():
-    """DRAM bytes (read + write) of the tcgen05 conv launches of one step, from the newest committed `ncu --set full`
-    capture (profiles/r*_traffic.json); (None, None) if there is none.  NOT measured by this run: bench.py cannot run
-    under a profiler and report a timing at once."""
-    import glob
-    files = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_traffic.json")))
-    for f in reversed(files):
-        try:
-            t = json.load(open(f))
-            return int(t["dram_bytes_read"] + t["dram_bytes_write"]), "committed capture %s: %s" % (os.path.basename(f), t["source"])
-        except (OSError, KeyError, ValueError):
-            continue
-    return None, None
 
 
 # --------------------------------------------------------------------------------------------- CPU oracle ----
@@ -268,31 +253,6 @@ class Job:
             self.dist.destroy_process_group()
 
 
-def umma_isolated(device):
-    """kind::f16 tcgen05.mma throughput with operands resident in shared memory (dcscn_umma_probe, csrc/umma_probe.cuh),
-    measured in this run: the pipe's peak at N = 256 and the cost of one K = 16 slice of the three-product scheme for the
-    widths of the thin layers (a UMMA cannot go faster than its operands leave shared memory: ~40 cycles at N <= 80)."""
-    import ctypes
-    from helper import engine as E
-    lib = E.load_library()
-
-    def one(n, mode, iters=3000):
-        ms, cyc = ctypes.c_float(), ctypes.c_double()
-        if lib.dcscn_umma_probe(device, 2, n, mode, iters, ctypes.byref(ms), ctypes.byref(cyc)):
-            return None
-        prods = 3 if mode == 0 else 1
-        macs = 74 * iters * 4 * prods * 256 * n * 16
-        return {"tflops_issued": round(2 * macs / (ms.value * 1e-3) / 1e12, 1), "cycles_per_k16_slice": round(cyc.value / (iters * 4), 1)}
-    try:
-        out = {"what": "tcgen05.mma kind::f16 cta_group::2 M=256, both operands in shared memory, 74 CTA pairs, no loads / epilogue",
-               "n256_three_products": one(256, 0)}
-        for n in (48, 80, 112, 160):
-            out["n%d_three_products" % n] = one(n, 0)
-        return out
-    except Exception as e:  # noqa: BLE001
-        return {"error": "%s: %s" % (type(e).__name__, e)}
-
-
 def headline(job, args):
     import torch
     from helper import engine as E
@@ -324,6 +284,7 @@ def headline(job, args):
     job.barrier()
     ms = job.max_over_ranks(ev0.elapsed_time(ev1))
     launches = eng.launch_count - launches0
+    y_last = y.cpu().numpy() if args.dump_outputs else None   # what the last timed step returned
     clocks = sampler.stop() if rank == 0 else None
     out_px_step = BATCH * (SCALE * TILE) ** 2
     value = world * out_px_step * args.steps / (ms / 1e3) / 1e6
@@ -350,16 +311,16 @@ def headline(job, args):
     torch.cuda.synchronize()
     per = {k: _median(v) for k, v in per.items()}
 
-    # ---- strict setting: every (chunk, dx) unit promoted to the fp32 RN sum (seg_chunks = 1): the setting that holds
+    # ---- strict setting: every 16-channel K slice promoted to the fp32 RN sum (seg_chunks = 1): the setting that holds
     # 1e-3 absolute against the fp64 forward on these uniform-noise tiles (tests/test_gpu_forward.py) ----
     eng.set_option("seg_chunks", 1)
     n_strict = max(5, min(args.steps, 20))
     ms_strict = job.timed(lambda i: eng.forward(x, x2, y), n_strict, 3) / n_strict
     eng.close()
-    strict = {"setting": "seg_chunks=1 (fp32 promotion after every (64-channel chunk, dx) unit of K = 192)",
+    strict = {"setting": "seg_chunks=1 (fp32 promotion after every 16-channel K slice)",
               "ms_per_step": ms_strict, "value": world * out_px_step / (ms_strict / 1e3) / 1e6, "unit": "Mpixels/s",
-              "noise_tile_error": "<= 1e-3 absolute vs the fp64 forward (default periods: ~1.35e-3; fp32 CPU forward: ~2.4e-3)"}
-    return dict(ms=ms, value=value, e2e_value=e2e_value, launches=launches, clocks=clocks, per=per, warm=warm, strict=strict,
+              "noise_tile_error": "<= 1e-3 absolute vs the fp64 forward (tests/test_gpu_forward.py)"}
+    return dict(ms=ms, value=value, e2e_value=e2e_value, launches=launches, clocks=clocks, per=per, warm=warm, strict=strict, y=y_last,
                 h2d=int(x_host.numel() * 4 + x2_host.numel() * 4), d2h=int(y_host.numel() * 4))
 
 
@@ -525,9 +486,19 @@ def sub_latency(job, args):
     return res
 
 
+def dump_outputs(d, y):
+    """The headline's output of its last timed step, [BATCH, 96, 96, 1] float32 (9.4 MB): with the same arguments the
+    seeded inputs are identical from run to run, so two builds can be compared output for output."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    np.save(os.path.join(d, "y.npy"), np.ascontiguousarray(y, dtype=np.float32))
+
+
 def run_ours(args, rank, world, local_rank):
     job = Job(rank, world, local_rank)
     hd = headline(job, args)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, hd["y"])
     subs = {}
     if args.sub:
         for name, fn in (("ensemble8", sub_ensemble), ("train", sub_train), ("ds", sub_ds), ("latency", sub_latency)):
@@ -546,20 +517,14 @@ def run_ours(args, rank, world, local_rank):
         tc_flops = 2.0 * MAC_PER_LR_PX_TC * lr_px
         achieved = tc_flops / (tc_ms / 1e3) / 1e12
         passes = 3 if args.precision == "f16x3" else 1
-        traffic, traffic_src = ncu_traffic()
-        isolated = umma_isolated(job.local)
         roofline = {
             "bound": "tensor",
-            "kernel": "conv_tc_halo2_kernel (3x3 layers) / conv_tc_pair_kernel (A1+B1): the %d tcgen05 conv launches of one step" % len(tc_names),
+            "kernel": "conv_tc_kernel: the %d wgmma conv launches of one step" % len(tc_names),
             "achieved": achieved, "peak": sustained, "unit": "TFLOP/s", "frac": achieved / sustained,
-            "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (%s); kind::f16 UMMAs issue at the bf16 rate - the pipe "
-                           "measured in isolation in this run is `kind_f16_isolated`" % how,
-            "kind_f16_isolated": isolated,
+            "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (%s); fp16 wgmma issues at the bf16 rate" % how,
             "algorithmic_flop_per_launch_set": tc_flops, "launch_set_ms": tc_ms,
             "launch_ms_method": "CUDA events around every launch on the launching stream, median of >= 5 steps",
             "mma_passes": passes, "frac_of_issued_mma": achieved * passes / sustained,
-            "traffic": traffic, "traffic_unit": "DRAM bytes (read + write) of the same launches of one step",
-            "traffic_source": traffic_src,
             "launch_ms": {k: round(v, 4) for k, v in per.items()},
         }
         secs, cores = cpu_oracle_passes(max(3, int(args.cpu_seconds / 0.7)), 1)
@@ -573,7 +538,7 @@ def run_ours(args, rank, world, local_rank):
             "config": {"workload": "DCSCN L12 F196->48 x2 inference, batch=256 synthetic 48x48 Y-tiles per GPU "
                                    "(BASELINE.json configs[1]), weights = reference L12 x2 checkpoint",
                        "global_batch": BATCH * world, "parallelism": "dp%d (independent tiles, no collective)" % world,
-                       "l2": "per-step working set (activation planes) 4.3 GB >> 126 MB L2; no explicit flush"},
+                       "l2": "per-step working set (activation planes) 4.3 GB >> 50 MB L2; no explicit flush"},
             "clocks": hd["clocks"],
             "e2e": {"value": hd["e2e_value"], "unit": "Mpixels/s", "h2d_bytes_per_step": hd["h2d"], "d2h_bytes_per_step": hd["d2h"]},
             "gpu_launches": int(hd["launches"]),
@@ -610,9 +575,13 @@ def main():
     ap.add_argument("--precision", default="f16x3", choices=["f16x3", "f16x1"])
     ap.add_argument("--cpu-seconds", type=float, default=10.0, dest="cpu_seconds")
     ap.add_argument("--no-sub", action="store_false", dest="sub", help="headline only (skip ensemble8 / train / ds / latency)")
+    ap.add_argument("--dump-outputs", default=None, dest="dump_outputs", metavar="DIR",
+                    help="write the headline's output of its last timed step to DIR/y.npy (float32)")
     ap.add_argument("--workload", default="infer", choices=["infer", "train", "ds", "ensemble", "latency"],
                     help="infer = headline line with all sub-records; the others print one sub-record alone")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "ours" or args.workload != "infer"):
+        ap.error("--dump-outputs writes the headline's output: it needs --impl ours and --workload infer")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))

@@ -1,7 +1,7 @@
 """
 DCSCN.SuperResolution - drop-in for the reference's model class (reference: DCSCN.py:28-769 and its base
-class helper/tf_graph.py:17-305), with the TensorFlow graph / session replaced by the B200 engine
-(hand-written sm_100a CUDA kernels behind the C-ABI of include/dcscn_b200.h).
+class helper/tf_graph.py:17-305), with the TensorFlow graph / session replaced by the H100 engine
+(hand-written sm_90a CUDA kernels behind the C-ABI of include/dcscn_b200.h).
 
 Kept from the reference: constructor arguments (the FLAGS object), the model-name grammar, the call order used
 by the CLIs (`build_graph` -> [`build_optimizer`] -> `build_summary_saver` -> `init_all_variables` ->
@@ -233,7 +233,7 @@ class SuperResolution:
         if self.optimizer != "adam":
             problems.append("--optimizer=%s (only adam)" % self.optimizer)
         if problems:
-            raise NotImplementedError("not supported by the B200 engine: " + ", ".join(problems))
+            raise NotImplementedError("not supported by the H100 engine: " + ", ".join(problems))
 
     # ------------------------------------------------------------------ graph ----
     def _engine_config(self):

@@ -1,4 +1,4 @@
-// Shared host/device declarations for the DCSCN sm_100a hot path.
+// Shared host/device declarations for the DCSCN sm_90a hot path.
 //
 // Data layout in HBM (see DESIGN.md "Data layout"):
 //   * Activations between tensor-core layers are kept as TWO fp16 planes ("hi" and "lo",
@@ -6,14 +6,14 @@
 //     layer of the feature-extraction stack owns a 16-channel-aligned slot of one shared
 //     "concat" buffer, so tf.concat (DCSCN.py:259,281) never materialises.
 //   * Weights are pre-packed per layer into the exact shared-memory image a K-major
-//     SWIZZLE_128B UMMA operand tile needs (hi and lo fp16 planes, scaled by a power of two).
+//     SWIZZLE_128B wgmma operand tile needs (hi and lo fp16 planes, scaled by a power of two).
 #pragma once
 #include <cstdint>
 #include <cuda_fp16.h>
 
 namespace dcscn {
 
-constexpr int kTileM = 128;          // pixels per CTA tile (UMMA M)
+constexpr int kTileM = 128;          // pixels per CTA tile (GEMM M: two m64 wgmma warpgroups)
 constexpr int kMaxSegments = 2;
 
 enum EpilogueMode : int {
@@ -59,9 +59,6 @@ struct EpiParams {
   uint32_t drop_seed;
   uint32_t drop_layer;
   int drop_ntotal;     // channel count the keep-mask index is built with (the slot width; 0 = the GEMM's padded N)
-  int store_mode;      // fp16 plane stores of the tensor-core epilogues: 0 = one 32-byte store per lane and plane (default),
-                       // 1 = two 16-byte stores (rounds 1-2), 2 = 32-byte stores with neighbouring lanes exchanging halves so
-                       // that one instruction covers 64 contiguous bytes of a pixel (streaming 3x3 kernel)
 };
 
 struct ConvGeom {
@@ -75,19 +72,11 @@ struct ConvTCParams {
   int ksz;               // 1 or 3
   int cin_pad;           // padded input channels of the source slot (multiple of 16)
   int chunks;            // ceil(cin_pad / KC)
-  int n_tiles;           // column tiles (N > 256 is split)
-  int n_pad;             // columns per tile, multiple of 16, <= 256
+  int n_tiles;           // column tiles (N > kMaxTileN is split)
+  int n_pad;             // columns per tile, multiple of 16, <= kMaxTileN (128)
   int seg_chunks;        // pipeline stages per accumulation segment (fp32 promotion period)
   int cluster_size;      // CTAs per cluster sharing (multicasting) the weight tiles: 1, 2 or 4
   const __half* wpack;   // packed weights [n_tile][tap][chunk][plane][n_pad x KC] (pre-swizzled)
-  // streaming kernel (conv_tc_halo2.cuh): weight-stage table of one (pixel tile, column tile) item, see kH2* there
-  const uint32_t* h2_stages;
-  int h2_nstages;
-  int h2_nseg;           // fp32-promotion segments per item
-  int h2_resident;       // all stages fit in shared memory: loaded once per CTA
-  int pair_stream;       // conv_tc_pair_kernel: streaming split-accumulator mode (1x1 layers)
-  unsigned long long* dbg;   // diagnostic builds (-DDCSCN_H2_DEBUG): per-cluster wait counters, else null
-  int h2_nreg;           // leading chunks with one tap per stage (issued by the compile-time-structured loop)
   EpiParams epi;
 };
 

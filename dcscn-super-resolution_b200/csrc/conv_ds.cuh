@@ -5,7 +5,7 @@
 //
 // These graphs are tiny (c-DCSCN: <= 131 channels, 14,240 MAC per LR pixel at x4) and bound by HBM traffic, not
 // math: one fused kernel per layer on CUDA cores, fp32 NHWC activations, no tensor cores (a 131 x 24 contraction per
-// pixel does not fill a UMMA tile).  The depthwise result never leaves registers / shared memory.
+// pixel does not fill a tensor-core tile).  The depthwise result never leaves registers / shared memory.
 #pragma once
 #include <cstdint>
 

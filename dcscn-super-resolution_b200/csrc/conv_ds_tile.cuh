@@ -1,7 +1,7 @@
 // Depthwise-separable layers, second generation (reference: helper/tf_graph.py:155-216; first generation and the full
 // statement of the op in conv_ds.cuh, kept as the cross-check `ds_impl = 1`).
 //
-// profiles/r1d_ds_ncu_summary.csv showed conv_ds.cuh instruction-issue bound (70-80 % issue active, DRAM 3-15 %): a
+// conv_ds.cuh is instruction-issue bound (a handful of FMAs per shared-memory load, DRAM mostly idle): a
 // warp walked 8 pixels serially for the depthwise pass (3 dependent global loads per pixel) and the pointwise GEMM left
 // half of the threads idle on layers with few output channels.  Here:
 //   * one CTA = a 16 x 16 pixel tile (3x3 layers) or 256 consecutive pixels (1x1 layers), ONE PIXEL PER THREAD;

@@ -1,4 +1,4 @@
-// Fused convolution epilogue shared by the tcgen05 kernel and the CUDA-core validation kernel:
+// Fused convolution epilogue shared by the tensor-core kernel and the CUDA-core validation kernel:
 //   acc * out_scale + bias  -> PReLU -> [inverted dropout] -> store
 // replacing the reference's un-fused  tf.add(bias) / PReLU / tf.nn.dropout / tf.concat /
 // tf.depth_to_space  ops (helper/tf_graph.py:109, :89-94, :130, :248; DCSCN.py:259,281).
@@ -31,24 +31,12 @@ __device__ __forceinline__ uint32_t pack_h2(__half a, __half b) {
   return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
 }
 
-// One 32-byte global store per lane (STG.256, sm_100): a lane's 16 fp16 channels of one plane in ONE instruction.  The
-// epilogue threads of a warp hold different pixels, 2816 bytes apart in the NHWC planes, so every lane of a store lands in
-// its own 128-byte line and the L1 spends one wavefront per (lane, instruction): with 16-byte stores the thin layers
-// (CNN6-12) were bound by exactly that - the epilogue warps 62-71 % of their time in the store phase while the issuing
-// thread waited for TMEM (profiles/r2c_issuer_epilogue_cycles.txt).  `dst` must be 32-byte aligned (16-channel slots).
-__device__ __forceinline__ void stg256(void* dst, const uint32_t (&w)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(dst), "r"(w[0]), "r"(w[1]), "r"(w[2]),
-               "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7])
-               : "memory");
-}
-__device__ __forceinline__ void store_words8(void* dst, const uint32_t (&w)[8], bool wide) {
-  if (wide) {
-    stg256(dst, w);
-  } else {                                   // store_mode 1: the two 16-byte stores of rounds 1-2c (A/B, cross-check)
-    uint4* q = reinterpret_cast<uint4*>(dst);
-    q[0] = make_uint4(w[0], w[1], w[2], w[3]);
-    q[1] = make_uint4(w[4], w[5], w[6], w[7]);
-  }
+// A lane's 16 fp16 channels of one plane as two 16-byte stores (sm_90 has no 32-byte global store).  `dst` must be
+// 16-byte aligned (16-channel slots).
+__device__ __forceinline__ void store_words8(void* dst, const uint32_t (&w)[8]) {
+  uint4* q = reinterpret_cast<uint4*>(dst);
+  q[0] = make_uint4(w[0], w[1], w[2], w[3]);
+  q[1] = make_uint4(w[4], w[5], w[6], w[7]);
 }
 
 // Two values at once: one packed conversion (cvt.rn.f16x2.f32 -> F2FP.PACK_AB) per plane instead of two scalar F2F, which
@@ -68,11 +56,11 @@ __device__ __forceinline__ void split_planes16(const float (&v)[16], uint32_t (&
   for (int i = 0; i < 8; ++i) split_f16x2(v[2 * i], v[2 * i + 1], ph[i], pl[i]);
 }
 
-__device__ __forceinline__ void store_planes16(__half* dst_hi, __half* dst_lo, size_t off, const float (&v)[16], bool wide = true) {
+__device__ __forceinline__ void store_planes16(__half* dst_hi, __half* dst_lo, size_t off, const float (&v)[16]) {
   uint32_t ph[8], pl[8];
   split_planes16(v, ph, pl);
-  store_words8(dst_hi + off, ph, wide);
-  if (dst_lo != nullptr) store_words8(dst_lo + off, pl, wide);
+  store_words8(dst_hi + off, ph);
+  if (dst_lo != nullptr) store_words8(dst_lo + off, pl);
 }
 
 // acc * out_scale + bias -> PReLU -> [inverted dropout] of 16 consecutive GEMM columns starting at `cg`; zn = fp16 pairs of
@@ -117,15 +105,14 @@ __device__ __forceinline__ void epilogue_store16(const EpiParams& e, const ConvG
   uint32_t zn[8];      // fp16 pairs of min(z, 0), only formed when a training segment asks for them
   const bool want_zneg = e.mode == EPI_PLANES && (e.seg[0].dst_zneg != nullptr || (e.num_seg > 1 && e.seg[1].dst_zneg != nullptr));
   epilogue_values16(e, g, n_total, img, y, x, cg, acc, v, zn, want_zneg);
-  const bool wide = e.store_mode != 1;
 
   if (e.mode == EPI_PLANES) {
 #pragma unroll
     for (int s = 0; s < kMaxSegments; ++s) {
       if (s < e.num_seg && cg >= e.seg[s].col_begin && cg < e.seg[s].col_end) {
         size_t off = ((size_t)((size_t)img * g.H + y) * g.W + x) * e.seg[s].pitch + (cg - e.seg[s].col_begin);
-        store_planes16(e.seg[s].dst_hi, e.seg[s].dst_lo, off, v, wide);
-        if (e.seg[s].dst_zneg != nullptr) store_words8(e.seg[s].dst_zneg + off, zn, wide);
+        store_planes16(e.seg[s].dst_hi, e.seg[s].dst_lo, off, v);
+        if (e.seg[s].dst_zneg != nullptr) store_words8(e.seg[s].dst_zneg + off, zn);
       }
     }
     return;
@@ -145,7 +132,7 @@ __device__ __forceinline__ void epilogue_store16(const EpiParams& e, const ConvG
 #pragma unroll
       for (int q = 0; q < 4; ++q) d[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
     } else {
-      store_planes16(e.seg[0].dst_hi, e.seg[0].dst_lo, pix * e.seg[0].pitch + c, v, wide);
+      store_planes16(e.seg[0].dst_hi, e.seg[0].dst_lo, pix * e.seg[0].pitch + c, v);
     }
   } else {
     // narrow pixel-shuffler outputs (c-DCSCN: pixel_shuffler_filters = 1): element-wise scatter

@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the sm_100a features the DCSCN kernels use:
-// mbarrier, TMA (cp.async.bulk[.tensor]), tcgen05 (alloc / mma / commit / ld / fences).
+// Thin inline-PTX wrappers for the sm_90a features the DCSCN kernels use:
+// mbarrier, TMA (cp.async.bulk[.tensor]), clusters, wgmma (mma_async / fence / commit_group / wait_group).
 #pragma once
 #include <cstdint>
 #include <cuda.h>
@@ -109,93 +109,153 @@ __device__ __forceinline__ void bulk_load_multicast(void* smem_dst, const void* 
       : "memory");
 }
 
-// ----------------------------------------------------------------- tcgen05 ----
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(cols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-// D[tmem] (+)= A[smem] * B[smem], kind::f16 (fp16/bf16 inputs, fp32 accumulate), one CTA.
-__device__ __forceinline__ void mma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                           uint32_t accumulate) {
+// Arrive on the mbarrier at the same shared-memory offset in CTA `cta` of this cluster (release at cluster scope).
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
   asm volatile(
       "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
+      ".reg .b32 remote;\n\t"
+      "mapa.shared::cluster.u32 remote, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [remote];\n\t"
+      "}\n" ::"r"(smem_u32(bar)),
+      "r"(cta)
       : "memory");
 }
 
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+// ------------------------------------------------------------------- wgmma ----
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-
-// Same arrival on the barrier at this offset in every CTA of `cta_mask`.
-__device__ __forceinline__ void mma_commit_multicast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes x 16 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+// Keeps the compiler from moving accumulator reads / writes across an asynchronous wgmma sequence.
+template <int R>
+__device__ __forceinline__ void reg_fence(float (&d)[R]) {
 #pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns (one instruction + wait).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+// Named barrier over `threads` threads (a warpgroup = 128); id 0 is __syncthreads.
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
-// TMEM -> registers: this warp's 32 lanes x 64 consecutive fp32 columns (one instruction + wait).
-__device__ __forceinline__ void tmem_ld64(uint32_t taddr, float (&v)[64]) {
-  uint32_t r[64];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x64.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, [%64];\n\t"
-      "tcgen05.wait::ld.sync.aligned;"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31]), "=r"(r[32]), "=r"(r[33]), "=r"(r[34]), "=r"(r[35]), "=r"(r[36]), "=r"(r[37]), "=r"(r[38]), "=r"(r[39]), "=r"(r[40]), "=r"(r[41]), "=r"(r[42]), "=r"(r[43]), "=r"(r[44]), "=r"(r[45]), "=r"(r[46]), "=r"(r[47]), "=r"(r[48]), "=r"(r[49]), "=r"(r[50]), "=r"(r[51]), "=r"(r[52]), "=r"(r[53]), "=r"(r[54]), "=r"(r[55]), "=r"(r[56]), "=r"(r[57]), "=r"(r[58]), "=r"(r[59]), "=r"(r[60]), "=r"(r[61]), "=r"(r[62]), "=r"(r[63])
-      : "r"(taddr)
-      : "memory");
-#pragma unroll
-  for (int i = 0; i < 64; ++i) v[i] = __uint_as_float(r[i]);
+// wgmma.mma_async m64nNk16, fp16 x fp16 -> fp32, both operands from shared-memory descriptors.  N is part of the
+// opcode, so every width the kernels use has its own wrapper; d holds the N / 2 accumulator registers of this thread.
+// TA / TB = 1: the operand is MN-major (transposed) instead of K-major.
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wgmma_f16(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d);
+#define DCSCN_WGMMA_N16(TA, TB)                                                                                      \
+  template <>                                                                                                           \
+  __device__ __forceinline__ void wgmma_f16<16, TA, TB>(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) { \
+    asm volatile(                                                                                                       \
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"                                                                   \
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, " #TA ", " #TB ";\n\t}\n"                  \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])                                                                                                            \
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d));                                                                      \
+  }
+DCSCN_WGMMA_N16(0, 0)
+DCSCN_WGMMA_N16(1, 1)
+#undef DCSCN_WGMMA_N16
+#define DCSCN_WGMMA_N32(TA, TB)                                                                                      \
+  template <>                                                                                                           \
+  __device__ __forceinline__ void wgmma_f16<32, TA, TB>(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) { \
+    asm volatile(                                                                                                       \
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"                                                                   \
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, " #TA ", " #TB ";\n\t}\n"                  \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])                                                                                                            \
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d));                                                                      \
+  }
+DCSCN_WGMMA_N32(0, 0)
+DCSCN_WGMMA_N32(1, 1)
+#undef DCSCN_WGMMA_N32
+#define DCSCN_WGMMA_N48(TA, TB)                                                                                      \
+  template <>                                                                                                           \
+  __device__ __forceinline__ void wgmma_f16<48, TA, TB>(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) { \
+    asm volatile(                                                                                                       \
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"                                                                   \
+        "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, " #TA ", " #TB ";\n\t}\n"                  \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])                                                                                                            \
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d));                                                                      \
+  }
+DCSCN_WGMMA_N48(0, 0)
+DCSCN_WGMMA_N48(1, 1)
+#undef DCSCN_WGMMA_N48
+#define DCSCN_WGMMA_N64(TA, TB)                                                                                      \
+  template <>                                                                                                           \
+  __device__ __forceinline__ void wgmma_f16<64, TA, TB>(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) { \
+    asm volatile(                                                                                                       \
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"                                                                   \
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, " #TA ", " #TB ";\n\t}\n"                  \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])                                                                                                            \
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d));                                                                      \
+  }
+DCSCN_WGMMA_N64(0, 0)
+DCSCN_WGMMA_N64(1, 1)
+#undef DCSCN_WGMMA_N64
+#define DCSCN_WGMMA_N80(TA, TB)                                                                                      \
+  template <>                                                                                                           \
+  __device__ __forceinline__ void wgmma_f16<80, TA, TB>(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) { \
+    asm volatile(                                                                                                       \
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"                                                                   \
+        "wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1, " #TA ", " #TB ";\n\t}\n"                  \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])                                                                                                            \
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d));                                                                      \
+  }
+DCSCN_WGMMA_N80(0, 0)
+DCSCN_WGMMA_N80(1, 1)
+#undef DCSCN_WGMMA_N80
+#define DCSCN_WGMMA_N96(TA, TB)                                                                                      \
+  template <>                                                                                                           \
+  __device__ __forceinline__ void wgmma_f16<96, TA, TB>(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) { \
+    asm volatile(                                                                                                       \
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"                                                                   \
+        "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, " #TA ", " #TB ";\n\t}\n"                  \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])                                                                                                            \
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d));                                                                      \
+  }
+DCSCN_WGMMA_N96(0, 0)
+DCSCN_WGMMA_N96(1, 1)
+#undef DCSCN_WGMMA_N96
+#define DCSCN_WGMMA_N112(TA, TB)                                                                                      \
+  template <>                                                                                                           \
+  __device__ __forceinline__ void wgmma_f16<112, TA, TB>(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) { \
+    asm volatile(                                                                                                       \
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %58, 0;\n\t"                                                                   \
+        "wgmma.mma_async.sync.aligned.m64n112k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55}, %56, %57, p, 1, 1, " #TA ", " #TB ";\n\t}\n"                  \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55])                                                                                                            \
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d));                                                                      \
+  }
+DCSCN_WGMMA_N112(0, 0)
+DCSCN_WGMMA_N112(1, 1)
+#undef DCSCN_WGMMA_N112
+#define DCSCN_WGMMA_N128(TA, TB)                                                                                      \
+  template <>                                                                                                           \
+  __device__ __forceinline__ void wgmma_f16<128, TA, TB>(float* d, uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) { \
+    asm volatile(                                                                                                       \
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"                                                                   \
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, " #TA ", " #TB ";\n\t}\n"                  \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])                                                                                                            \
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d));                                                                      \
+  }
+DCSCN_WGMMA_N128(0, 0)
+DCSCN_WGMMA_N128(1, 1)
+#undef DCSCN_WGMMA_N128
+
+// Width chosen at run time (uniform branch per instruction): one accumulator array of 64 registers serves every
+// column tile width of the kernels (n <= 128, multiple of 16); registers past n / 2 are left untouched.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_f16_n(int n, float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+  switch (n) {
+    case 16: wgmma_f16<16, TA, TB>(d, desc_a, desc_b, scale_d); break;
+    case 32: wgmma_f16<32, TA, TB>(d, desc_a, desc_b, scale_d); break;
+    case 48: wgmma_f16<48, TA, TB>(d, desc_a, desc_b, scale_d); break;
+    case 64: wgmma_f16<64, TA, TB>(d, desc_a, desc_b, scale_d); break;
+    case 80: wgmma_f16<80, TA, TB>(d, desc_a, desc_b, scale_d); break;
+    case 96: wgmma_f16<96, TA, TB>(d, desc_a, desc_b, scale_d); break;
+    case 112: wgmma_f16<112, TA, TB>(d, desc_a, desc_b, scale_d); break;
+    default: wgmma_f16<128, TA, TB>(d, desc_a, desc_b, scale_d); break;
+  }
 }
 
 }  // namespace ptx

@@ -3,9 +3,9 @@
 // mse + l2_decay * sum(l2_loss(W)), tf.clip_by_global_norm, tf.train.AdamOptimizer).
 //
 // Split of the work:
-//   * data gradients (dgrad) of every 3x3 / 1x1 layer run on the SAME tcgen05 implicit-GEMM kernels as the forward
+//   * data gradients (dgrad) of every 3x3 / 1x1 layer run on the SAME wgmma implicit-GEMM kernels as the forward
 //     pass (conv_tc*.cuh) with the filters transposed and spatially flipped - no extra MMA code;
-//   * filter gradients (wgrad) of those layers run on tcgen05 too, with MN-major operands read straight from the NHWC
+//   * filter gradients (wgrad) of those layers run on wgmma too, with MN-major operands read straight from the NHWC
 //     planes (wgrad_tc.cuh); `wgrad_kernel` below is the CUDA-core version kept as the cross-check (option wgrad_impl);
 //   * everything else is in this file, on CUDA cores, laid out so a warp touches whole 128-byte lines: loss / output
 //     gradient, R-CNN1 forward / backward fused with the depth_to_space gradient (= space_to_depth), CNN1's filter
@@ -808,7 +808,7 @@ __global__ void __launch_bounds__(256) adam_kernel(const AdamParams p) {
 
 
 // ---- device-side refresh of the packed operand images after an optimizer step -------------------------------------
-// dst = CTA-pair operand image (hi plane block, then lo plane block, per [n_tile][tap][chunk][rank]); map[i] = flat
+// dst = operand image (hi plane block, then lo plane block, per [n_tile][tap][chunk]); map[i] = flat
 // index into the fp32 master weights behind hi-plane element i (-1 = structural zero).  Also records max |w * scale|
 // so the host can tell when the power-of-two scale has to be re-chosen.
 struct RepackParams {
@@ -816,12 +816,12 @@ struct RepackParams {
   const int* map;
   __half* dst;
   unsigned long long n;
-  int half_elems;
+  int half_elems;     // elements of one plane block
   float wscale;
   unsigned* wmax;     // float bits (values are non-negative, so unsigned order == float order)
 };
 
-__global__ void __launch_bounds__(256) repack_pair_kernel(const RepackParams p) {
+__global__ void __launch_bounds__(256) repack_kernel(const RepackParams p) {
   float m = 0.f;
   for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < p.n;
        i += (unsigned long long)gridDim.x * blockDim.x) {

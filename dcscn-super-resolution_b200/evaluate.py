@@ -25,7 +25,7 @@ FLAGS = args.get()
 
 def build_model():
     if FLAGS.frozenInference:
-        raise NotImplementedError("--frozenInference loads a TensorFlow GraphDef; not supported by the B200 engine")
+        raise NotImplementedError("--frozenInference loads a TensorFlow GraphDef; not supported by the H100 engine")
     # under torchrun / --gpus=N the flips of the self-ensemble are shared out over one process per GPU (DCSCN.do)
     DCSCN.init_distributed(FLAGS)
     return DCSCN.create(FLAGS)

@@ -219,7 +219,7 @@ for _name, _default, _help in _REFERENCE_FLAGS:
 
 def get(argv=None):
     print("Python Interpreter version:%s" % sys.version[:3])
-    print("engine: dcscn_b200 (sm_100a CUDA, no TensorFlow)")
+    print("engine: dcscn_b200 (sm_90a CUDA, no TensorFlow)")
     print("numpy version:%s" % np.__version__)
     if not FLAGS._parsed:
         FLAGS.parse(sys.argv if argv is None else argv)

@@ -4,7 +4,7 @@ ctypes binding of the C-ABI in include/dcscn_b200.h (libdcscn_b200.so, built fro
 This is what stands where `self.sess.run(...)` stood in the reference
 (DCSCN.py:420, :565, :575): PyTorch tensors are only the device containers whose
 raw pointers are handed to the library.  There is NO CPU fallback: if the shared
-library is missing or no B200 is present, construction raises.
+library is missing or no H100 is present, construction raises.
 """
 
 import ctypes
@@ -55,7 +55,7 @@ EXPORTED_SYMBOLS = [
     "dcscn_set_option", "dcscn_get_timings", "dcscn_launch_count", "dcscn_device_bytes",
     "dcscn_train_step", "dcscn_train_step_host", "dcscn_get_grad", "dcscn_get_adam_slot", "dcscn_set_adam_slot", "dcscn_get_adam_step",
     "dcscn_set_adam_step", "dcscn_last_grad_norm",
-    "dcscn_patch_store_set", "dcscn_train_step_indexed", "dcscn_patch_gather", "dcscn_dropout_mask", "dcscn_grad_buffer", "dcscn_apply_gradients", "dcscn_apply_gradients_avg", "dcscn_reset_optimizer", "dcscn_umma_probe", "dcscn_graph_replays",
+    "dcscn_patch_store_set", "dcscn_train_step_indexed", "dcscn_patch_gather", "dcscn_dropout_mask", "dcscn_grad_buffer", "dcscn_apply_gradients", "dcscn_apply_gradients_avg", "dcscn_reset_optimizer", "dcscn_graph_replays",
 ]
 
 _lib = None
@@ -118,9 +118,6 @@ def load_library(path=None):
     lib.dcscn_device_bytes.restype = c64
     lib.dcscn_graph_replays.argtypes = [vp]
     lib.dcscn_graph_replays.restype = c64
-    lib.dcscn_umma_probe.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                     ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_double)]
-    lib.dcscn_umma_probe.restype = ctypes.c_int
     _lib = lib
     return lib
 

@@ -1,5 +1,5 @@
 """
-Super-resolve one image file: the reference's `sr.py` command line on the B200 engine.
+Super-resolve one image file: the reference's `sr.py` command line on the H100 engine.
 
   python sr.py --file=your_file.png [--scale=3 --layers=8 --filters=96 ...]
 

@@ -1,5 +1,5 @@
 /*
- * dcscn_b200.h - C-ABI of the B200-native DCSCN forward / backward hot path.
+ * dcscn_b200.h - C-ABI of the H100-native (sm_90a) DCSCN forward / backward hot path.
  *
  * The reference (jiny2001/dcscn-super-resolution) has no FFI: its seam is the Python class
  * DCSCN.SuperResolution and the four `sess.run` call sites.  Each entry point below names the
@@ -23,7 +23,7 @@ typedef struct dcscn_handle dcscn_handle;
 
 /* Arithmetic of the tensor-core layers. */
 enum {
-  DCSCN_PRECISION_F16X3 = 0, /* fp32-equivalent: fp16 hi/lo split operands, 3 UMMA passes, fp32 accumulate */
+  DCSCN_PRECISION_F16X3 = 0, /* fp32-equivalent: fp16 hi/lo split operands, 3 wgmma passes, fp32 accumulate */
   DCSCN_PRECISION_F16X1 = 1  /* single-pass fp16 operands (PSNR-neutral, not 1e-3-pixel exact) */
 };
 
@@ -164,21 +164,12 @@ int dcscn_dropout_mask(dcscn_handle* h, const char* tensor, uint32_t seed, int n
  */
 int dcscn_get_activation(dcscn_handle* h, const char* tensor, float* host_data, int64_t numel);
 
-/* Options: "conv_impl" 0 = tcgen05 (default), 1 = CUDA-core fp32 validation kernels;
+/* Options: "conv_impl" 0 = wgmma tensor cores (default), 1 = CUDA-core fp32 validation kernels;
  *          "kc" 64 | 32 = K-chunk (channels per pipeline stage) of the tensor-core kernel;
  *          "seg_chunks" = pipeline stages per fp32-promotion segment (default 0 = automatic: 2, or 3 for thin layers);
- *          "halo" 0 | 1 | 2 | 3 = 3x3 layers: one A tile per tap (0), three 18x8 boxes per channel chunk (1), one
- *                     18x10 box per channel chunk serving all nine taps with two-pass segments (2), or the same box with
- *                     streaming weight stages and split correction / dominant accumulators (3, default);
- *          "pair" 1 | 0 = CTA-pair kernel (tcgen05 cta_group::2, weight tiles split across two SMs; default 1);
- *          "cluster" 1 | 2 | 4 = CTAs per cluster multicasting weight tiles in the single-CTA kernel (default 1);
+ *          "cluster" 1 | 2 | 4 = CTAs per cluster multicasting weight tiles in the tensor-core kernel (default 1);
  *          "fuse_last" 1 | 0 = compute the per-pixel half of R-CNN1 inside the last Up-PS epilogue (default 1);
  *          "timing" 0 | 1 = record per-launch CUDA events (see dcscn_get_timings);
- *          "store_mode" 2 | 0 | 1 = fp16 plane stores of the tensor-core epilogues: 32-byte stores with neighbouring lanes
- *          exchanging halves so that each instruction writes 64 contiguous bytes of a pixel (default; streaming 3x3 kernel,
- *          elsewhere like 0), one 32-byte store per lane and plane, or two 16-byte stores (the round-1/2 form, cross-check);
- *          "wide_tiles" 1 | 0 = column tiles of the streaming 3x3 kernel capped at 256 (default: layers wider than 160
- *          columns use two TMEM buffers and read each input box once per pixel tile) or at 160 (three buffers);
  *          "ds_impl" 0 | 1 = depthwise-separable layers on the tile kernels (default) or the first-generation kernels (cross-check);
  *          "act_grad_impl" 0 | 1 = activation gradients with 16-byte (default) or channel-pair accesses (cross-check);
  *          "ds_cache" 1 | 0 = depthwise-separable pixel-shuffler layers keep their depthwise values across column groups;
@@ -187,8 +178,8 @@ int dcscn_get_activation(dcscn_handle* h, const char* tensor, float* host_data, 
  *          the same input pointer has been seen twice in a row (default 1; off while "timing" = 1 or "conv_impl" = 1);
  *          "l1_loss" 0 | 1 = image_loss of the train step is mean |y_ - y| instead of the MSE (--use_l1_loss,
  *          DCSCN.py:342-344; the returned mse stays the MSE);
- *          "wgrad_impl" 0 | 1 = filter gradients on tcgen05 (default) or on CUDA cores (cross-check);
- *          "wgrad_taps" 0..3 = filter taps per wgrad CTA (0 = automatic);
+ *          "wgrad_impl" 0 | 1 = filter gradients on wgmma tensor cores (default) or on CUDA cores (cross-check);
+ *          "wgrad_taps" 0..2 = filter taps per wgrad CTA (0 = automatic);
  *          "host_repack" 0 | 1 = after an optimizer step rebuild the packed tensor-core weight images on the host
  *          (validation of the default device-side refresh). */
 int dcscn_set_option(dcscn_handle* h, const char* key, int64_t value);
@@ -201,12 +192,6 @@ int64_t dcscn_launch_count(dcscn_handle* h);
 int64_t dcscn_graph_replays(dcscn_handle* h);
 /* Bytes of device memory currently held by the handle. */
 int64_t dcscn_device_bytes(dcscn_handle* h);
-/* Measurement only (no reference counterpart; bench.py's roofline denominator): kind::f16 tcgen05.mma throughput with
- * both operands resident in shared memory, every SM busy.  group = 1 | 2 (cta_group), n = accumulator width of one
- * product (multiple of 16), mode 0 = the three hi/lo products of the conv kernels per K = 16 slice, 1 = the stacked
- * form (one UMMA of width 2n + one of width n; group 1, n <= 128), 2 = a single product; iters x 4 slices are issued by
- * each cluster.  Returns the launch duration (ms, CUDA events) and the longest issuing-thread span (SM cycles). */
-int dcscn_umma_probe(int device_id, int group, int n, int mode, int iters, float* out_ms, double* out_cycles);
 
 #ifdef __cplusplus
 }

@@ -126,7 +126,7 @@ def test_device_refresh_equals_host_repack(kw):
 
 
 def test_tensor_core_wgrad_matches_cuda_core_wgrad_full_model():
-    """Filter gradients of the full L12 x2 model (196..48 filters, 1301-channel concat, 384-column Up-PS): the tcgen05
+    """Filter gradients of the full L12 x2 model (196..48 filters, 1301-channel concat, 384-column Up-PS): the wgmma
     wgrad (transposed zero-bordered operands, K-split partial sums) against the straightforward CUDA-core kernel on the
     same planes.  Both accumulate in fp32; 1e-4 of each tensor's max covers the different summation orders."""
     from helper import engine as E, tf_bundle

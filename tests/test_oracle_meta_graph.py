@@ -78,16 +78,18 @@ def test_oracle_equals_the_shipped_graph_executed_op_by_op(model):
     assert set(g.nodes[g.root]["input"]) == {"R-CNN1/R-CNN1_conv", "x2"}
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/models"), reason="reference checkout not present (GPU box)")
 @pytest.mark.parametrize("model", META_MODELS)
 def test_fixture_is_what_the_reference_ships(model, tmp_path):
-    """Where the reference is mounted, re-extract the sub-graph from its .meta and require the committed fixture."""
+    """Re-extract the sub-graph from the reference's own .meta (stored xz-compressed beside the fixture, byte for byte
+    the file the reference ships) and require the committed fixture."""
     import importlib.util
     import json
+    import lzma
     spec = importlib.util.spec_from_file_location("make_meta_fixture", os.path.join(ROOT, "scripts", "make_meta_fixture.py"))
     mod = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(mod)
-    nodes, _ = mod.graph_nodes(open("/root/reference/models/%s.ckpt.meta" % model, "rb").read())
+    meta = lzma.decompress(open(os.path.join(GOLDEN, "meta", "%s.ckpt.meta.xz" % model), "rb").read())
+    nodes, _ = mod.graph_nodes(meta)
     root, keep = mod.forward_subgraph(nodes)
     doc = json.load(open(_fixture(model)))
     assert doc["root"] == root and doc["nodes"] == json.loads(json.dumps(keep))
