@@ -3,22 +3,33 @@
 // Replaces  tf.nn.conv2d(SAME, stride 1, NHWC, HWIO) + bias + PReLU  of the reference
 // (helper/tf_graph.py:104-153 conv2d / build_conv; :238-249 build_pixel_shuffler_layer).
 //
-// GEMM view:  D[M = 128 pixels (TH x TW patch), N = cout (padded to 16, <= 128 per column tile)]
-//             = sum over taps (ky,kx) and input-channel chunks of  A_tap[128 x KC] * W_tap[KC x N]
-//   * A tiles are fetched by TMA (4-D tiled tensor map over the NHWC fp16 plane, box {KC, TW, TH, 1});
-//     the box origin is shifted by the tap offset and TMA zero-fills out-of-image pixels, which IS
-//     TF's SAME padding - no halo handling in the kernel.
+// GEMM view:  D[M = 128 pixels (TH x TW patch), N = cout (padded to 16, <= 112 per column tile)]
+//             = sum over input-channel chunks, taps (kx, ky) of  A_tap[128 x KC] * W_tap[KC x N]
+//   * A tiles are fetched by TMA (4-D tiled tensor map over the NHWC fp16 plane).  A k x k layer (k = 3 or 5) loads ONE
+//     box of TW x (TH + k - 1) pixels per (chunk, kx), its origin shifted by (kx - k / 2, -k / 2); the k ky taps read it
+//     at row offsets 0, TW, ..., (k - 1) TW.  The host only picks patches with TW a multiple of 8, so every offset is a
+//     whole number of 8-row swizzle atoms and the operand descriptors stay valid.  TMA zero-fills out-of-image pixels, which IS TF's SAME padding - no halo handling in
+//     the kernel.  A 1x1 layer loads one TW x TH box per chunk.
 //   * fp32-equivalent precision from fp16 tensor cores:  a = a_hi + a_lo,  w*2^s = w_hi + w_lo
 //     (each 11-bit significands), D += a_hi*w_hi + a_lo*w_hi + a_hi*w_lo   (3 x m64nNk16 wgmma per 16 channels,
 //     fp32 accumulation in registers).  NPLANES == 1 is the single-pass fp16 "fast" mode.
 //   * The tensor core's fp32 accumulator update truncates (round-toward-zero), a bias that grows linearly with the
-//     number of accumulation steps.  K is therefore cut into short segments (`seg_chunks` pipeline stages): each
-//     segment accumulates from zero, and the sum is added into a second set of fp32 registers with round-to-nearest
-//     ("promotion").  `seg_chunks` == 1 (the strict setting) promotes after every 16-channel K slice.  Accumulator + running sum take N registers per thread, which is what caps a column tile at 128.
-//   * Weight tiles are the dominant L2->SM traffic (every 128-pixel tile streams the whole layer's weights).  CTAs
-//     are launched in clusters of `cs` (1, 2 or 4) that walk pixel tiles in lockstep; each CTA fetches 1/cs of
+//     number of accumulation steps.  K is therefore cut into short segments (`seg_chunks` weight tiles): each segment
+//     accumulates the two correction products in `corr` and the dominant a_hi*w_hi product in `dom`, both from zero,
+//     and at its end both are added into the running fp32 `sum` with round-to-nearest ("promotion").  Only `dom`
+//     grows large, so only the dominant chain contributes truncation error.  `seg_chunks` == 1 (the strict setting)
+//     promotes after every 16-channel K slice.  The three register sets take 3 N / 2 floats per thread, which is what
+//     caps a column tile at 112 (kMaxTileN).
+//   * The column-tile width N is a template parameter: the wgmma width is an immediate of the instruction, and a
+//     straight-line run of same-width wgmma needs no per-instruction selection.
+//   * Two shared-memory rings with their own full/empty mbarriers: activation slots (one per (chunk, kx)) and weight
+//     tiles (one per (tap, chunk), read from the packed image [n_tile][tap][chunk]).  The consumers commit one wgmma
+//     group per weight tile and release a slot as soon as `wgmma.wait_group 1` shows the group that last read it
+//     has completed, so both rings work purely as prefetch depth.
+//   * Weight tiles are a large share of the L2->SM traffic (every 128-pixel tile streams the whole layer's weights).
+//     CTAs are launched in clusters of `cs` (1, 2 or 4) that walk pixel tiles in lockstep; each CTA fetches 1/cs of
 //     every weight tile and multicasts it to the whole cluster (cp.async.bulk ... .multicast::cluster), and each
-//     consumer warpgroup releases a pipeline stage in all cluster members (remote mbarrier arrive).
+//     consumer warpgroup releases a weight slot in all cluster members (remote mbarrier arrive).
 //   * Warp roles: warpgroup 0 = producer (warp 0 issues TMA), warpgroups 1 and 2 = consumers, one per 64-pixel half
 //     of the tile: they issue the wgmma of their rows, promote, and run the epilogue (bias/PReLU/split -> global) after
 //     an exchange through shared memory that gives every thread one pixel and a run of 16-column chunks.  Persistent
@@ -33,8 +44,11 @@ namespace dcscn {
 constexpr int kConsumerWGs = 2;                    // one per 64-pixel half of the 128-pixel tile
 constexpr int kTcThreads = (1 + kConsumerWGs) * 128;
 constexpr int kRegsIssue = 40, kRegsEpilogue = 232;  // setmaxnreg budgets (128*40 + 256*232 <= 64K)
-constexpr int kMaxStages = 12;
-constexpr int kMaxTileN = 128;                     // column tile cap: accumulator + promoted sum = n_pad registers
+constexpr int kMaxASlots = 4;                      // activation ring slots
+constexpr int kMaxWSlots = 12;                     // weight ring slots
+constexpr int kTcBarrierBytes = 2 * (kMaxASlots + kMaxWSlots) * 8;
+constexpr int kMaxTileN = 112;                     // column tile cap: corr + dom + promoted sum = 3 N / 2 registers;
+                                                   // at N = 128 (192 of them) ptxas spills inside the K loop
 constexpr int kRdotSmemBytes = 9 * 128 * 4;         // fused R-CNN1 filter taps (d2s_cout <= 128) staged in shared memory
 constexpr int kColSplit = 2;                       // epilogue threads per pixel, each owning a contiguous run of chunks
 constexpr int kXchgStride = 36;                    // floats per pixel row of the epilogue exchange buffer (2 chunks + pad)
@@ -43,7 +57,6 @@ constexpr int kXchgBytes = kConsumerWGs * 64 * kXchgStride * 4;
 template <int KC>
 struct TcSmem {
   static constexpr int kRowBytes = KC * 2;                  // 128 (SWIZZLE_128B) or 64 (SWIZZLE_64B)
-  static constexpr int kABytes = kTileM * kRowBytes;        // one A plane tile
   static constexpr int kSbo = 8 * kRowBytes;                // 8-row core-matrix group stride
   static constexpr uint64_t kLayout = (KC == 64) ? 1ull : 2ull;  // wgmma descriptor layout type: SW128 = 1, SW64 = 2
 };
@@ -56,23 +69,56 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
          (TcSmem<KC>::kLayout << 62);
 }
 
-__host__ __device__ inline size_t tc_stage_bytes(int KC, int nplanes, int n_pad) {
-  return (size_t)nplanes * ((size_t)kTileM * KC * 2 + (size_t)n_pad * KC * 2);
+// Bytes of one activation plane in a ring slot: the TMA box of TW x (TH + ksz - 1) pixels, rounded up to 1024 bytes
+// so that every slot and plane starts on a swizzle-atom boundary.
+__host__ __device__ inline uint32_t tc_a_plane_bytes(int KC, int TW, int TH, int ksz) {
+  return ((uint32_t)TW * (uint32_t)(TH + ksz - 1) * (uint32_t)KC * 2u + 1023u) & ~1023u;
+}
+__host__ __device__ inline uint32_t tc_w_tile_bytes(int KC, int nplanes, int n_pad) {
+  return (uint32_t)nplanes * (uint32_t)n_pad * (uint32_t)KC * 2u;
 }
 
-template <int KC, int NPLANES>
+// One wgmma batch: the products of KS consecutive 16-channel K slices of a weight tile, committed as one group.
+// corr += a_lo*w_hi + a_hi*w_lo, dom += a_hi*w_hi; acc_on == 0 starts both from zero.
+template <int N, int NPLANES, int KS>
+__device__ __forceinline__ void tile_products(float (&corr)[N / 2], float (&dom)[N / 2], uint64_t a_hi, uint64_t a_lo,
+                                              uint64_t b_hi, uint64_t b_lo, uint32_t acc_on) {
+  ptx::wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) {
+    const uint64_t kadd = (uint64_t)ks * 2u;   // 32 bytes (16 fp16 along K) in 16-byte descriptor units
+    const uint32_t on = ks == 0 ? acc_on : 1u;
+    if (NPLANES == 2) {
+      ptx::wgmma_f16<N, 0, 0>(corr, a_lo + kadd, b_hi + kadd, on);
+      ptx::wgmma_f16<N, 0, 0>(corr, a_hi + kadd, b_lo + kadd, 1u);
+    }
+    ptx::wgmma_f16<N, 0, 0>(dom, a_hi + kadd, b_hi + kadd, on);
+  }
+  ptx::wgmma_commit();
+}
+
+template <int KC, int NPLANES, int N>
 __global__ void __launch_bounds__(kTcThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo,
-               const ConvTCParams p, const int num_stages) {
+               const ConvTCParams p, const int a_slots, const int w_slots) {
+  static_assert(N % 16 == 0 && N >= 16 && N <= kMaxTileN, "column tile width");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [stages x (A_hi, A_lo, B_hi, B_lo)] then barriers, R-CNN1 taps, epilogue exchange
+  // carve: [a_slots x (A_hi, A_lo)] [w_slots x (W_hi, W_lo)] then barriers, R-CNN1 taps, epilogue exchange
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  constexpr int A_BYTES = TcSmem<KC>::kABytes;
-  const int B_BYTES = p.n_pad * KC * 2;
-  const int STAGE_BYTES = NPLANES * (A_BYTES + B_BYTES);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)num_stages * STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + kMaxStages;
-  float* s_rdot = reinterpret_cast<float*>(empty_bar + kMaxStages);   // 16-byte aligned (barriers start 1024-aligned)
+  const ConvGeom& g = p.g;
+  const int ksz = p.ksz;
+  const uint32_t A_PLANE = tc_a_plane_bytes(KC, g.TW, g.TH, ksz);
+  const uint32_t A_SLOT = NPLANES * A_PLANE;
+  const uint32_t A_TX = (uint32_t)NPLANES * (uint32_t)g.TW * (uint32_t)(g.TH + ksz - 1) * KC * 2u;  // bytes TMA delivers
+  constexpr uint32_t B_BYTES = N * KC * 2;
+  constexpr uint32_t W_TILE = NPLANES * B_BYTES;
+  uint8_t* a_ring = smem;
+  uint8_t* w_ring = smem + (size_t)a_slots * A_SLOT;
+  uint64_t* a_full = reinterpret_cast<uint64_t*>(w_ring + (size_t)w_slots * W_TILE);
+  uint64_t* a_empty = a_full + kMaxASlots;
+  uint64_t* w_full = a_empty + kMaxASlots;
+  uint64_t* w_empty = w_full + kMaxWSlots;
+  float* s_rdot = reinterpret_cast<float*>(w_empty + kMaxWSlots);   // 16-byte aligned (barriers start 1024-aligned)
   float* s_xchg = s_rdot + kRdotSmemBytes / 4;
 
   const int wg = threadIdx.x >> 7;
@@ -82,9 +128,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
   const uint16_t cta_mask = (uint16_t)((1u << cs) - 1u);
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < num_stages; ++s) {
-      ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], kConsumerWGs * cs);   // one arrival per consumer warpgroup of every cluster CTA
+    for (int s = 0; s < a_slots; ++s) {
+      ptx::mbar_init(&a_full[s], 1);
+      ptx::mbar_init(&a_empty[s], kConsumerWGs);        // activations are this CTA's own
+    }
+    for (int s = 0; s < w_slots; ++s) {
+      ptx::mbar_init(&w_full[s], 1);
+      ptx::mbar_init(&w_empty[s], kConsumerWGs * cs);   // one arrival per consumer warpgroup of every cluster CTA
     }
     ptx::fence_barrier_init();
     ptx::fence_proxy_async();
@@ -94,16 +144,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
   __syncthreads();
   if (cs > 1) ptx::cluster_sync();               // peers' barriers are initialised before anything targets them
 
-  const ConvGeom& g = p.g;
   const int tiles_per_img = g.tiles_x * g.tiles_y;
   const int num_tiles = g.n_img * tiles_per_img;
   const int groups = (num_tiles + cs - 1) / cs;  // cs pixel tiles are processed by one cluster iteration
   const int num_items = groups * p.n_tiles;
   const int cluster_id = blockIdx.x / cs;
   const int num_clusters = gridDim.x / cs;
-  const int taps = p.ksz * p.ksz;
-  const int half = p.ksz >> 1;
-  const int total_chunks = taps * p.chunks;
+  const int half = ksz >> 1;
+  const int chunks = p.chunks;
 
   if (wg == 0) {
     ptx::setmaxnreg_dec<kRegsIssue>();
@@ -111,11 +159,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
     if (threadIdx.x == 0) {
       ptx::prefetch_tensormap(&tm_hi);
       if (NPLANES == 2) ptx::prefetch_tensormap(&tm_lo);
-      const int slice_rows = p.n_pad / cs;                       // this CTA's share of every weight tile
-      const uint32_t slice_bytes = (uint32_t)(slice_rows * KC * 2);
+      constexpr uint32_t slice_full = B_BYTES;
+      const uint32_t slice_bytes = slice_full / (uint32_t)cs;     // this CTA's share of every weight plane
       const uint32_t slice_off = rank * slice_bytes;
-      int stage = 0;
-      uint32_t phase = 0;
+      int as = 0, ws = 0;
+      uint32_t a_ph = 0, w_ph = 0;
       for (int item = cluster_id; item < num_items; item += num_clusters) {
         const int n_tile = item % p.n_tiles;
         int tile = (item / p.n_tiles) * cs + (int)rank;
@@ -123,28 +171,31 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
         const int img = tile / tiles_per_img;
         const int t2 = tile - img * tiles_per_img;
         const int ty = t2 / g.tiles_x, tx = t2 - ty * g.tiles_x;
-        const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.wpack) +
-                              (size_t)n_tile * total_chunks * (size_t)(NPLANES * B_BYTES);
-        for (int tap = 0; tap < taps; ++tap) {
-          const int dy = tap / p.ksz - half, dx = tap % p.ksz - half;
-          for (int ch = 0; ch < p.chunks; ++ch) {
-            ptx::mbar_wait(&empty_bar[stage], phase ^ 1);
-            uint8_t* st = smem + (size_t)stage * STAGE_BYTES;
-            ptx::mbar_arrive_expect_tx(&full_bar[stage], (uint32_t)STAGE_BYTES);
-            ptx::tma_load_4d(st, &tm_hi, &full_bar[stage], ch * KC, tx * g.TW + dx, ty * g.TH + dy, img);
-            if (NPLANES == 2)
-              ptx::tma_load_4d(st + A_BYTES, &tm_lo, &full_bar[stage], ch * KC, tx * g.TW + dx, ty * g.TH + dy, img);
-            const uint8_t* wtile = wsrc + (size_t)(tap * p.chunks + ch) * (NPLANES * B_BYTES);
-            uint8_t* bdst = st + NPLANES * A_BYTES;
-            if (cs == 1) {
-              ptx::bulk_load(bdst, wtile, (uint32_t)(NPLANES * B_BYTES), &full_bar[stage]);
-            } else {
+        const int x0 = tx * g.TW - half, y0 = ty * g.TH - half;
+        const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.wpack) + (size_t)n_tile * ksz * ksz * chunks * W_TILE;
+        for (int ch = 0; ch < chunks; ++ch) {
+          for (int dx = 0; dx < ksz; ++dx) {
+            ptx::mbar_wait(&a_empty[as], a_ph ^ 1);
+            uint8_t* ad = a_ring + (size_t)as * A_SLOT;
+            ptx::mbar_arrive_expect_tx(&a_full[as], A_TX);
+            ptx::tma_load_4d(ad, &tm_hi, &a_full[as], ch * KC, x0 + dx, y0, img);
+            if (NPLANES == 2) ptx::tma_load_4d(ad + A_PLANE, &tm_lo, &a_full[as], ch * KC, x0 + dx, y0, img);
+            if (++as == a_slots) { as = 0; a_ph ^= 1; }
+            for (int dy = 0; dy < ksz; ++dy) {
+              ptx::mbar_wait(&w_empty[ws], w_ph ^ 1);
+              uint8_t* wd = w_ring + (size_t)ws * W_TILE;
+              ptx::mbar_arrive_expect_tx(&w_full[ws], W_TILE);
+              const uint8_t* wtile = wsrc + (size_t)((dy * ksz + dx) * chunks + ch) * W_TILE;
+              if (cs == 1) {
+                ptx::bulk_load(wd, wtile, W_TILE, &w_full[ws]);
+              } else {
 #pragma unroll
-              for (int pl = 0; pl < NPLANES; ++pl)
-                ptx::bulk_load_multicast(bdst + pl * B_BYTES + slice_off, wtile + (size_t)pl * B_BYTES + slice_off,
-                                         slice_bytes, &full_bar[stage], cta_mask);
+                for (int pl = 0; pl < NPLANES; ++pl)
+                  ptx::bulk_load_multicast(wd + pl * B_BYTES + slice_off, wtile + (size_t)pl * B_BYTES + slice_off,
+                                           slice_bytes, &w_full[ws], cta_mask);
+              }
+              if (++ws == w_slots) { ws = 0; w_ph ^= 1; }
             }
-            if (++stage == num_stages) { stage = 0; phase ^= 1; }
           }
         }
       }
@@ -155,13 +206,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
     const int cw = wg - 1;                   // which 64-pixel half of the tile
     const int t = threadIdx.x & 127;
     const int wq = t >> 5;                   // warp inside the warpgroup: accumulator rows 16 wq .. 16 wq + 15
-    const int n = p.n_pad;
-    const int nch = n >> 4;
-    const int per = (nch + kColSplit - 1) / kColSplit;
-    const int nseg = (total_chunks + p.seg_chunks - 1) / p.seg_chunks;
-    const int n_total = p.n_tiles * p.n_pad;
-    const uint32_t smem_base_u32 = ptx::smem_u32(smem);
+    constexpr int nch = N >> 4;
+    constexpr int per = (nch + kColSplit - 1) / kColSplit;
+    const int n_total = p.n_tiles * N;
+    const bool strict = p.seg_chunks == 1;
+    const uint32_t a_ring_u32 = ptx::smem_u32(a_ring);
+    const uint32_t w_ring_u32 = ptx::smem_u32(w_ring);
     const uint32_t a_off = (uint32_t)(cw * 64 * TcSmem<KC>::kRowBytes);
+    const uint32_t dy_step = (uint32_t)(g.TW * TcSmem<KC>::kRowBytes);   // one image row of the box: whole 8-row atoms
     // epilogue ownership after the exchange: pixel `row`, chunks [grp * per, grp * per + my_chunks)
     const int row = cw * 64 + (t >> 1);
     const int grp = t & 1;
@@ -169,8 +221,16 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
     const int first_chunk = grp * per;
     const int my_chunks = (nch - first_chunk) < per ? ((nch - first_chunk) > 0 ? nch - first_chunk : 0) : per;
     float* xchg = s_xchg + cw * 64 * kXchgStride;
-    int stage = 0;
-    uint32_t phase = 0;
+    // a slot is released once the wgmma group that last read it has completed (one arrival per warpgroup, by thread 0;
+    // a weight slot in every CTA of the cluster)
+    auto release_a = [&](int s) { ptx::mbar_arrive_if(&a_empty[s], t == 0); };
+    auto release_w = [&](int s) {
+      if (cs == 1) ptx::mbar_arrive_if(&w_empty[s], t == 0);
+      else
+        for (int r = 0; r < cs; ++r) ptx::mbar_arrive_cluster_if(&w_empty[s], (uint32_t)r, t == 0);
+    };
+    int as = 0, ws = 0;
+    uint32_t a_ph = 0, w_ph = 0;
     for (int item = cluster_id; item < num_items; item += num_clusters) {
       const int n_tile = item % p.n_tiles;
       const int tile = (item / p.n_tiles) * cs + (int)rank;
@@ -181,111 +241,86 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
       const int y = ty * g.TH + py, x = tx * g.TW + px;
       const bool valid = real && (y < g.H) && (x < g.W);
 
-      float sum[64];
+      float sum[N / 2], corr[N / 2], dom[N / 2];
 #pragma unroll
-      for (int i = 0; i < 64; ++i) sum[i] = 0.f;
-      for (int s = 0; s < nseg; ++s) {
-        const int c0 = s * p.seg_chunks;
-        const int c1 = (c0 + p.seg_chunks < total_chunks) ? c0 + p.seg_chunks : total_chunks;
-        float acc[64];
-        if (p.seg_chunks == 1) {
-          // strictest setting: the segment is one stage and every 16-channel K slice (its three products) is promoted
-          // on its own, so no accumulator ever holds more than one slice
-          const int ch = c0 % p.chunks;
-          ptx::mbar_wait(&full_bar[stage], phase);
-          const uint32_t st_addr = smem_base_u32 + (uint32_t)stage * (uint32_t)STAGE_BYTES;
-          const uint64_t a_hi = make_smem_desc<KC>(st_addr + a_off);
-          const uint64_t a_lo = make_smem_desc<KC>(st_addr + A_BYTES + a_off);
-          const uint64_t b_hi = make_smem_desc<KC>(st_addr + NPLANES * A_BYTES);
-          const uint64_t b_lo = make_smem_desc<KC>(st_addr + NPLANES * A_BYTES + B_BYTES);
-          int ksteps = (p.cin_pad - ch * KC);
-          ksteps = (ksteps > KC ? KC : ksteps) >> 4;
+      for (int i = 0; i < N / 2; ++i) sum[i] = 0.f;
+      auto promote = [&]() {   // fp32 round-to-nearest: the small corrections first, then the dominant chain
+        ptx::reg_fence(corr);
+        ptx::reg_fence(dom);
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) {
+          if (NPLANES == 2) sum[i] += corr[i];
+          sum[i] += dom[i];
+        }
+      };
+      uint32_t acc_on = 0;          // 0: the next products start a new segment (accumulators from zero)
+      int seg_left = p.seg_chunks;  // weight tiles left in the current segment
+      int pend_w = -1, pend_a = -1; // slots read by the last committed, not yet completed group
+      for (int ch = 0; ch < chunks; ++ch) {
+        int ksteps = p.cin_pad - ch * KC;
+        ksteps = (ksteps > KC ? KC : ksteps) >> 4;
+        for (int dx = 0; dx < ksz; ++dx) {
+          ptx::mbar_wait(&a_full[as], a_ph);
+          const uint32_t a_addr = a_ring_u32 + (uint32_t)as * A_SLOT + a_off;
+          for (int dy = 0; dy < ksz; ++dy) {
+            ptx::mbar_wait(&w_full[ws], w_ph);
+            const uint32_t w_addr = w_ring_u32 + (uint32_t)ws * W_TILE;
+            const uint64_t a_hi = make_smem_desc<KC>(a_addr + (uint32_t)dy * dy_step);
+            const uint64_t a_lo = make_smem_desc<KC>(a_addr + (uint32_t)dy * dy_step + A_PLANE);
+            const uint64_t b_hi = make_smem_desc<KC>(w_addr);
+            const uint64_t b_lo = make_smem_desc<KC>(w_addr + B_BYTES);
+            const bool a_done = dy == ksz - 1;   // last tap that reads this activation slot
+            if (strict) {
+              // every 16-channel K slice (its three products) is promoted on its own
 #pragma unroll 1
-          for (int ks = 0; ks < ksteps; ++ks) {
-            const uint64_t kadd = (uint64_t)ks * 2u;
-            ptx::wgmma_fence();
-            if (NPLANES == 2) {
-              ptx::wgmma_f16_n<0, 0>(n, acc, a_lo + kadd, b_hi + kadd, 0);
-              ptx::wgmma_f16_n<0, 0>(n, acc, a_hi + kadd, b_lo + kadd, 1);
+              for (int ks = 0; ks < ksteps; ++ks) {
+                const uint64_t kadd = (uint64_t)ks * 2u;   // 32 bytes (16 fp16 along K) in 16-byte descriptor units
+                // acc_on is always 0 here; a run-time 0 rather than a literal keeps ptxas from treating the products
+                // as fresh definitions of corr / dom (which makes it wait for every group at every loop join)
+                tile_products<N, NPLANES, 1>(corr, dom, a_hi + kadd, a_lo + kadd, b_hi + kadd, b_lo + kadd, acc_on);
+                ptx::wgmma_wait<0>();
+                promote();
+              }
+              release_w(ws);
+              if (a_done) release_a(as);
+            } else {
+              // one straight-line batch per K-slice count: a branch inside a batch makes ptxas serialise the wgmma
+              if (ksteps == KC / 16)
+                tile_products<N, NPLANES, KC / 16>(corr, dom, a_hi, a_lo, b_hi, b_lo, acc_on);
+              else if (ksteps == 1)
+                tile_products<N, NPLANES, 1>(corr, dom, a_hi, a_lo, b_hi, b_lo, acc_on);
+              else if (KC == 64 && ksteps == 2)
+                tile_products<N, NPLANES, 2>(corr, dom, a_hi, a_lo, b_hi, b_lo, acc_on);
+              else if (KC == 64)
+                tile_products<N, NPLANES, 3>(corr, dom, a_hi, a_lo, b_hi, b_lo, acc_on);
+              acc_on = 1;
+              const bool item_end = a_done && dx == ksz - 1 && ch == chunks - 1;
+              if (--seg_left == 0 || item_end) {
+                ptx::wgmma_wait<0>();
+                promote();
+                acc_on = 0;
+                seg_left = p.seg_chunks;
+                if (pend_w >= 0) release_w(pend_w);
+                if (pend_a >= 0) release_a(pend_a);
+                release_w(ws);
+                if (a_done) release_a(as);
+                pend_w = pend_a = -1;
+              } else {
+                ptx::wgmma_wait<1>();   // the previous weight tile's group has completed
+                if (pend_w >= 0) release_w(pend_w);
+                if (pend_a >= 0) release_a(pend_a);
+                pend_w = ws;
+                pend_a = a_done ? as : -1;
+              }
             }
-            ptx::wgmma_f16_n<0, 0>(n, acc, a_hi + kadd, b_hi + kadd, NPLANES == 2 ? 1u : 0u);
-            ptx::wgmma_commit();
-            ptx::wgmma_wait<0>();
-            ptx::reg_fence(acc);
-#pragma unroll
-            for (int i = 0; i < 64; ++i) sum[i] += acc[i];
+            if (++ws == w_slots) { ws = 0; w_ph ^= 1; }
           }
-          if (t == 0) {
-            if (cs == 1) ptx::mbar_arrive(&empty_bar[stage]);
-            else
-              for (int r = 0; r < cs; ++r) ptx::mbar_arrive_cluster(&empty_bar[stage], (uint32_t)r);
-          }
-          if (++stage == num_stages) { stage = 0; phase ^= 1; }
-          continue;
+          if (++as == a_slots) { as = 0; a_ph ^= 1; }
         }
-        uint32_t accumulate = 0;   // every segment starts from zero
-        ptx::wgmma_fence();
-        // Pass A: as the stages of this segment land, issue the small correction products (a_lo*w_hi, a_hi*w_lo).
-        // Pass B: the dominant a_hi*w_hi products.  The accumulator only becomes large in pass B, so only those
-        // products contribute truncation error: 3x fewer "effective" steps per segment.
-        int st = stage;
-        uint32_t ph = phase;
-        for (int c = c0; c < c1; ++c) {
-          const int ch = c % p.chunks;
-          ptx::mbar_wait(&full_bar[st], ph);
-          if (NPLANES == 2) {
-            const uint32_t st_addr = smem_base_u32 + (uint32_t)st * (uint32_t)STAGE_BYTES;
-            const uint64_t a_hi = make_smem_desc<KC>(st_addr + a_off);
-            const uint64_t a_lo = make_smem_desc<KC>(st_addr + A_BYTES + a_off);
-            const uint64_t b_hi = make_smem_desc<KC>(st_addr + NPLANES * A_BYTES);
-            const uint64_t b_lo = make_smem_desc<KC>(st_addr + NPLANES * A_BYTES + B_BYTES);
-            int ksteps = (p.cin_pad - ch * KC);
-            ksteps = (ksteps > KC ? KC : ksteps) >> 4;
-#pragma unroll 1
-            for (int ks = 0; ks < ksteps; ++ks) {
-              const uint64_t kadd = (uint64_t)ks * 2u;  // 32 bytes (16 fp16 along K) in 16-byte descriptor units
-              ptx::wgmma_f16_n<0, 0>(n, acc, a_lo + kadd, b_hi + kadd, accumulate);
-              ptx::wgmma_f16_n<0, 0>(n, acc, a_hi + kadd, b_lo + kadd, 1);
-              accumulate = 1;
-            }
-          }
-          if (++st == num_stages) { st = 0; ph ^= 1; }
-        }
-        st = stage;
-        for (int c = c0; c < c1; ++c) {
-          const int ch = c % p.chunks;
-          const uint32_t st_addr = smem_base_u32 + (uint32_t)st * (uint32_t)STAGE_BYTES;
-          const uint64_t a_hi = make_smem_desc<KC>(st_addr + a_off);
-          const uint64_t b_hi = make_smem_desc<KC>(st_addr + NPLANES * A_BYTES);
-          int ksteps = (p.cin_pad - ch * KC);
-          ksteps = (ksteps > KC ? KC : ksteps) >> 4;
-#pragma unroll 1
-          for (int ks = 0; ks < ksteps; ++ks) {
-            const uint64_t kadd = (uint64_t)ks * 2u;
-            ptx::wgmma_f16_n<0, 0>(n, acc, a_hi + kadd, b_hi + kadd, accumulate);
-            accumulate = 1;
-          }
-          if (++st == num_stages) st = 0;
-        }
-        ptx::wgmma_commit();
-        ptx::wgmma_wait<0>();
-        ptx::reg_fence(acc);
-        // the segment's stages have been read: release them in every CTA of the cluster
-        st = stage;
-        for (int c = c0; c < c1; ++c) {
-          if (t == 0) {
-            if (cs == 1) ptx::mbar_arrive(&empty_bar[st]);
-            else
-              for (int r = 0; r < cs; ++r) ptx::mbar_arrive_cluster(&empty_bar[st], (uint32_t)r);
-          }
-          if (++st == num_stages) st = 0;
-        }
-        stage = st;
-        phase = ph;
-        // fp32 round-to-nearest promotion (registers past n / 2 hold no columns and are never stored)
-#pragma unroll
-        for (int i = 0; i < 64; ++i) sum[i] += acc[i];
       }
+      // the last weight tile ended a segment, so every group has completed; saying so here keeps ptxas from placing
+      // its own wait inside the loop, ahead of the exchange that reuses the accumulator registers
+      ptx::wgmma_wait<0>();
 
       // Exchange: the wgmma layout gives a thread rows 16 wq + lane / 4 (+ 8) and column pairs 8 j + 2 (lane % 4); the
       // epilogue wants one pixel and 16 consecutive columns per thread.  Round k moves chunks k and per + k.
@@ -294,12 +329,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
       for (int i = 0; i < 9; ++i) v9[i] = 0.f;
       const int r0 = wq * 16 + (lane >> 2), cq = 2 * (lane & 3);
 #pragma unroll
-      for (int k = 0; k < kMaxTileN / 16 / kColSplit; ++k) {
-        if (k >= per) break;
+      for (int k = 0; k < per; ++k) {
         ptx::named_bar_sync(1 + cw, 128);    // readers of the previous round are done
 #pragma unroll
-        for (int c = 0; c < kMaxTileN / 16; ++c) {
-          if (c < nch && (c == k || c == per + k)) {
+        for (int c = 0; c < nch; ++c) {
+          if (c == k || c == per + k) {
             float* dst = xchg + (c == k ? 0 : 16);
 #pragma unroll
             for (int h = 0; h < 2; ++h) {      // 8-column halves of the chunk: accumulator group j = 2 c + h
@@ -320,7 +354,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
             const float4 f = srcp[q];
             v[4 * q] = f.x; v[4 * q + 1] = f.y; v[4 * q + 2] = f.z; v[4 * q + 3] = f.w;
           }
-          const int cg = n_tile * p.n_pad + (first_chunk + k) * 16;
+          const int cg = n_tile * N + (first_chunk + k) * 16;
           if (p.epi.mode == EPI_D2S_RDOT) {
             // the host guarantees that a thread's columns are whole sub-pixels (rdot_parts == 1) or an equal share of
             // one sub-pixel (rdot_parts > 1: each share writes its own partial plane set)

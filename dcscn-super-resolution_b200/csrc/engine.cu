@@ -104,7 +104,7 @@ struct TcLaunch {
   ConvTCParams p;
   ConvRefParams ref;
   int grid = 0;
-  int stages = 0;
+  int a_slots = 0, w_slots = 0;  // activation / weight ring depths of conv_tc_kernel
   size_t smem = 0;
 };
 
@@ -732,12 +732,28 @@ static int ensure_workspace(dcscn_handle* h, size_t lr_px) {
 }
 
 // --------------------------------------------------------------------------------------- plans ----
-static void choose_patch(int H, int W, int* TH, int* TW) {
-  // 128-pixel rectangular patches; minimise padded area, prefer wide patches (contiguous TMA rows)
+// Shared memory of conv_tc_kernel left for its activation and weight rings (barriers, R-CNN1 taps and the epilogue
+// exchange take the rest).
+constexpr size_t kTcRingBudget = 227 * 1024 - 1024 - kTcBarrierBytes - kRdotSmemBytes - kXchgBytes;
+
+// Whether a k x k layer (k > 1) can run on a TH x TW patch: its ky taps are read at row offsets of TW pixels inside one
+// activation box of TW x (TH + k - 1) pixels, which the swizzled operand descriptors allow only in whole 8-row atoms (TW
+// a multiple of 8), and two such boxes plus two weight tiles must fit in shared memory.
+static bool tc_patch_fits(int KC, int nplanes, int n_pad, int ksz, int TH, int TW) {
+  if (ksz == 1) return true;
+  if (TW % 8 != 0) return false;
+  return 2 * (size_t)nplanes * tc_a_plane_bytes(KC, TW, TH, ksz) + 2 * (size_t)tc_w_tile_bytes(KC, nplanes, n_pad) <=
+         kTcRingBudget;
+}
+
+// 128-pixel rectangular patches; minimise padded area, prefer wide patches (contiguous TMA rows).  Returns false when no
+// patch suits the layer.
+static bool choose_patch(int H, int W, int KC, int nplanes, int n_pad, int ksz, int* TH, int* TW) {
   static const int cand[][2] = {{8, 16}, {4, 32}, {16, 8}, {2, 64}, {32, 4}, {1, 128}, {64, 2}, {128, 1}};
   long long best = -1;
   for (auto& c : cand) {
     const int th = c[0], tw = c[1];
+    if (!tc_patch_fits(KC, nplanes, n_pad, ksz, th, tw)) continue;
     long long area = (long long)((H + th - 1) / th) * th * ((W + tw - 1) / tw) * tw;
     if (best < 0 || area < best) {
       best = area;
@@ -745,6 +761,7 @@ static void choose_patch(int H, int W, int* TH, int* TW) {
       *TW = tw;
     }
   }
+  return best >= 0;
 }
 
 static int encode_map(dcscn_handle* h, CUtensorMap* tm, const __half* base, int cin_pad, int pitch, int n, int H,
@@ -768,12 +785,17 @@ static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, const __ha
                          int src_pitch, int n, int H, int W, const EpiParams& epi) {
   TcLaunch L;
   memset(&L, 0, sizeof(L));
-  int TH, TW;
-  choose_patch(H, W, &TH, &TW);
+  int TH = 0, TW = 0;
+  if (!choose_patch(H, W, h->kc, planes(h), t.n_pad, t.ksz, &TH, &TW))
+    return fail("layer %s: no pixel patch fits a %dx%d filter in shared memory", t.name.c_str(), t.ksz, t.ksz);
+  // the kernel's ky taps start TW pixels apart inside the box: whole 8-row swizzle atoms, or the operands are misread
+  if (t.ksz > 1 && (TW * h->kc * 2) % (8 * h->kc * 2) != 0)
+    return fail("internal: layer %s: patch width %d is not a whole number of swizzle atoms", t.name.c_str(), TW);
   ConvGeom g{n, H, W, (W + TW - 1) / TW, (H + TH - 1) / TH, TW, TH};
-  if (encode_map(h, &L.tm_hi, src_hi, t.cin_pad, src_pitch, n, H, W, TH, TW)) return 1;
+  const int box_rows = TH + t.ksz - 1;   // a k x k layer's box carries the rows of all k ky taps
+  if (encode_map(h, &L.tm_hi, src_hi, t.cin_pad, src_pitch, n, H, W, box_rows, TW)) return 1;
   if (planes(h) == 2) {
-    if (encode_map(h, &L.tm_lo, src_lo, t.cin_pad, src_pitch, n, H, W, TH, TW)) return 1;
+    if (encode_map(h, &L.tm_lo, src_lo, t.cin_pad, src_pitch, n, H, W, box_rows, TW)) return 1;
   } else {
     L.tm_lo = L.tm_hi;
   }
@@ -783,7 +805,9 @@ static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, const __ha
   L.p.chunks = (t.cin_pad + h->kc - 1) / h->kc;
   L.p.n_tiles = t.n_tiles;
   L.p.n_pad = t.n_pad;
-  L.p.seg_chunks = h->seg_chunks;  // finalised per kernel variant below (needs the stage count)
+  // weight tiles per promotion segment; 1 = promote every 16-channel K slice.  The automatic lengths keep the dominant
+  // chain as short as the earlier two-pass scheme had it (2 tiles for wide layers, 3 for thin ones).
+  L.p.seg_chunks = h->seg_chunks > 0 ? h->seg_chunks : (t.n_pad > 64 ? 2 : 3);
   int cs = h->cluster;
   while (cs > 1 && (t.n_pad % cs != 0 || h->sm_count % cs != 0)) cs >>= 1;
   L.p.cluster_size = cs;
@@ -802,16 +826,26 @@ static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, const __ha
   L.p.epi.n_valid = t.n_valid;
   L.p.epi.drop_ntotal = pad16(t.cout);   // keep-mask index stride = slot width, whatever the column tiling
 
-  const size_t stage = tc_stage_bytes(h->kc, planes(h), t.n_pad);
-  const size_t budget = 227 * 1024 - 2048 - kRdotSmemBytes - kXchgBytes;
-  int stages = (int)std::min<size_t>(kMaxStages, budget / stage);
-  if (stages < 2) return fail("layer %s: pipeline stage of %zu bytes does not fit twice in shared memory", t.name.c_str(), stage);
-  L.stages = stages;
-  {
-    int seg = h->seg_chunks > 0 ? h->seg_chunks : (t.n_pad >= 112 ? 2 : 3);
-    L.p.seg_chunks = std::max(1, std::min(seg, stages - 1));   // a segment's stages stay resident until its 2nd pass
+  // Ring depths.  The consumers release a slot one weight tile late, so each ring needs at least two slots.  A k x k layer
+  // reads k weight tiles per activation slot: three activation slots when four weight tiles still fit, else two.
+  // A 1x1 layer pairs one activation slot with one weight tile.
+  const size_t a_slot = (size_t)planes(h) * tc_a_plane_bytes(h->kc, TW, TH, t.ksz);
+  const size_t w_tile = tc_w_tile_bytes(h->kc, planes(h), t.n_pad);
+  const size_t budget = kTcRingBudget;
+  int a_slots, w_slots;
+  if (t.ksz == 1) {
+    a_slots = w_slots = (int)std::min<size_t>(kMaxASlots, budget / (a_slot + w_tile));
+  } else {
+    a_slots = 3;
+    if (budget < a_slots * a_slot + 4 * w_tile) a_slots = 2;
+    w_slots = budget < a_slots * a_slot ? 0 : (int)std::min<size_t>(kMaxWSlots, (budget - a_slots * a_slot) / w_tile);
   }
-  L.smem = stages * stage + 1024 + 256 + kRdotSmemBytes + kXchgBytes;
+  if (a_slots < 2 || w_slots < 2)
+    return fail("layer %s: two %zu-byte activation slots and two %zu-byte weight tiles do not fit in shared memory",
+                t.name.c_str(), a_slot, w_tile);
+  L.a_slots = a_slots;
+  L.w_slots = w_slots;
+  L.smem = a_slots * a_slot + w_slots * w_tile + 1024 + kTcBarrierBytes + kRdotSmemBytes + kXchgBytes;
   const long long tiles = (long long)n * g.tiles_x * g.tiles_y;
   const long long items = ((tiles + cs - 1) / cs) * t.n_tiles;    // cluster iterations
   L.grid = (int)std::min<long long>(items, h->sm_count / cs) * cs;
@@ -960,12 +994,12 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
 }
 
 // ------------------------------------------------------------------------------------- forward ----
-template <int KC, int NPL>
+template <int KC, int NPL, int N>
 static int launch_tc_inst(dcscn_handle* h, const TcLaunch& L, cudaStream_t st) {
   static bool attr_set_dev[64] = {};   // function attributes are per device
   bool& attr_set = attr_set_dev[h->cfg.device_id & 63];
   if (!attr_set) {
-    CUDA_TRY(cudaFuncSetAttribute(conv_tc_kernel<KC, NPL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    CUDA_TRY(cudaFuncSetAttribute(conv_tc_kernel<KC, NPL, N>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
   cudaLaunchConfig_t cfg;
@@ -981,8 +1015,23 @@ static int launch_tc_inst(dcscn_handle* h, const TcLaunch& L, cudaStream_t st) {
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = L.p.cluster_size > 1 ? 1 : 0;
-  CUDA_TRY(cudaLaunchKernelEx(&cfg, conv_tc_kernel<KC, NPL>, L.tm_hi, L.tm_lo, L.p, L.stages));
+  CUDA_TRY(cudaLaunchKernelEx(&cfg, conv_tc_kernel<KC, NPL, N>, L.tm_hi, L.tm_lo, L.p, L.a_slots, L.w_slots));
   return 0;
+}
+
+// The column-tile width is a template parameter of the kernel (the wgmma width is an immediate of the instruction).
+template <int KC, int NPL>
+static int launch_tc_width(dcscn_handle* h, const TcLaunch& L, cudaStream_t st) {
+  switch (L.p.n_pad) {
+    case 16: return launch_tc_inst<KC, NPL, 16>(h, L, st);
+    case 32: return launch_tc_inst<KC, NPL, 32>(h, L, st);
+    case 48: return launch_tc_inst<KC, NPL, 48>(h, L, st);
+    case 64: return launch_tc_inst<KC, NPL, 64>(h, L, st);
+    case 80: return launch_tc_inst<KC, NPL, 80>(h, L, st);
+    case 96: return launch_tc_inst<KC, NPL, 96>(h, L, st);
+    case 112: return launch_tc_inst<KC, NPL, 112>(h, L, st);
+  }
+  return fail("internal: column tile width %d is not a multiple of 16 in [16, %d]", L.p.n_pad, kMaxTileN);
 }
 
 static int launch_tc(dcscn_handle* h, const TcLaunch& Lc, cudaStream_t st) {
@@ -1003,8 +1052,8 @@ static int launch_tc(dcscn_handle* h, const TcLaunch& Lc, cudaStream_t st) {
   }
   const int npl = planes(h);
   if (L.p.wpack == nullptr) return fail("internal: weight image was not packed for this layer");
-  if (h->kc == 64) return npl == 2 ? launch_tc_inst<64, 2>(h, L, st) : launch_tc_inst<64, 1>(h, L, st);
-  return npl == 2 ? launch_tc_inst<32, 2>(h, L, st) : launch_tc_inst<32, 1>(h, L, st);
+  if (h->kc == 64) return npl == 2 ? launch_tc_width<64, 2>(h, L, st) : launch_tc_width<64, 1>(h, L, st);
+  return npl == 2 ? launch_tc_width<32, 2>(h, L, st) : launch_tc_width<32, 1>(h, L, st);
 }
 
 static int mark(dcscn_handle* h, cudaStream_t st) {

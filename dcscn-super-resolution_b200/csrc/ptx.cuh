@@ -109,15 +109,31 @@ __device__ __forceinline__ void bulk_load_multicast(void* smem_dst, const void* 
       : "memory");
 }
 
-// Arrive on the mbarrier at the same shared-memory offset in CTA `cta` of this cluster (release at cluster scope).
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+// Releases of a pipeline slot whose readers were wgmma (complete once wgmma.wait_group returns): executed by every
+// thread and predicated on `pred` inside the instruction, so no branch breaks the warp-uniform path of a wgmma sequence
+// in flight (a divergent branch there makes ptxas serialise the wgmma).  Default (.release.cta) semantics: a
+// .release.cluster arrive costs a GPU-scope memory barrier per call, and the slot's next writer is the async proxy.
+__device__ __forceinline__ void mbar_arrive_if(uint64_t* bar, bool pred) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %1, 0;\n\t"
+      "@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t"
+      "}\n" ::"r"(smem_u32(bar)),
+      "r"((uint32_t)pred)
+      : "memory");
+}
+// Same, on the mbarrier at the same shared-memory offset in CTA `cta` of this cluster.
+__device__ __forceinline__ void mbar_arrive_cluster_if(uint64_t* bar, uint32_t cta, bool pred) {
   asm volatile(
       "{\n\t"
       ".reg .b32 remote;\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %2, 0;\n\t"
       "mapa.shared::cluster.u32 remote, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [remote];\n\t"
+      "@p mbarrier.arrive.shared::cluster.b64 _, [remote];\n\t"
       "}\n" ::"r"(smem_u32(bar)),
-      "r"(cta)
+      "r"(cta), "r"((uint32_t)pred)
       : "memory");
 }
 
@@ -242,8 +258,8 @@ DCSCN_WGMMA_N128(0, 0)
 DCSCN_WGMMA_N128(1, 1)
 #undef DCSCN_WGMMA_N128
 
-// Width chosen at run time (uniform branch per instruction): one accumulator array of 64 registers serves every
-// column tile width of the kernels (n <= 128, multiple of 16); registers past n / 2 are left untouched.
+// Width chosen at run time (uniform branch per instruction), for the filter-gradient kernel: one accumulator array of 64
+// registers serves every product width (n <= 128, multiple of 16); registers past n / 2 are left untouched.
 template <int TA, int TB>
 __device__ __forceinline__ void wgmma_f16_n(int n, float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
   switch (n) {
