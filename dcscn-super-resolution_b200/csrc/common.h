@@ -71,12 +71,11 @@ struct ConvTCParams {
   ConvGeom g;
   int ksz;               // 1 or 3
   int cin_pad;           // padded input channels of the source slot (multiple of 16)
-  int chunks;            // ceil(cin_pad / KC)
+  int chunks;            // ceil(cin_pad / 64)
   int n_tiles;           // column tiles (N > kMaxTileN is split)
   int n_pad;             // columns per tile, multiple of 16, <= kMaxTileN (112)
   int seg_chunks;        // pipeline stages per accumulation segment (fp32 promotion period)
-  int cluster_size;      // CTAs per cluster sharing (multicasting) the weight tiles: 1, 2 or 4
-  const __half* wpack;   // packed weights [n_tile][tap][chunk][plane][n_pad x KC] (pre-swizzled)
+  const __half* wpack;   // packed weights [n_tile][tap][chunk][plane][n_pad x 64] (pre-swizzled)
   EpiParams epi;
 };
 

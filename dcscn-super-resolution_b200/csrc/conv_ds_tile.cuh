@@ -1,9 +1,11 @@
-// Depthwise-separable layers, second generation (reference: helper/tf_graph.py:155-216; first generation and the full
-// statement of the op in conv_ds.cuh, kept as the cross-check `ds_impl = 1`).
+// Depthwise-separable DCSCN layers (reference: helper/tf_graph.py:155-216 `depthwise_separable_conv2d` /
+// `build_depthwise_separable_conv`, i.e. tf.nn.separable_conv2d: depthwise k x k with channel multiplier 1 and no
+// bias, then pointwise 1x1, then +bias, then PReLU; used for EVERY layer of a `--depthwise_separable` graph incl. the
+// 1x1 A1/B1 (a per-channel scale) and R-CNN1).
 //
-// conv_ds.cuh is instruction-issue bound (a handful of FMAs per shared-memory load, DRAM mostly idle): a
-// warp walked 8 pixels serially for the depthwise pass (3 dependent global loads per pixel) and the pointwise GEMM left
-// half of the threads idle on layers with few output channels.  Here:
+// These graphs are tiny (c-DCSCN: <= 131 channels, 14,240 MAC per LR pixel at x4): a 131 x 24 contraction per pixel
+// does not fill a tensor-core tile, so every layer is one kernel on CUDA cores over fp32 NHWC activations, and the
+// depthwise value never leaves registers.  The layout keeps every thread issuing FMAs:
 //   * one CTA = a 16 x 16 pixel tile (3x3 layers) or 256 consecutive pixels (1x1 layers), ONE PIXEL PER THREAD;
 //   * the input tile (+1 halo, 32-channel chunks) is staged with 16-byte coalesced loads into shared memory with an odd
 //     channel pitch (33) and a row stride of 24 pixels, so that the 4 x 8 pixel block of a warp reads 32 distinct banks
@@ -13,7 +15,9 @@
 //     thread, no second pass over shared memory, no idle threads;
 //   * layers with more than 32 output columns (Up-PS: 32 -> 128) loop over groups of 32 columns on the staged tile;
 //   * two destinations (the fused A1 | B1 1x1 layer writes its A1 columns to the [B2 | A1] buffer and its B1 columns
-//     to the B1 buffer), depth_to_space scatter and the final + x2 are epilogue variants as before.
+//     to the B1 buffer), depth_to_space scatter and the final + x2 are epilogue variants;
+//   * R-CNN1 (1 -> 1 channel at HR resolution) has kernels of its own: four pixels of a row per thread
+//     (ds_single4_kernel), or one pixel per thread where the row width or the alignment does not allow four.
 // fp32 throughout (CUDA cores): the contraction depth is <= 140 and the layers are HBM / issue bound, not FLOP bound.
 #pragma once
 #include <cstdint>
@@ -37,7 +41,6 @@ struct DsTileParams {
   int d2s_r, d2s_cout;       // depth_to_space scatter (DCR) into dst [N, r*H, r*W, dst_pitch]
   const float* add;          // + x2 on channel 0 (cout == 1)
   int tiles_x, tiles_y;      // 3x3: 16 x 16 tiles per image
-  int cache_u;               // keep the depthwise values of a thread across column groups (host: ds_tile_caches_depthwise)
 };
 
 constexpr int kDtThreads = 256;
@@ -67,7 +70,8 @@ __global__ void __launch_bounds__(kDtThreads) ds_tile_kernel(const DsTileParams 
   float* s_pw = s_in + IN_PX * kDtCP;                              // [cin][COLS]  (current column group)
   float* s_dw = s_pw + p.cin * COLS;                               // [kk][cin]
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const bool cache_u = KSZ == 3 && p.cache_u != 0 && p.cout > COLS && p.cin <= kDtCC;
+  // the host's ds_tile_caches_depthwise test (cout > COLS only when cout > 32), which sized shared memory for the cache
+  const bool cache_u = KSZ == 3 && p.cout > COLS && p.cin <= kDtCC;
   float* s_u = s_dw + kk * p.cin + tid * kDtCP;                    // this thread's depthwise values [<= 32] (odd pitch: no bank conflicts)
 
   // ---- which pixels ----
@@ -305,6 +309,35 @@ __global__ void __launch_bounds__(256) ds_single4_kernel(const float* __restrict
     }
     const float4 x2 = add ? __ldg(reinterpret_cast<const float4*>(add + row * W + 4 * x4)) : make_float4(0.f, 0.f, 0.f, 0.f);
     *reinterpret_cast<float4*>(dst + row * W + 4 * x4) = make_float4(acc[0] + x2.x, acc[1] + x2.y, acc[2] + x2.z, acc[3] + x2.w);
+  }
+}
+
+// Same layer (k x k) with one pixel per thread: for HR widths that are not a multiple of 4, unaligned x2 / y, or a 1x1
+// R-CNN1.  Row and column come from 64-bit pixel indices, so any number of pixels is covered.
+template <int KSZ>
+__global__ void __launch_bounds__(256) ds_single_kernel(const float* __restrict__ src, const float* __restrict__ add,
+                                                        float* __restrict__ dst, int n_img, int H, int W, const float* dw,
+                                                        const float* pw, const float* bias, const float* alpha) {
+  constexpr int kk = KSZ * KSZ, half = KSZ >> 1;
+  float w[kk];
+#pragma unroll
+  for (int t = 0; t < kk; ++t) w[t] = __ldg(dw + t) * __ldg(pw);
+  const float b = bias ? __ldg(bias) : 0.f;
+  const long long total = (long long)n_img * H * W;
+  for (long long gp = (long long)blockIdx.x * blockDim.x + threadIdx.x; gp < total; gp += (long long)gridDim.x * blockDim.x) {
+    const long long row = gp / W;
+    const int x = (int)(gp - row * W);
+    const int y = (int)(row % H);
+    float acc = b;
+#pragma unroll
+    for (int t = 0; t < kk; ++t) {
+      const int dy = t / KSZ - half, dx = t % KSZ - half;
+      if ((unsigned)(y + dy) < (unsigned)H && (unsigned)(x + dx) < (unsigned)W)
+        acc = fmaf(__ldg(src + gp + (long long)dy * W + dx), w[t], acc);
+    }
+    if (alpha) acc = acc > 0.f ? acc : __ldg(alpha) * acc;
+    if (add) acc += __ldg(add + gp);
+    dst[gp] = acc;
   }
 }
 

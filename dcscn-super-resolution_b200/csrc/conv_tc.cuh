@@ -4,7 +4,7 @@
 // (helper/tf_graph.py:104-153 conv2d / build_conv; :238-249 build_pixel_shuffler_layer).
 //
 // GEMM view:  D[M = 128 pixels (TH x TW patch), N = cout (padded to 16, <= 112 per column tile)]
-//             = sum over input-channel chunks, taps (kx, ky) of  A_tap[128 x KC] * W_tap[KC x N]
+//             = sum over 64-channel input chunks, taps (kx, ky) of  A_tap[128 x 64] * W_tap[64 x N]
 //   * A tiles are fetched by TMA (4-D tiled tensor map over the NHWC fp16 plane).  A k x k layer (k = 3 or 5) loads ONE
 //     box of TW x (TH + k - 1) pixels per (chunk, kx), its origin shifted by (kx - k / 2, -k / 2); the k ky taps read it
 //     at row offsets 0, TW, ..., (k - 1) TW.  The host only picks patches with TW a multiple of 8, so every offset is a
@@ -25,15 +25,11 @@
 //   * Two shared-memory rings with their own full/empty mbarriers: activation slots (one per (chunk, kx)) and weight
 //     tiles (one per (tap, chunk), read from the packed image [n_tile][tap][chunk]).  The consumers commit one wgmma
 //     group per weight tile and release a slot as soon as `wgmma.wait_group 1` shows the group that last read it
-//     has completed, so both rings work purely as prefetch depth.
-//   * Weight tiles are a large share of the L2->SM traffic (every 128-pixel tile streams the whole layer's weights).
-//     CTAs are launched in clusters of `cs` (1, 2 or 4) that walk pixel tiles in lockstep; each CTA fetches 1/cs of
-//     every weight tile and multicasts it to the whole cluster (cp.async.bulk ... .multicast::cluster), and each
-//     consumer warpgroup releases a weight slot in all cluster members (remote mbarrier arrive).
+//     has completed, so both rings work purely as prefetch depth.  A weight tile arrives as one bulk copy.
 //   * Warp roles: warpgroup 0 = producer (warp 0 issues TMA), warpgroups 1 and 2 = consumers, one per 64-pixel half
 //     of the tile: they issue the wgmma of their rows, promote, and run the epilogue (bias/PReLU/split -> global) after
 //     an exchange through shared memory that gives every thread one pixel and a run of 16-column chunks.  Persistent
-//     CTAs stride over (pixel-tile, column-tile) work items.
+//     CTAs (one per SM) stride over (pixel-tile, column-tile) work items.
 #pragma once
 #include "common.h"
 #include "epilogue.cuh"
@@ -53,29 +49,29 @@ constexpr int kRdotSmemBytes = 9 * 128 * 4;         // fused R-CNN1 filter taps 
 constexpr int kColSplit = 2;                       // epilogue threads per pixel, each owning a contiguous run of chunks
 constexpr int kXchgStride = 36;                    // floats per pixel row of the epilogue exchange buffer (2 chunks + pad)
 constexpr int kXchgBytes = kConsumerWGs * 64 * kXchgStride * 4;
+constexpr int kTcKC = 64;                          // input channels per K chunk: an fp16 operand row is 128 bytes,
+                                                   // one row of the SWIZZLE_128B layout
 
-template <int KC>
 struct TcSmem {
-  static constexpr int kRowBytes = KC * 2;                  // 128 (SWIZZLE_128B) or 64 (SWIZZLE_64B)
+  static constexpr int kRowBytes = kTcKC * 2;               // 128 (SWIZZLE_128B)
   static constexpr int kSbo = 8 * kRowBytes;                // 8-row core-matrix group stride
-  static constexpr uint64_t kLayout = (KC == 64) ? 1ull : 2ull;  // wgmma descriptor layout type: SW128 = 1, SW64 = 2
+  static constexpr uint64_t kLayout = 1ull;                 // wgmma descriptor layout type: SW128 = 1
 };
 
 // wgmma shared-memory matrix descriptor of a K-major swizzled operand tile: start address >> 4 in [0,14), leading
 // byte offset (unused for swizzled K-major, 1) in [16,30), stride byte offset >> 4 in [32,46), layout type in [62,64).
-template <int KC>
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(TcSmem<KC>::kSbo >> 4) << 32) |
-         (TcSmem<KC>::kLayout << 62);
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(TcSmem::kSbo >> 4) << 32) |
+         (TcSmem::kLayout << 62);
 }
 
 // Bytes of one activation plane in a ring slot: the TMA box of TW x (TH + ksz - 1) pixels, rounded up to 1024 bytes
 // so that every slot and plane starts on a swizzle-atom boundary.
-__host__ __device__ inline uint32_t tc_a_plane_bytes(int KC, int TW, int TH, int ksz) {
-  return ((uint32_t)TW * (uint32_t)(TH + ksz - 1) * (uint32_t)KC * 2u + 1023u) & ~1023u;
+__host__ __device__ inline uint32_t tc_a_plane_bytes(int TW, int TH, int ksz) {
+  return ((uint32_t)TW * (uint32_t)(TH + ksz - 1) * (uint32_t)kTcKC * 2u + 1023u) & ~1023u;
 }
-__host__ __device__ inline uint32_t tc_w_tile_bytes(int KC, int nplanes, int n_pad) {
-  return (uint32_t)nplanes * (uint32_t)n_pad * (uint32_t)KC * 2u;
+__host__ __device__ inline uint32_t tc_w_tile_bytes(int nplanes, int n_pad) {
+  return (uint32_t)nplanes * (uint32_t)n_pad * (uint32_t)kTcKC * 2u;
 }
 
 // One wgmma batch: the products of KS consecutive 16-channel K slices of a weight tile, committed as one group.
@@ -97,7 +93,7 @@ __device__ __forceinline__ void tile_products(float (&corr)[N / 2], float (&dom)
   ptx::wgmma_commit();
 }
 
-template <int KC, int NPLANES, int N>
+template <int NPLANES, int N>
 __global__ void __launch_bounds__(kTcThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant__ CUtensorMap tm_lo,
                const ConvTCParams p, const int a_slots, const int w_slots) {
@@ -107,10 +103,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const ConvGeom& g = p.g;
   const int ksz = p.ksz;
-  const uint32_t A_PLANE = tc_a_plane_bytes(KC, g.TW, g.TH, ksz);
+  const uint32_t A_PLANE = tc_a_plane_bytes(g.TW, g.TH, ksz);
   const uint32_t A_SLOT = NPLANES * A_PLANE;
-  const uint32_t A_TX = (uint32_t)NPLANES * (uint32_t)g.TW * (uint32_t)(g.TH + ksz - 1) * KC * 2u;  // bytes TMA delivers
-  constexpr uint32_t B_BYTES = N * KC * 2;
+  const uint32_t A_TX = (uint32_t)NPLANES * (uint32_t)g.TW * (uint32_t)(g.TH + ksz - 1) * kTcKC * 2u;  // bytes TMA delivers
+  constexpr uint32_t B_BYTES = N * kTcKC * 2;
   constexpr uint32_t W_TILE = NPLANES * B_BYTES;
   uint8_t* a_ring = smem;
   uint8_t* w_ring = smem + (size_t)a_slots * A_SLOT;
@@ -123,18 +119,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
 
   const int wg = threadIdx.x >> 7;
   const int lane = threadIdx.x & 31;
-  const int cs = p.cluster_size;
-  const uint32_t rank = cs > 1 ? ptx::cluster_ctarank() : 0u;
-  const uint16_t cta_mask = (uint16_t)((1u << cs) - 1u);
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < a_slots; ++s) {
       ptx::mbar_init(&a_full[s], 1);
-      ptx::mbar_init(&a_empty[s], kConsumerWGs);        // activations are this CTA's own
+      ptx::mbar_init(&a_empty[s], kConsumerWGs);   // one arrival per consumer warpgroup
     }
     for (int s = 0; s < w_slots; ++s) {
       ptx::mbar_init(&w_full[s], 1);
-      ptx::mbar_init(&w_empty[s], kConsumerWGs * cs);   // one arrival per consumer warpgroup of every cluster CTA
+      ptx::mbar_init(&w_empty[s], kConsumerWGs);
     }
     ptx::fence_barrier_init();
     ptx::fence_proxy_async();
@@ -142,14 +135,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
   if (p.epi.mode == EPI_D2S_RDOT)
     for (int i = threadIdx.x; i < p.epi.rdot_taps * p.epi.d2s_cout; i += blockDim.x) s_rdot[i] = p.epi.rdot_w[i];
   __syncthreads();
-  if (cs > 1) ptx::cluster_sync();               // peers' barriers are initialised before anything targets them
 
   const int tiles_per_img = g.tiles_x * g.tiles_y;
-  const int num_tiles = g.n_img * tiles_per_img;
-  const int groups = (num_tiles + cs - 1) / cs;  // cs pixel tiles are processed by one cluster iteration
-  const int num_items = groups * p.n_tiles;
-  const int cluster_id = blockIdx.x / cs;
-  const int num_clusters = gridDim.x / cs;
+  const int num_items = g.n_img * tiles_per_img * p.n_tiles;
   const int half = ksz >> 1;
   const int chunks = p.chunks;
 
@@ -159,15 +147,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
     if (threadIdx.x == 0) {
       ptx::prefetch_tensormap(&tm_hi);
       if (NPLANES == 2) ptx::prefetch_tensormap(&tm_lo);
-      constexpr uint32_t slice_full = B_BYTES;
-      const uint32_t slice_bytes = slice_full / (uint32_t)cs;     // this CTA's share of every weight plane
-      const uint32_t slice_off = rank * slice_bytes;
       int as = 0, ws = 0;
       uint32_t a_ph = 0, w_ph = 0;
-      for (int item = cluster_id; item < num_items; item += num_clusters) {
+      for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
         const int n_tile = item % p.n_tiles;
-        int tile = (item / p.n_tiles) * cs + (int)rank;
-        if (tile >= num_tiles) tile = num_tiles - 1;             // lockstep filler (stores are masked)
+        const int tile = item / p.n_tiles;
         const int img = tile / tiles_per_img;
         const int t2 = tile - img * tiles_per_img;
         const int ty = t2 / g.tiles_x, tx = t2 - ty * g.tiles_x;
@@ -178,22 +162,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
             ptx::mbar_wait(&a_empty[as], a_ph ^ 1);
             uint8_t* ad = a_ring + (size_t)as * A_SLOT;
             ptx::mbar_arrive_expect_tx(&a_full[as], A_TX);
-            ptx::tma_load_4d(ad, &tm_hi, &a_full[as], ch * KC, x0 + dx, y0, img);
-            if (NPLANES == 2) ptx::tma_load_4d(ad + A_PLANE, &tm_lo, &a_full[as], ch * KC, x0 + dx, y0, img);
+            ptx::tma_load_4d(ad, &tm_hi, &a_full[as], ch * kTcKC, x0 + dx, y0, img);
+            if (NPLANES == 2) ptx::tma_load_4d(ad + A_PLANE, &tm_lo, &a_full[as], ch * kTcKC, x0 + dx, y0, img);
             if (++as == a_slots) { as = 0; a_ph ^= 1; }
             for (int dy = 0; dy < ksz; ++dy) {
               ptx::mbar_wait(&w_empty[ws], w_ph ^ 1);
               uint8_t* wd = w_ring + (size_t)ws * W_TILE;
               ptx::mbar_arrive_expect_tx(&w_full[ws], W_TILE);
               const uint8_t* wtile = wsrc + (size_t)((dy * ksz + dx) * chunks + ch) * W_TILE;
-              if (cs == 1) {
-                ptx::bulk_load(wd, wtile, W_TILE, &w_full[ws]);
-              } else {
-#pragma unroll
-                for (int pl = 0; pl < NPLANES; ++pl)
-                  ptx::bulk_load_multicast(wd + pl * B_BYTES + slice_off, wtile + (size_t)pl * B_BYTES + slice_off,
-                                           slice_bytes, &w_full[ws], cta_mask);
-              }
+              ptx::bulk_load(wd, wtile, W_TILE, &w_full[ws]);
               if (++ws == w_slots) { ws = 0; w_ph ^= 1; }
             }
           }
@@ -212,8 +189,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
     const bool strict = p.seg_chunks == 1;
     const uint32_t a_ring_u32 = ptx::smem_u32(a_ring);
     const uint32_t w_ring_u32 = ptx::smem_u32(w_ring);
-    const uint32_t a_off = (uint32_t)(cw * 64 * TcSmem<KC>::kRowBytes);
-    const uint32_t dy_step = (uint32_t)(g.TW * TcSmem<KC>::kRowBytes);   // one image row of the box: whole 8-row atoms
+    const uint32_t a_off = (uint32_t)(cw * 64 * TcSmem::kRowBytes);
+    const uint32_t dy_step = (uint32_t)(g.TW * TcSmem::kRowBytes);   // one image row of the box: whole 8-row atoms
     // epilogue ownership after the exchange: pixel `row`, chunks [grp * per, grp * per + my_chunks)
     const int row = cw * 64 + (t >> 1);
     const int grp = t & 1;
@@ -221,25 +198,19 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
     const int first_chunk = grp * per;
     const int my_chunks = (nch - first_chunk) < per ? ((nch - first_chunk) > 0 ? nch - first_chunk : 0) : per;
     float* xchg = s_xchg + cw * 64 * kXchgStride;
-    // a slot is released once the wgmma group that last read it has completed (one arrival per warpgroup, by thread 0;
-    // a weight slot in every CTA of the cluster)
+    // a slot is released once the wgmma group that last read it has completed (one arrival per warpgroup, by thread 0)
     auto release_a = [&](int s) { ptx::mbar_arrive_if(&a_empty[s], t == 0); };
-    auto release_w = [&](int s) {
-      if (cs == 1) ptx::mbar_arrive_if(&w_empty[s], t == 0);
-      else
-        for (int r = 0; r < cs; ++r) ptx::mbar_arrive_cluster_if(&w_empty[s], (uint32_t)r, t == 0);
-    };
+    auto release_w = [&](int s) { ptx::mbar_arrive_if(&w_empty[s], t == 0); };
     int as = 0, ws = 0;
     uint32_t a_ph = 0, w_ph = 0;
-    for (int item = cluster_id; item < num_items; item += num_clusters) {
+    for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
       const int n_tile = item % p.n_tiles;
-      const int tile = (item / p.n_tiles) * cs + (int)rank;
-      const bool real = tile < num_tiles;
+      const int tile = item / p.n_tiles;
       const int img = tile / tiles_per_img;
       const int t2 = tile - img * tiles_per_img;
       const int ty = t2 / g.tiles_x, tx = t2 - ty * g.tiles_x;
       const int y = ty * g.TH + py, x = tx * g.TW + px;
-      const bool valid = real && (y < g.H) && (x < g.W);
+      const bool valid = (y < g.H) && (x < g.W);
 
       float sum[N / 2], corr[N / 2], dom[N / 2];
 #pragma unroll
@@ -257,18 +228,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
       int seg_left = p.seg_chunks;  // weight tiles left in the current segment
       int pend_w = -1, pend_a = -1; // slots read by the last committed, not yet completed group
       for (int ch = 0; ch < chunks; ++ch) {
-        int ksteps = p.cin_pad - ch * KC;
-        ksteps = (ksteps > KC ? KC : ksteps) >> 4;
+        int ksteps = p.cin_pad - ch * kTcKC;
+        ksteps = (ksteps > kTcKC ? kTcKC : ksteps) >> 4;
         for (int dx = 0; dx < ksz; ++dx) {
           ptx::mbar_wait(&a_full[as], a_ph);
           const uint32_t a_addr = a_ring_u32 + (uint32_t)as * A_SLOT + a_off;
           for (int dy = 0; dy < ksz; ++dy) {
             ptx::mbar_wait(&w_full[ws], w_ph);
             const uint32_t w_addr = w_ring_u32 + (uint32_t)ws * W_TILE;
-            const uint64_t a_hi = make_smem_desc<KC>(a_addr + (uint32_t)dy * dy_step);
-            const uint64_t a_lo = make_smem_desc<KC>(a_addr + (uint32_t)dy * dy_step + A_PLANE);
-            const uint64_t b_hi = make_smem_desc<KC>(w_addr);
-            const uint64_t b_lo = make_smem_desc<KC>(w_addr + B_BYTES);
+            const uint64_t a_hi = make_smem_desc(a_addr + (uint32_t)dy * dy_step);
+            const uint64_t a_lo = make_smem_desc(a_addr + (uint32_t)dy * dy_step + A_PLANE);
+            const uint64_t b_hi = make_smem_desc(w_addr);
+            const uint64_t b_lo = make_smem_desc(w_addr + B_BYTES);
             const bool a_done = dy == ksz - 1;   // last tap that reads this activation slot
             if (strict) {
               // every 16-channel K slice (its three products) is promoted on its own
@@ -285,13 +256,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
               if (a_done) release_a(as);
             } else {
               // one straight-line batch per K-slice count: a branch inside a batch makes ptxas serialise the wgmma
-              if (ksteps == KC / 16)
-                tile_products<N, NPLANES, KC / 16>(corr, dom, a_hi, a_lo, b_hi, b_lo, acc_on);
+              if (ksteps == 4)
+                tile_products<N, NPLANES, 4>(corr, dom, a_hi, a_lo, b_hi, b_lo, acc_on);
               else if (ksteps == 1)
                 tile_products<N, NPLANES, 1>(corr, dom, a_hi, a_lo, b_hi, b_lo, acc_on);
-              else if (KC == 64 && ksteps == 2)
+              else if (ksteps == 2)
                 tile_products<N, NPLANES, 2>(corr, dom, a_hi, a_lo, b_hi, b_lo, acc_on);
-              else if (KC == 64)
+              else
                 tile_products<N, NPLANES, 3>(corr, dom, a_hi, a_lo, b_hi, b_lo, acc_on);
               acc_on = 1;
               const bool item_end = a_done && dx == ksz - 1 && ch == chunks - 1;
@@ -373,7 +344,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
   }
 
   __syncthreads();
-  if (cs > 1) ptx::cluster_sync();  // nobody exits while a peer may still signal its barriers
 }
 
 }  // namespace dcscn

@@ -20,7 +20,6 @@
 #include "common.h"
 #include "conv_aux.cuh"
 #include "conv_tc.cuh"
-#include "conv_ds.cuh"
 #include "conv_ds_tile.cuh"
 #include "train.cuh"
 #include "wgrad_tc.cuh"
@@ -86,7 +85,7 @@ struct TcLayer {
   float* d_alpha = nullptr;
   float* d_wref = nullptr;      // fp32 HWIO for the validation kernel
   int* d_in_map = nullptr;
-  int packed_kc = 0, packed_planes = 0;
+  int packed_planes = 0;
   int* d_img_map = nullptr;     // training: flat parameter index behind every hi-plane element of d_wpack (-1 = zero)
   size_t img_map_n = 0;
 };
@@ -158,9 +157,7 @@ struct dcscn_handle {
   double* ensio_y = nullptr;
   size_t ensio_cap = 0;
   int l1_loss = 0;                   // --use_l1_loss: image_loss = mean |y_ - y| (DCSCN.py:342-344)
-  int wgrad_taps = 0;                // 0 = automatic (up to 2 filter taps per wgrad CTA), else the cap
   int wgrad_impl = 0;                // 0 = wgmma (wgrad_tc.cuh), 1 = CUDA cores (validation)
-  int host_repack = 0;               // option: always re-pack on the host after an update (validation of the device path)
   bool shadow_mode = false;          // P() returns index-coded shadows (build_refresh_maps)
   bool refresh_ready = false;        // device-side weight refresh maps are valid for the current packing
   std::vector<struct GatherJob> gather_jobs;
@@ -200,8 +197,6 @@ struct dcscn_handle {
   struct DsDev { float *dw = nullptr, *pw = nullptr, *bias = nullptr, *alpha = nullptr; };
   std::vector<DsDev> ds;             // same order as `layers`
   DsDev ds_ab;                       // fused A1 | B1 1x1 layer of the tile kernels: [concat positions][A1 cols | B1 cols], scales folded
-  int ds_impl = 0;                   // 0 = tile kernels (conv_ds_tile.cuh), 1 = first-generation kernels (cross-check)
-  int ds_cache = 1;                  // option "ds_cache": pixel-shuffler layers keep their depthwise values across column groups
   float *ds_feat = nullptr, *ds_b1 = nullptr, *ds_nin = nullptr, *ds_mid = nullptr, *ds_hr = nullptr;
   int ds_total = 0;                  // channels of the (unpadded) concat buffer
   int ds_n = 0, ds_h = 0, ds_w = 0;  // geometry of the last DS forward
@@ -209,17 +204,14 @@ struct dcscn_handle {
 
   std::vector<std::unique_ptr<Plan>> plans;
   Plan* last_plan = nullptr;
-  int gather_impl = 0;               // option "gather_impl": 0 = four pixels per thread when the shape allows, 1 = generic kernel
   int use_graph = 1;                 // option "graph": replay the per-(n,h,w) launch sequence of a forward as one CUDA graph
   uint64_t graph_epoch = 1;          // bumped by everything a captured launch bakes in (options, weight re-packs)
   cudaStream_t cap_stream = nullptr; // capture happens on a private stream (the caller's may be the legacy default stream)
   int64_t graph_replays = 0;
 
   int conv_impl = 0;
-  int kc = 64;
   int seg_chunks = 0;                // pipeline stages per fp32-promotion segment; 0 = automatic
   int act_grad_impl = 0;             // 0: 16-byte activation-gradient kernel, 1: channel-pair kernel (cross-check)
-  int cluster = 1;                   // CTAs per cluster multicasting the weight tiles (single-CTA kernel)
   int timing = 0;
   int fuse_last = 1;                 // fold the per-pixel half of R-CNN1 into the last Up-PS epilogue
   std::vector<cudaEvent_t> ev;       // timing events (launch boundaries of the last forward)
@@ -383,11 +375,10 @@ static void choose_tiling(int n_total_pad16, int* n_tiles, int* n_pad, int cap =
 }
 
 // Values (unscaled fp32) of the operand image of a layer, one per hi-plane element, in image order:
-// [n_tile][tap][chunk][n_pad rows x KC halves], the shared-memory image of a K-major swizzled wgmma operand tile
-// (16-byte chunk j of row r at chunk j ^ f(r); SW128: f = r & 7, SW64: f = (r >> 1) & 3).
-static void tile_image(const TcLayer& t, int KC, std::vector<float>& img) {
-  const int taps = t.ksz * t.ksz, chunks = (t.cin_pad + KC - 1) / KC, n_total = t.n_tiles * t.n_pad;
-  const int row_chunks = KC / 8;
+// [n_tile][tap][chunk][n_pad rows x 64 halves], the shared-memory image of a K-major SWIZZLE_128B wgmma operand tile
+// (16-byte chunk j of row r at chunk j ^ (r & 7)).
+static void tile_image(const TcLayer& t, std::vector<float>& img) {
+  const int taps = t.ksz * t.ksz, chunks = (t.cin_pad + kTcKC - 1) / kTcKC, n_total = t.n_tiles * t.n_pad;
   std::vector<float> wq((size_t)taps * t.cin_pad * n_total, 0.f);   // dense, channel-position-indexed  Wq[tap][q][n]
   for (int tp = 0; tp < taps; ++tp)
     for (int ci = 0; ci < t.cin; ++ci) {
@@ -395,7 +386,7 @@ static void tile_image(const TcLayer& t, int KC, std::vector<float>& img) {
       for (int co = 0; co < t.cout; ++co)
         wq[((size_t)tp * t.cin_pad + q) * n_total + co] = t.w_host[((size_t)tp * t.cin + ci) * t.cout + co];
     }
-  const size_t tile_elems = (size_t)t.n_pad * KC;
+  const size_t tile_elems = (size_t)t.n_pad * kTcKC;
   img.assign((size_t)t.n_tiles * taps * chunks * tile_elems, 0.f);
   for (int nt = 0; nt < t.n_tiles; ++nt)
     for (int tp = 0; tp < taps; ++tp)
@@ -403,26 +394,25 @@ static void tile_image(const TcLayer& t, int KC, std::vector<float>& img) {
         float* base = img.data() + (((size_t)nt * taps + tp) * chunks + ch) * tile_elems;
         for (int r = 0; r < t.n_pad; ++r) {
           const int n = nt * t.n_pad + r;
-          const int sw = (KC == 64) ? (r & 7) : ((r >> 1) & 3);
-          for (int kk = 0; kk < KC; ++kk) {
-            const int q = ch * KC + kk;
-            if (q < t.cin_pad) base[(size_t)r * KC + (size_t)(((kk / 8) ^ sw) % row_chunks) * 8 + kk % 8] = wq[((size_t)tp * t.cin_pad + q) * n_total + n];
+          const int sw = r & 7;
+          for (int kk = 0; kk < kTcKC; ++kk) {
+            const int q = ch * kTcKC + kk;
+            if (q < t.cin_pad) base[(size_t)r * kTcKC + (size_t)((kk / 8) ^ sw) * 8 + kk % 8] = wq[((size_t)tp * t.cin_pad + q) * n_total + n];
           }
         }
       }
 }
 
 static int pack_tc_layer(dcscn_handle* h, TcLayer& t) {
-  const int KC = h->kc;
   const int NPL = planes(h);
   float maxw = 0.f;
   for (float v : t.w_host) maxw = std::max(maxw, std::fabs(v));
   t.wscale = 1.f;
   if (maxw > 0.f) t.wscale = std::ldexp(1.0f, (int)std::floor(std::log2(16384.0 / (double)maxw)));
 
-  const size_t tile_elems = (size_t)t.n_pad * KC;
+  const size_t tile_elems = (size_t)t.n_pad * kTcKC;
   std::vector<float> img;
-  tile_image(t, KC, img);
+  tile_image(t, img);
   std::vector<__half> pack(img.size() * NPL);
   for (size_t i = 0; i < img.size(); ++i) {
     const size_t blk = i / tile_elems, pos = i - blk * tile_elems;
@@ -436,7 +426,6 @@ static int pack_tc_layer(dcscn_handle* h, TcLayer& t) {
   if (upload(&t.d_alpha, t.alpha_host, h)) return 1;
   if (upload(&t.d_wref, t.w_host, h)) return 1;
   if (upload(&t.d_in_map, t.in_map, h)) return 1;
-  t.packed_kc = KC;
   t.packed_planes = NPL;
   return 0;
 }
@@ -524,18 +513,15 @@ static int finalize_params_ds(dcscn_handle* h) {
     const std::vector<float>& dwv = P(h, l.scope + "/depthwise_W");   // [k,k,cin,1] == [taps][cin]
     const std::vector<float>& pwv = P(h, l.scope + "/pointwise_W");   // [1,1,cin,cout] == [cin][cout]
     if (l.scope == "A1" || l.scope == "B1") {
-      // these read the whole concat buffer: spread their rows over the 4-aligned slot positions
-      std::vector<float> dwp((size_t)l.k * l.k * T, 0.f), pwp((size_t)T * l.cout, 0.f);
+      // both run as the one fused layer ds_ab over the whole concat buffer: their rows go to the 4-aligned slot
+      // positions, with the per-channel depthwise scale folded in
       const int col0 = l.scope == "A1" ? 0 : na;
       int ci = 0;
       for (int li = 0; li < L; ++li)
         for (int k = 0; k < h->filters[li]; ++k, ++ci) {
           const int pos = h->ds_off[li] + k;
-          for (int t = 0; t < l.k * l.k; ++t) dwp[(size_t)t * T + pos] = dwv[(size_t)t * l.cin + ci];
-          for (int co = 0; co < l.cout; ++co) {
-            pwp[(size_t)pos * l.cout + co] = pwv[(size_t)ci * l.cout + co];
+          for (int co = 0; co < l.cout; ++co)
             if (l.k == 1) ab_pw[(size_t)pos * (na + nb) + col0 + co] = dwv[ci] * pwv[(size_t)ci * l.cout + co];
-          }
         }
       const auto& B = P(h, l.scope + "/conv_B");
       const auto& A = P(h, l.scope + "/prelu/" + base + "_prelu");
@@ -543,10 +529,9 @@ static int finalize_params_ds(dcscn_handle* h) {
         ab_bias[col0 + co] = B[co];
         ab_alpha[col0 + co] = A[co];
       }
-      if (upload(&h->ds[i].dw, dwp, h) || upload(&h->ds[i].pw, pwp, h)) return 1;
-    } else {
-      if (upload(&h->ds[i].dw, dwv, h) || upload(&h->ds[i].pw, pwv, h)) return 1;
+      continue;
     }
+    if (upload(&h->ds[i].dw, dwv, h) || upload(&h->ds[i].pw, pwv, h)) return 1;
     if (l.bias && upload(&h->ds[i].bias, P(h, l.scope + "/conv_B"), h)) return 1;
     if (l.prelu && upload(&h->ds[i].alpha, P(h, l.scope + "/prelu/" + base + "_prelu"), h)) return 1;
   }
@@ -739,21 +724,21 @@ constexpr size_t kTcRingBudget = 227 * 1024 - 1024 - kTcBarrierBytes - kRdotSmem
 // Whether a k x k layer (k > 1) can run on a TH x TW patch: its ky taps are read at row offsets of TW pixels inside one
 // activation box of TW x (TH + k - 1) pixels, which the swizzled operand descriptors allow only in whole 8-row atoms (TW
 // a multiple of 8), and two such boxes plus two weight tiles must fit in shared memory.
-static bool tc_patch_fits(int KC, int nplanes, int n_pad, int ksz, int TH, int TW) {
+static bool tc_patch_fits(int nplanes, int n_pad, int ksz, int TH, int TW) {
   if (ksz == 1) return true;
   if (TW % 8 != 0) return false;
-  return 2 * (size_t)nplanes * tc_a_plane_bytes(KC, TW, TH, ksz) + 2 * (size_t)tc_w_tile_bytes(KC, nplanes, n_pad) <=
+  return 2 * (size_t)nplanes * tc_a_plane_bytes(TW, TH, ksz) + 2 * (size_t)tc_w_tile_bytes(nplanes, n_pad) <=
          kTcRingBudget;
 }
 
 // 128-pixel rectangular patches; minimise padded area, prefer wide patches (contiguous TMA rows).  Returns false when no
 // patch suits the layer.
-static bool choose_patch(int H, int W, int KC, int nplanes, int n_pad, int ksz, int* TH, int* TW) {
+static bool choose_patch(int H, int W, int nplanes, int n_pad, int ksz, int* TH, int* TW) {
   static const int cand[][2] = {{8, 16}, {4, 32}, {16, 8}, {2, 64}, {32, 4}, {1, 128}, {64, 2}, {128, 1}};
   long long best = -1;
   for (auto& c : cand) {
     const int th = c[0], tw = c[1];
-    if (!tc_patch_fits(KC, nplanes, n_pad, ksz, th, tw)) continue;
+    if (!tc_patch_fits(nplanes, n_pad, ksz, th, tw)) continue;
     long long area = (long long)((H + th - 1) / th) * th * ((W + tw - 1) / tw) * tw;
     if (best < 0 || area < best) {
       best = area;
@@ -764,16 +749,15 @@ static bool choose_patch(int H, int W, int KC, int nplanes, int n_pad, int ksz, 
   return best >= 0;
 }
 
+// Tensor map of an NHWC fp16 plane whose boxes are 64 channels x TW x TH pixels, swizzled as the wgmma operands expect.
 static int encode_map(dcscn_handle* h, CUtensorMap* tm, const __half* base, int cin_pad, int pitch, int n, int H,
-                      int W, int TH, int TW, int kc_override = 0) {
-  const int KC = kc_override ? kc_override : h->kc;
+                      int W, int TH, int TW) {
   cuuint64_t dims[4] = {(cuuint64_t)cin_pad, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)n};
   cuuint64_t strides[3] = {(cuuint64_t)pitch * 2, (cuuint64_t)W * pitch * 2, (cuuint64_t)H * W * pitch * 2};
-  cuuint32_t box[4] = {(cuuint32_t)KC, (cuuint32_t)TW, (cuuint32_t)TH, 1};
+  cuuint32_t box[4] = {(cuuint32_t)kTcKC, (cuuint32_t)TW, (cuuint32_t)TH, 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
   CUresult r = h->encode(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, (void*)base, dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         KC == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
     return fail("cuTensorMapEncodeTiled failed (%d) cin_pad=%d pitch=%d n=%d H=%d W=%d box=%dx%d", (int)r, cin_pad,
@@ -786,10 +770,10 @@ static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, const __ha
   TcLaunch L;
   memset(&L, 0, sizeof(L));
   int TH = 0, TW = 0;
-  if (!choose_patch(H, W, h->kc, planes(h), t.n_pad, t.ksz, &TH, &TW))
+  if (!choose_patch(H, W, planes(h), t.n_pad, t.ksz, &TH, &TW))
     return fail("layer %s: no pixel patch fits a %dx%d filter in shared memory", t.name.c_str(), t.ksz, t.ksz);
   // the kernel's ky taps start TW pixels apart inside the box: whole 8-row swizzle atoms, or the operands are misread
-  if (t.ksz > 1 && (TW * h->kc * 2) % (8 * h->kc * 2) != 0)
+  if (t.ksz > 1 && TW % 8 != 0)
     return fail("internal: layer %s: patch width %d is not a whole number of swizzle atoms", t.name.c_str(), TW);
   ConvGeom g{n, H, W, (W + TW - 1) / TW, (H + TH - 1) / TH, TW, TH};
   const int box_rows = TH + t.ksz - 1;   // a k x k layer's box carries the rows of all k ky taps
@@ -802,15 +786,12 @@ static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, const __ha
   L.p.g = g;
   L.p.ksz = t.ksz;
   L.p.cin_pad = t.cin_pad;
-  L.p.chunks = (t.cin_pad + h->kc - 1) / h->kc;
+  L.p.chunks = (t.cin_pad + kTcKC - 1) / kTcKC;
   L.p.n_tiles = t.n_tiles;
   L.p.n_pad = t.n_pad;
   // weight tiles per promotion segment; 1 = promote every 16-channel K slice.  The automatic lengths keep the dominant
   // chain as short as the earlier two-pass scheme had it (2 tiles for wide layers, 3 for thin ones).
   L.p.seg_chunks = h->seg_chunks > 0 ? h->seg_chunks : (t.n_pad > 64 ? 2 : 3);
-  int cs = h->cluster;
-  while (cs > 1 && (t.n_pad % cs != 0 || h->sm_count % cs != 0)) cs >>= 1;
-  L.p.cluster_size = cs;
   L.p.wpack = t.d_wpack;
   L.p.epi = epi;
   L.p.epi.bias = t.d_bias;
@@ -829,8 +810,8 @@ static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, const __ha
   // Ring depths.  The consumers release a slot one weight tile late, so each ring needs at least two slots.  A k x k layer
   // reads k weight tiles per activation slot: three activation slots when four weight tiles still fit, else two.
   // A 1x1 layer pairs one activation slot with one weight tile.
-  const size_t a_slot = (size_t)planes(h) * tc_a_plane_bytes(h->kc, TW, TH, t.ksz);
-  const size_t w_tile = tc_w_tile_bytes(h->kc, planes(h), t.n_pad);
+  const size_t a_slot = (size_t)planes(h) * tc_a_plane_bytes(TW, TH, t.ksz);
+  const size_t w_tile = tc_w_tile_bytes(planes(h), t.n_pad);
   const size_t budget = kTcRingBudget;
   int a_slots, w_slots;
   if (t.ksz == 1) {
@@ -847,8 +828,8 @@ static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, const __ha
   L.w_slots = w_slots;
   L.smem = a_slots * a_slot + w_slots * w_tile + 1024 + kTcBarrierBytes + kRdotSmemBytes + kXchgBytes;
   const long long tiles = (long long)n * g.tiles_x * g.tiles_y;
-  const long long items = ((tiles + cs - 1) / cs) * t.n_tiles;    // cluster iterations
-  L.grid = (int)std::min<long long>(items, h->sm_count / cs) * cs;
+  const long long items = tiles * t.n_tiles;
+  L.grid = (int)std::min<long long>(items, h->sm_count);
 
   // validation twin
   L.ref.g = g;
@@ -994,42 +975,30 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
 }
 
 // ------------------------------------------------------------------------------------- forward ----
-template <int KC, int NPL, int N>
+template <int NPL, int N>
 static int launch_tc_inst(dcscn_handle* h, const TcLaunch& L, cudaStream_t st) {
   static bool attr_set_dev[64] = {};   // function attributes are per device
   bool& attr_set = attr_set_dev[h->cfg.device_id & 63];
   if (!attr_set) {
-    CUDA_TRY(cudaFuncSetAttribute(conv_tc_kernel<KC, NPL, N>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    CUDA_TRY(cudaFuncSetAttribute(conv_tc_kernel<NPL, N>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_set = true;
   }
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(L.grid);
-  cfg.blockDim = dim3(kTcThreads);
-  cfg.dynamicSmemBytes = L.smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = L.p.cluster_size;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = L.p.cluster_size > 1 ? 1 : 0;
-  CUDA_TRY(cudaLaunchKernelEx(&cfg, conv_tc_kernel<KC, NPL, N>, L.tm_hi, L.tm_lo, L.p, L.a_slots, L.w_slots));
+  conv_tc_kernel<NPL, N><<<L.grid, kTcThreads, L.smem, st>>>(L.tm_hi, L.tm_lo, L.p, L.a_slots, L.w_slots);
+  CUDA_TRY(cudaGetLastError());
   return 0;
 }
 
 // The column-tile width is a template parameter of the kernel (the wgmma width is an immediate of the instruction).
-template <int KC, int NPL>
+template <int NPL>
 static int launch_tc_width(dcscn_handle* h, const TcLaunch& L, cudaStream_t st) {
   switch (L.p.n_pad) {
-    case 16: return launch_tc_inst<KC, NPL, 16>(h, L, st);
-    case 32: return launch_tc_inst<KC, NPL, 32>(h, L, st);
-    case 48: return launch_tc_inst<KC, NPL, 48>(h, L, st);
-    case 64: return launch_tc_inst<KC, NPL, 64>(h, L, st);
-    case 80: return launch_tc_inst<KC, NPL, 80>(h, L, st);
-    case 96: return launch_tc_inst<KC, NPL, 96>(h, L, st);
-    case 112: return launch_tc_inst<KC, NPL, 112>(h, L, st);
+    case 16: return launch_tc_inst<NPL, 16>(h, L, st);
+    case 32: return launch_tc_inst<NPL, 32>(h, L, st);
+    case 48: return launch_tc_inst<NPL, 48>(h, L, st);
+    case 64: return launch_tc_inst<NPL, 64>(h, L, st);
+    case 80: return launch_tc_inst<NPL, 80>(h, L, st);
+    case 96: return launch_tc_inst<NPL, 96>(h, L, st);
+    case 112: return launch_tc_inst<NPL, 112>(h, L, st);
   }
   return fail("internal: column tile width %d is not a multiple of 16 in [16, %d]", L.p.n_pad, kMaxTileN);
 }
@@ -1052,8 +1021,7 @@ static int launch_tc(dcscn_handle* h, const TcLaunch& Lc, cudaStream_t st) {
   }
   const int npl = planes(h);
   if (L.p.wpack == nullptr) return fail("internal: weight image was not packed for this layer");
-  if (h->kc == 64) return npl == 2 ? launch_tc_width<64, 2>(h, L, st) : launch_tc_width<64, 1>(h, L, st);
-  return npl == 2 ? launch_tc_width<32, 2>(h, L, st) : launch_tc_width<32, 1>(h, L, st);
+  return npl == 2 ? launch_tc_width<2>(h, L, st) : launch_tc_width<1>(h, L, st);
 }
 
 static int mark(dcscn_handle* h, cudaStream_t st) {
@@ -1067,40 +1035,7 @@ static int mark(dcscn_handle* h, cudaStream_t st) {
   return 0;
 }
 
-static int mark(dcscn_handle* h, cudaStream_t st);
-static int launch_ds(dcscn_handle* h, const LayerDef& l, const dcscn_handle::DsDev& d, const float* src, int src_pitch,
-                     float* dst, int dst_pitch, int dst_off, int n, int H, int W, int d2s_r, int d2s_cout,
-                     const float* add, cudaStream_t st) {
-  DsLayerParams p;
-  memset(&p, 0, sizeof(p));
-  p.n_img = n; p.H = H; p.W = W; p.ksz = l.k; p.cin = l.cin; p.cout = l.cout;
-  p.src = src; p.src_pitch = src_pitch; p.dw = d.dw; p.pw = d.pw; p.bias = d.bias; p.alpha = d.alpha;
-  p.dst = dst; p.dst_pitch = dst_pitch; p.dst_off = dst_off; p.d2s_r = d2s_r; p.d2s_cout = d2s_cout; p.add = add;
-  if (l.k != 1 && l.k != 3) return fail("depthwise-separable layer %s: kernel size %d is not supported (1 or 3)", l.scope.c_str(), l.k);
-  const long long total = (long long)n * H * W;
-  if (l.cin == 1 && l.cout == 1 && d2s_r == 0 && total < (1ll << 32)) {
-    const int grid = (int)std::min<long long>((total + 255) / 256, (long long)h->sm_count * 16);
-    if (l.k == 3) ds_single_kernel<3><<<grid, 256, 0, st>>>(p); else ds_single_kernel<1><<<grid, 256, 0, st>>>(p);
-  } else {
-    const size_t smem = ds_smem_bytes(l.k, l.cin, l.cout);
-    if (smem > 200 * 1024) return fail("depthwise-separable layer %s: %d -> %d channels exceed the kernel's shared memory", l.scope.c_str(), l.cin, l.cout);
-    static size_t ds_smem_attr_dev[64] = {};  // current opt-in limit of the DS kernels per device (only ever raised)
-    size_t& ds_smem_attr = ds_smem_attr_dev[h->cfg.device_id & 63];
-    if (ds_smem_attr == 0) ds_smem_attr = 48 * 1024;
-    if (smem > ds_smem_attr) {   // raise the opt-in limit only as far as needed (keeps the L1 carve-out large)
-      CUDA_TRY(cudaFuncSetAttribute(ds_layer_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      CUDA_TRY(cudaFuncSetAttribute(ds_layer_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      ds_smem_attr = smem;
-    }
-    const unsigned grid = (unsigned)((total + kDsPix - 1) / kDsPix);
-    if (l.k == 3) ds_layer_kernel<3><<<grid, kDsThreads, smem, st>>>(p); else ds_layer_kernel<1><<<grid, kDsThreads, smem, st>>>(p);
-  }
-  CUDA_TRY(cudaGetLastError());
-  h->launches++;
-  return mark(h, st);
-}
-
-// ---- second-generation depthwise-separable kernels (conv_ds_tile.cuh) ----
+// ---- depthwise-separable kernels (conv_ds_tile.cuh) ----
 template <int KSZ>
 static int launch_ds_tile_k(dcscn_handle* h, const DsTileParams& p, unsigned grid, size_t smem, cudaStream_t st) {
   const int cols = p.cout < 32 ? ((p.cout + 3) & ~3) : 32;
@@ -1132,8 +1067,7 @@ static int launch_ds_tile(dcscn_handle* h, DsTileParams p, int ksz, cudaStream_t
   // the kernel's shared-memory carve-up uses the per-pass column count of the instantiated template
   const int tcols = cols <= 4 ? 4 : cols <= 8 ? 8 : cols <= 16 ? 16 : cols <= 24 ? 24 : 32;
   const size_t in_px = ksz == 3 ? (size_t)(kDtT + 2) * kDtS : (size_t)kDtThreads;
-  p.cache_u = (h->ds_cache && ds_tile_caches_depthwise(ksz, p.cin, p.cout)) ? 1 : 0;
-  const size_t cache = p.cache_u ? (size_t)kDtThreads * kDtCP : 0;   // private depthwise rows
+  const size_t cache = ds_tile_caches_depthwise(ksz, p.cin, p.cout) ? (size_t)kDtThreads * kDtCP : 0;   // private depthwise rows
   const size_t smem = (in_px * kDtCP + (size_t)p.cin * tcols + (size_t)ksz * ksz * p.cin + cache) * sizeof(float);
   if (smem > 200 * 1024) return fail("depthwise-separable layer %d -> %d exceeds the kernel's shared memory", p.cin, p.cout);
   unsigned grid;
@@ -1160,6 +1094,7 @@ static DsTileParams ds_tile_params(const LayerDef& l, const dcscn_handle::DsDev&
   return p;
 }
 
+// Depthwise-separable graph (DCSCN.py:246-249, 264-271, 318-320; tf_graph.py:240-243): fp32 NHWC, CUDA cores.
 static int forward_ds_tile(dcscn_handle* h, const float* x, const float* x2, float* y, int n, int H, int W, cudaStream_t st) {
   const dcscn_config& c = h->cfg;
   const int L = c.layers, T = h->ds_total, na = c.nin_filters, nb = c.nin_filters2, cps = na + nb;
@@ -1215,61 +1150,23 @@ static int forward_ds_tile(dcscn_handle* h, const float* x, const float* x2, flo
   // R-CNN1 (no bias / activation) + x2
   const LayerDef& lr = h->layers[li];
   const dcscn_handle::DsDev& d = h->ds[li];
-  const long long total = (long long)n * HH * WW;
-  if (lr.cin == 1 && lr.cout == 1 && lr.k == 3 && (WW & 3) == 0 && total < (1ll << 32) &&
-      ((reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(x2)) & 15) == 0) {
-    const int grid = (int)std::min<long long>((total / 4 + 255) / 256, (long long)h->sm_count * 16);
-    ds_single4_kernel<<<grid, 256, 0, st>>>(h->ds_hr, x2, y, n, HH, WW, d.dw, d.pw, d.bias, d.alpha);
+  if (lr.cin == 1 && lr.cout == 1) {
+    if (lr.k != 1 && lr.k != 3) return fail("depthwise-separable R-CNN1: kernel size %d is not supported (1 or 3)", lr.k);
+    const long long total = (long long)n * HH * WW;
+    // four pixels per thread when the row width and the x2 / y alignment allow it, else one
+    const bool vec4 = lr.k == 3 && (WW & 3) == 0 && total < (1ll << 32) &&
+                      ((reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(x2)) & 15) == 0;
+    const int grid = (int)std::min<long long>(((vec4 ? total / 4 : total) + 255) / 256, (long long)h->sm_count * 16);
+    if (vec4) ds_single4_kernel<<<grid, 256, 0, st>>>(h->ds_hr, x2, y, n, HH, WW, d.dw, d.pw, d.bias, d.alpha);
+    else if (lr.k == 3) ds_single_kernel<3><<<grid, 256, 0, st>>>(h->ds_hr, x2, y, n, HH, WW, d.dw, d.pw, d.bias, d.alpha);
+    else ds_single_kernel<1><<<grid, 256, 0, st>>>(h->ds_hr, x2, y, n, HH, WW, d.dw, d.pw, d.bias, d.alpha);
     CUDA_TRY(cudaGetLastError());
     h->launches++;
     return mark(h, st);
   }
-  if (lr.cin == 1 && lr.cout == 1) return launch_ds(h, lr, d, h->ds_hr, h->ps_out, y, 1, 0, n, HH, WW, 0, 0, x2, st);
   DsTileParams p = ds_tile_params(lr, d, h->ds_hr, h->ps_out, y, 1, 0, n, HH, WW);
   p.add = x2;
   return launch_ds_tile(h, p, lr.k, st);
-}
-
-// Depthwise-separable graph (DCSCN.py:246-249, 264-271, 318-320; tf_graph.py:240-243): fp32 NHWC, CUDA cores.
-static int forward_ds(dcscn_handle* h, const float* x, const float* x2, float* y, int n, int H, int W, cudaStream_t st) {
-  if (h->ds_impl == 0) return forward_ds_tile(h, x, x2, y, n, H, W, st);
-  const dcscn_config& c = h->cfg;
-  const int L = c.layers, T = h->ds_total, cps = c.nin_filters + c.nin_filters2;
-  h->ev_used = 0;
-  if (mark(h, st)) return 1;
-  size_t li = 0;
-  for (int i = 0; i < L; ++i, ++li) {
-    const float* src = i == 0 ? x : h->ds_feat + h->ds_off[i - 1];
-    if (launch_ds(h, h->layers[li], h->ds[li], src, i == 0 ? c.channels : T, h->ds_feat, T, h->ds_off[i], n, H, W, 0, 0, nullptr, st)) return 1;
-  }
-  LayerDef la = h->layers[li], lb = h->layers[li + 1];
-  la.cin = lb.cin = T;   // their filters are spread over the 4-aligned concat positions (finalize_params_ds)
-  if (launch_ds(h, la, h->ds[li], h->ds_feat, T, h->ds_nin, cps, c.nin_filters2, n, H, W, 0, 0, nullptr, st)) return 1;  // A1
-  ++li;
-  if (launch_ds(h, lb, h->ds[li], h->ds_feat, T, h->ds_b1, c.nin_filters2, 0, n, H, W, 0, 0, nullptr, st)) return 1;     // B1
-  ++li;
-  if (launch_ds(h, h->layers[li], h->ds[li], h->ds_b1, c.nin_filters2, h->ds_nin, cps, 0, n, H, W, 0, 0, nullptr, st)) return 1;     // B2
-  ++li;
-  int HH = H, WW = W;
-  if (c.scale == 4) {
-    if (launch_ds(h, h->layers[li], h->ds[li], h->ds_nin, cps, h->ds_mid, cps, 0, n, H, W, 2, cps, nullptr, st)) return 1;           // Up-PS
-    ++li;
-    HH = 2 * H; WW = 2 * W;
-    if (launch_ds(h, h->layers[li], h->ds[li], h->ds_mid, cps, h->ds_hr, h->ps_out, 0, n, HH, WW, 2, h->ps_out, nullptr, st)) return 1;  // Up-PS2
-    ++li;
-    HH *= 2; WW *= 2;
-  } else {
-    if (launch_ds(h, h->layers[li], h->ds[li], h->ds_nin, cps, h->ds_hr, h->ps_out, 0, n, H, W, c.scale, h->ps_out, nullptr, st)) return 1;
-    ++li;
-    HH = c.scale * H; WW = c.scale * W;
-  }
-  // R-CNN1 (no bias / activation) + x2
-  if (h->wait_x2) {
-    CUDA_TRY(cudaStreamWaitEvent(st, h->x2_ready, 0));
-    h->wait_x2 = false;
-  }
-  if (launch_ds(h, h->layers[li], h->ds[li], h->ds_hr, h->ps_out, y, 1, 0, n, HH, WW, 0, 0, x2, st)) return 1;
-  return 0;
 }
 
 // CNN1 and the tensor-core layers of one forward, in execution order, on `st` (a capturing stream when the plan's graph is
@@ -1309,7 +1206,7 @@ static int forward_impl(dcscn_handle* h, const float* x, const float* x2, float*
   if (ensure_workspace(h, (size_t)n * H * W)) return 1;
   if (h->cfg.depthwise_separable) {
     h->ds_n = n; h->ds_h = H; h->ds_w = W;
-    return forward_ds(h, x, x2, y, n, H, W, st);
+    return forward_ds_tile(h, x, x2, y, n, H, W, st);
   }
   Plan* pl = get_plan(h, n, H, W);
   if (!pl) return 1;
@@ -1358,7 +1255,7 @@ static int forward_impl(dcscn_handle* h, const float* x, const float* x2, float*
     p.x2 = x2;
     p.y = y;
     const size_t total = (size_t)p.n_img * p.H * p.W;
-    const bool vec4 = p.ksz == 3 && (p.W & 3) == 0 && ((reinterpret_cast<uintptr_t>(x2) | reinterpret_cast<uintptr_t>(y)) & 15) == 0 && h->gather_impl == 0;
+    const bool vec4 = p.ksz == 3 && (p.W & 3) == 0 && ((reinterpret_cast<uintptr_t>(x2) | reinterpret_cast<uintptr_t>(y)) & 15) == 0;
     if (vec4) {
       const int grid = (int)std::min<size_t>((total / 4 + 255) / 256, (size_t)h->sm_count * 16);
       conv_last_gather4_kernel<<<grid, 256, 0, st>>>(p);
@@ -1801,34 +1698,9 @@ int dcscn_set_option(dcscn_handle* h, const char* key, int64_t value) {
     h->use_graph = value ? 1 : 0;
     return 0;
   }
-  if (k == "gather_impl") {
-    h->gather_impl = value ? 1 : 0;
-    return 0;
-  }
-  if (k == "ds_cache") {
-    h->ds_cache = value ? 1 : 0;
-    return 0;
-  }
   if (k == "conv_impl") {
     if (value != 0 && value != 1) return fail("conv_impl must be 0 (wgmma) or 1 (CUDA-core validation)");
     h->conv_impl = (int)value;
-  } else if (k == "kc") {
-    if (value != 64 && value != 32) return fail("kc must be 64 or 32");
-    if (h->kc != (int)value) {
-      h->kc = (int)value;
-      h->cap_px = 0;
-      h->params_dirty = true;  // weight tiles depend on KC
-      h->plans.clear();
-      h->last_plan = nullptr;
-    }
-  } else if (k == "ds_impl") {
-    if (value != 0 && value != 1) return fail("ds_impl must be 0 (tile kernels) or 1 (first-generation kernels)");
-    h->ds_impl = (int)value;
-  } else if (k == "cluster") {
-    if (value != 1 && value != 2 && value != 4) return fail("cluster must be 1, 2 or 4");
-    h->cluster = (int)value;
-    h->plans.clear();
-    h->last_plan = nullptr;
   } else if (k == "fuse_last") {
     h->fuse_last = value ? 1 : 0;
   } else if (k == "timing") {
@@ -1838,11 +1710,6 @@ int dcscn_set_option(dcscn_handle* h, const char* key, int64_t value) {
     h->wgrad_impl = (int)value;
   } else if (k == "l1_loss") {
     h->l1_loss = value ? 1 : 0;
-  } else if (k == "wgrad_taps") {
-    if (value < 0 || value > kWgMaxTaps) return fail("wgrad_taps must be 0 (automatic) .. %d", kWgMaxTaps);
-    h->wgrad_taps = (int)value;
-  } else if (k == "host_repack") {
-    h->host_repack = value ? 1 : 0;
   } else if (k == "act_grad_impl") {
     if (value < 0 || value > 1) return fail("act_grad_impl must be 0 or 1");
     h->act_grad_impl = (int)value;
@@ -1872,8 +1739,8 @@ int dcscn_get_timings(dcscn_handle* h, float* ms, int capacity, int* count, char
       s = "";
       for (const LayerDef& l : h->layers) {
         std::string nm = l.scope.substr(0, l.scope.find('/'));
-        if (h->ds_impl == 0 && nm == "B1") continue;          // the tile kernels run A1 | B1 as one launch
-        if (h->ds_impl == 0 && nm == "A1") nm = "A1+B1";
+        if (nm == "B1") continue;          // A1 | B1 run as one launch
+        if (nm == "A1") nm = "A1+B1";
         s += (s.empty() ? "" : ",") + nm;
       }
     } else {

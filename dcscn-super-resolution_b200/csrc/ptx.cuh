@@ -1,5 +1,5 @@
 // Thin inline-PTX wrappers for the sm_90a features the DCSCN kernels use:
-// mbarrier, TMA (cp.async.bulk[.tensor]), clusters, wgmma (mma_async / fence / commit_group / wait_group).
+// mbarrier, TMA (cp.async.bulk[.tensor]), wgmma (mma_async / fence / commit_group / wait_group).
 #pragma once
 #include <cstdint>
 #include <cuda.h>
@@ -31,17 +31,6 @@ __device__ __forceinline__ void setmaxnreg_inc() {
 template <int N>
 __device__ __forceinline__ void setmaxnreg_dec() {
   asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
-}
-
-// ----------------------------------------------------------------- cluster ----
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
 // ---------------------------------------------------------------- mbarrier ----
@@ -99,16 +88,6 @@ __device__ __forceinline__ void bulk_load(void* smem_dst, const void* gsrc, uint
       : "memory");
 }
 
-// Same, delivered to the same shared-memory offset (and mbarrier offset) of every CTA in `cta_mask`.
-__device__ __forceinline__ void bulk_load_multicast(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar,
-                                                    uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::
-          "r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(smem_u32(bar)), "h"(cta_mask)
-      : "memory");
-}
-
 // Releases of a pipeline slot whose readers were wgmma (complete once wgmma.wait_group returns): executed by every
 // thread and predicated on `pred` inside the instruction, so no branch breaks the warp-uniform path of a wgmma sequence
 // in flight (a divergent branch there makes ptxas serialise the wgmma).  Default (.release.cta) semantics: a
@@ -121,19 +100,6 @@ __device__ __forceinline__ void mbar_arrive_if(uint64_t* bar, bool pred) {
       "@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t"
       "}\n" ::"r"(smem_u32(bar)),
       "r"((uint32_t)pred)
-      : "memory");
-}
-// Same, on the mbarrier at the same shared-memory offset in CTA `cta` of this cluster.
-__device__ __forceinline__ void mbar_arrive_cluster_if(uint64_t* bar, uint32_t cta, bool pred) {
-  asm volatile(
-      "{\n\t"
-      ".reg .b32 remote;\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %2, 0;\n\t"
-      "mapa.shared::cluster.u32 remote, %0, %1;\n\t"
-      "@p mbarrier.arrive.shared::cluster.b64 _, [remote];\n\t"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(cta), "r"((uint32_t)pred)
       : "memory");
 }
 

@@ -165,23 +165,15 @@ int dcscn_dropout_mask(dcscn_handle* h, const char* tensor, uint32_t seed, int n
 int dcscn_get_activation(dcscn_handle* h, const char* tensor, float* host_data, int64_t numel);
 
 /* Options: "conv_impl" 0 = wgmma tensor cores (default), 1 = CUDA-core fp32 validation kernels;
- *          "kc" 64 | 32 = K-chunk (channels per pipeline stage) of the tensor-core kernel;
  *          "seg_chunks" = pipeline stages per fp32-promotion segment (default 0 = automatic: 2, or 3 for thin layers);
- *          "cluster" 1 | 2 | 4 = CTAs per cluster multicasting weight tiles in the tensor-core kernel (default 1);
  *          "fuse_last" 1 | 0 = compute the per-pixel half of R-CNN1 inside the last Up-PS epilogue (default 1);
  *          "timing" 0 | 1 = record per-launch CUDA events (see dcscn_get_timings);
- *          "ds_impl" 0 | 1 = depthwise-separable layers on the tile kernels (default) or the first-generation kernels (cross-check);
  *          "act_grad_impl" 0 | 1 = activation gradients with 16-byte (default) or channel-pair accesses (cross-check);
- *          "ds_cache" 1 | 0 = depthwise-separable pixel-shuffler layers keep their depthwise values across column groups;
- *          "gather_impl" 0 | 1 = R-CNN1 gather with four pixels per thread (default where W % 4 == 0) or the generic kernel;
  *          "graph" 1 | 0 = replay the launches of a forward (all but the last kernel) as one CUDA graph per (n, h, w) once
  *          the same input pointer has been seen twice in a row (default 1; off while "timing" = 1 or "conv_impl" = 1);
  *          "l1_loss" 0 | 1 = image_loss of the train step is mean |y_ - y| instead of the MSE (--use_l1_loss,
  *          DCSCN.py:342-344; the returned mse stays the MSE);
- *          "wgrad_impl" 0 | 1 = filter gradients on wgmma tensor cores (default) or on CUDA cores (cross-check);
- *          "wgrad_taps" 0..2 = filter taps per wgrad CTA (0 = automatic);
- *          "host_repack" 0 | 1 = after an optimizer step rebuild the packed tensor-core weight images on the host
- *          (validation of the default device-side refresh). */
+ *          "wgrad_impl" 0 | 1 = filter gradients on wgmma tensor cores (default) or on CUDA cores (cross-check). */
 int dcscn_set_option(dcscn_handle* h, const char* key, int64_t value);
 /* With option "timing" = 1 every launch of a forward is bracketed by CUDA events on its stream; this returns the
  * device time in ms of each launch of the LAST forward (in launch order) and their comma-separated names. */

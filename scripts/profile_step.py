@@ -16,7 +16,7 @@ prec = E.PRECISION_F16X1 if (len(sys.argv) > 3 and sys.argv[3] == "f16x1") else 
 eng = E.Engine(E.make_config(precision=prec))
 eng.set_params(bench.load_weights())
 eng.set_option("graph", 0)                      # one kernel launch per layer for ncu's -k / -s / -c filters
-for kv in filter(None, os.environ.get("DCSCN_OPTS", "").split(",")):   # e.g. DCSCN_OPTS=cluster=2,seg_chunks=1
+for kv in filter(None, os.environ.get("DCSCN_OPTS", "").split(",")):   # e.g. DCSCN_OPTS=seg_chunks=1,fuse_last=0
     k, v = kv.split("=")
     eng.set_option(k, int(v))
 g = torch.Generator().manual_seed(0)

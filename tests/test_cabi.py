@@ -60,8 +60,12 @@ def test_every_option_key_is_documented_in_the_header():
     body = src[src.index("int dcscn_set_option("):]
     body = body[:body.index("\nint dcscn_get_timings")] if "\nint dcscn_get_timings" in body else body[:6000]
     keys = set(re.findall(r'k == "([a-z_0-9]+)"', body))
-    assert {"graph", "fuse_last", "cluster", "seg_chunks", "conv_impl", "timing"} <= keys
+    assert {"graph", "fuse_last", "seg_chunks", "conv_impl", "timing"} <= keys
     header = open(os.path.join(ROOT, "include", "dcscn_b200.h")).read()
     doc = header[header.index("int dcscn_set_option") - 6000:header.index("int dcscn_set_option")]
     documented = set(re.findall(r'"([a-z_0-9]+)"', doc))
     assert keys <= documented, sorted(keys - documented)
+    # the other way round: the header's option list names no key the engine refuses (e.g. one that was removed)
+    options = header[header.index("/* Options:"):header.index("int dcscn_set_option")]
+    listed = set(re.findall(r'"([a-z_0-9]+)"', options))
+    assert listed <= keys, sorted(listed - keys)
