@@ -155,6 +155,7 @@ class SuperResolution:
 
         self.batch_dir = flags.batch_dir
         self.precision = getattr(flags, "precision", "f16x3")
+        self.workspace_mb = getattr(flags, "workspace_mb", 0)
 
         self.name = self.get_model_name(model_name)
         self.total_epochs = 0
@@ -250,6 +251,8 @@ class SuperResolution:
     def build_graph(self):
         """DCSCN.py:222-332: creates the engine (variables at their initial values) and the bookkeeping strings."""
         self.engine = eng.Engine(self._engine_config())
+        if self.workspace_mb > 0:   # inference above this workspace runs as overlapping windows (bit-identical)
+            self.engine.set_option("workspace_mb", self.workspace_mb)
         shapes = self.engine.param_shapes()
         # complexity / receptive-field bookkeeping of tf_graph.py:100-110,143-147 and DCSCN.py:267-275
         self.features = ""

@@ -24,6 +24,7 @@
 #include "train.cuh"
 #include "wgrad_tc.cuh"
 #include "train_ds.cuh"
+#include "tile.cuh"
 
 using namespace dcscn;
 
@@ -192,6 +193,15 @@ struct dcscn_handle {
   cudaEvent_t x2_ready = nullptr;
   bool wait_x2 = false;                // the next forward's last kernel waits for x2_ready
   int64_t device_bytes = 0;
+  // tiled inference (option "workspace_mb"): staging buffers of one batch of windows, grow-only
+  int64_t workspace_mb = 0;          // 0 = whole-image forwards only
+  float *tile_x = nullptr, *tile_x2 = nullptr, *tile_y = nullptr;
+  size_t tile_cap = 0;               // LR window pixels the staging buffers hold
+  int64_t tile_bytes = 0;
+  bool tiling = false;               // a tiled forward is issuing its batches (forward_impl keeps the timing events)
+  bool tile_vec4 = false;            // while tiling: the four-pixel R-CNN1 kernel the whole-image forward would pick
+  bool tiled_last = false;           // the last forward ran tiled: the activation buffers hold its last batch
+  int tiled_batches = 0;             // batches of the last tiled forward (timing names)
 
   // depthwise-separable graphs: fp32 buffers + per-layer device filters
   struct DsDev { float *dw = nullptr, *pw = nullptr, *bias = nullptr, *alpha = nullptr; };
@@ -680,38 +690,72 @@ static int dev_alloc(dcscn_handle* h, T** p, size_t count, bool zero) {
   return 0;
 }
 
+// Elements per LR pixel of every buffer ensure_workspace allocates: the one statement of their sizes, shared by the
+// allocation and by the tile planner's workspace budget (valid once the parameters are finalised).
+struct WorkspaceShape {
+  size_t feat, b1, nin, mid;   // fp16 elements per plane (tensor-core graphs) or fp32 (depthwise-separable graphs)
+  size_t hr, vbuf;             // fp32
+  int planes;                  // fp16 planes (tensor-core graphs)
+  size_t bytes_per_px(bool ds) const {
+    return ds ? 4 * (feat + b1 + nin + mid + hr) : 2 * (size_t)planes * (feat + b1 + nin + mid) + 4 * (hr + vbuf);
+  }
+};
+
+static WorkspaceShape workspace_shape(const dcscn_handle* h) {
+  const dcscn_config& c = h->cfg;
+  const size_t s2 = (size_t)c.scale * c.scale;
+  WorkspaceShape w;
+  if (c.depthwise_separable) {
+    const int cps = c.nin_filters + c.nin_filters2;
+    w.feat = h->ds_total;
+    w.b1 = c.nin_filters2;
+    w.nin = cps;
+    w.mid = c.scale == 4 ? 4 * (size_t)cps : 0;
+    w.hr = s2 * h->ps_out;
+    w.vbuf = 0;
+    w.planes = 1;
+    return w;
+  }
+  w.feat = h->feat_pitch;
+  w.b1 = h->b1_w;
+  w.nin = h->nin_pitch;
+  w.mid = c.scale == 4 ? 4 * (size_t)h->mid_pitch : 0;
+  w.hr = s2 * h->ps_out;
+  w.vbuf = s2 * 9 * (size_t)rdot_parts(h->tcl.empty() ? 16 : h->tcl.back().n_pad, h->ps_out);
+  w.planes = planes(h);
+  return w;
+}
+
 static int ensure_workspace(dcscn_handle* h, size_t lr_px) {
   if (lr_px <= h->cap_px) return 0;
   const dcscn_config& c = h->cfg;
+  const WorkspaceShape ws = workspace_shape(h);
   if (c.depthwise_separable) {
     h->device_bytes = 0;
-    const size_t s2 = (size_t)c.scale * c.scale;
-    const int cps = c.nin_filters + c.nin_filters2;
-    if (dev_alloc(h, &h->ds_feat, lr_px * h->ds_total, true)) return 1;   // pad channels must stay zero
-    if (dev_alloc(h, &h->ds_b1, lr_px * c.nin_filters2, false)) return 1;
-    if (dev_alloc(h, &h->ds_nin, lr_px * cps, false)) return 1;
-    if (c.scale == 4 && dev_alloc(h, &h->ds_mid, lr_px * 4 * cps, false)) return 1;
-    if (dev_alloc(h, &h->ds_hr, lr_px * s2 * h->ps_out, false)) return 1;
+    if (dev_alloc(h, &h->ds_feat, lr_px * ws.feat, true)) return 1;   // pad channels must stay zero
+    if (dev_alloc(h, &h->ds_b1, lr_px * ws.b1, false)) return 1;
+    if (dev_alloc(h, &h->ds_nin, lr_px * ws.nin, false)) return 1;
+    if (c.scale == 4 && dev_alloc(h, &h->ds_mid, lr_px * ws.mid, false)) return 1;
+    if (dev_alloc(h, &h->ds_hr, lr_px * ws.hr, false)) return 1;
     h->cap_px = lr_px;
     return 0;
   }
   h->plans.clear();
   h->last_plan = nullptr;
   h->device_bytes = 0;
-  const bool two = planes(h) == 2;
-  const size_t s2 = (size_t)c.scale * c.scale;
-  if (dev_alloc(h, &h->feat_hi, lr_px * h->feat_pitch, true)) return 1;
-  if (dev_alloc(h, &h->feat_lo, two ? lr_px * h->feat_pitch : 0, true)) return 1;
-  if (dev_alloc(h, &h->b1_hi, lr_px * h->b1_w, true)) return 1;
-  if (dev_alloc(h, &h->b1_lo, two ? lr_px * h->b1_w : 0, true)) return 1;
-  if (dev_alloc(h, &h->nin_hi, lr_px * h->nin_pitch, true)) return 1;
-  if (dev_alloc(h, &h->nin_lo, two ? lr_px * h->nin_pitch : 0, true)) return 1;
+  const bool two = ws.planes == 2;
+  if (dev_alloc(h, &h->feat_hi, lr_px * ws.feat, true)) return 1;
+  if (dev_alloc(h, &h->feat_lo, two ? lr_px * ws.feat : 0, true)) return 1;
+  if (dev_alloc(h, &h->b1_hi, lr_px * ws.b1, true)) return 1;
+  if (dev_alloc(h, &h->b1_lo, two ? lr_px * ws.b1 : 0, true)) return 1;
+  if (dev_alloc(h, &h->nin_hi, lr_px * ws.nin, true)) return 1;
+  if (dev_alloc(h, &h->nin_lo, two ? lr_px * ws.nin : 0, true)) return 1;
   if (c.scale == 4) {
-    if (dev_alloc(h, &h->mid_hi, lr_px * 4 * h->mid_pitch, true)) return 1;
-    if (dev_alloc(h, &h->mid_lo, two ? lr_px * 4 * h->mid_pitch : 0, true)) return 1;
+    if (dev_alloc(h, &h->mid_hi, lr_px * ws.mid, true)) return 1;
+    if (dev_alloc(h, &h->mid_lo, two ? lr_px * ws.mid : 0, true)) return 1;
   }
-  if (dev_alloc(h, &h->hr, lr_px * s2 * h->ps_out, true)) return 1;
-  if (dev_alloc(h, &h->vbuf, lr_px * s2 * 9 * (size_t)rdot_parts(h->tcl.empty() ? 16 : h->tcl.back().n_pad, h->ps_out), true)) return 1;
+  if (dev_alloc(h, &h->hr, lr_px * ws.hr, true)) return 1;
+  if (dev_alloc(h, &h->vbuf, lr_px * ws.vbuf, true)) return 1;
   h->cap_px = lr_px;
   return 0;
 }
@@ -1098,8 +1142,10 @@ static DsTileParams ds_tile_params(const LayerDef& l, const dcscn_handle::DsDev&
 static int forward_ds_tile(dcscn_handle* h, const float* x, const float* x2, float* y, int n, int H, int W, cudaStream_t st) {
   const dcscn_config& c = h->cfg;
   const int L = c.layers, T = h->ds_total, na = c.nin_filters, nb = c.nin_filters2, cps = na + nb;
-  h->ev_used = 0;
-  if (mark(h, st)) return 1;
+  if (!h->tiling) {   // a tiled forward keeps one event sequence over all its batches
+    h->ev_used = 0;
+    if (mark(h, st)) return 1;
+  }
   size_t li = 0;
   for (int i = 0; i < L; ++i, ++li) {
     const float* src = i == 0 ? x : h->ds_feat + h->ds_off[i - 1];
@@ -1154,8 +1200,10 @@ static int forward_ds_tile(dcscn_handle* h, const float* x, const float* x2, flo
     if (lr.k != 1 && lr.k != 3) return fail("depthwise-separable R-CNN1: kernel size %d is not supported (1 or 3)", lr.k);
     const long long total = (long long)n * HH * WW;
     // four pixels per thread when the row width and the x2 / y alignment allow it, else one
+    // (a tiled forward takes the kernel the whole image would take: they sum the taps in different orders)
     const bool vec4 = lr.k == 3 && (WW & 3) == 0 && total < (1ll << 32) &&
-                      ((reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(x2)) & 15) == 0;
+                      ((reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(x2)) & 15) == 0 &&
+                      (!h->tiling || h->tile_vec4);
     const int grid = (int)std::min<long long>(((vec4 ? total / 4 : total) + 255) / 256, (long long)h->sm_count * 16);
     if (vec4) ds_single4_kernel<<<grid, 256, 0, st>>>(h->ds_hr, x2, y, n, HH, WW, d.dw, d.pw, d.bias, d.alpha);
     else if (lr.k == 3) ds_single_kernel<3><<<grid, 256, 0, st>>>(h->ds_hr, x2, y, n, HH, WW, d.dw, d.pw, d.bias, d.alpha);
@@ -1204,6 +1252,7 @@ static int forward_impl(dcscn_handle* h, const float* x, const float* x2, float*
   CUDA_TRY(cudaSetDevice(h->cfg.device_id));
   if (h->params_dirty && finalize_params(h)) return 1;
   if (ensure_workspace(h, (size_t)n * H * W)) return 1;
+  if (!h->tiling) h->tiled_last = false;
   if (h->cfg.depthwise_separable) {
     h->ds_n = n; h->ds_h = H; h->ds_w = W;
     return forward_ds_tile(h, x, x2, y, n, H, W, st);
@@ -1211,8 +1260,10 @@ static int forward_impl(dcscn_handle* h, const float* x, const float* x2, float*
   Plan* pl = get_plan(h, n, H, W);
   if (!pl) return 1;
   h->last_plan = pl;
-  h->ev_used = 0;
-  if (mark(h, st)) return 1;
+  if (!h->tiling) {
+    h->ev_used = 0;
+    if (mark(h, st)) return 1;
+  }
   const bool fused = pl->fused_last && h->fuse_last && h->conv_impl == 0;
 
   // ---- graph replay / capture of the launches in front of the last kernel (SURVEY 7 step 5: 15 launches per step)
@@ -1255,7 +1306,9 @@ static int forward_impl(dcscn_handle* h, const float* x, const float* x2, float*
     p.x2 = x2;
     p.y = y;
     const size_t total = (size_t)p.n_img * p.H * p.W;
-    const bool vec4 = p.ksz == 3 && (p.W & 3) == 0 && ((reinterpret_cast<uintptr_t>(x2) | reinterpret_cast<uintptr_t>(y)) & 15) == 0;
+    // (a tiled forward takes the kernel the whole image would take: they can differ in the sign of a zero)
+    const bool vec4 = p.ksz == 3 && (p.W & 3) == 0 && ((reinterpret_cast<uintptr_t>(x2) | reinterpret_cast<uintptr_t>(y)) & 15) == 0 &&
+                      (!h->tiling || h->tile_vec4);
     if (vec4) {
       const int grid = (int)std::min<size_t>((total / 4 + 255) / 256, (size_t)h->sm_count * 16);
       conv_last_gather4_kernel<<<grid, 256, 0, st>>>(p);
@@ -1281,6 +1334,137 @@ static int forward_impl(dcscn_handle* h, const float* x, const float* x2, float*
     if (mark(h, st)) return 1;
   }
   return 0;
+}
+
+// ------------------------------------------------------------------------------ tiled inference ----
+// LR pixels of context a window core needs: the longest dependency path CNN1 .. CNNL -> B1 (1x1) -> B2 -> Up-PS
+// [-> Up-PS2 at 2x] -> R-CNN1 at HR resolution, walked back from an LR core edge.  An HR reach of q pixels past an edge
+// of s-times upscaled pixels is ceil(q / s) pixels before the upscale.
+static int tile_halo(const dcscn_handle* h) {
+  auto half = [](int k) { return (k - 1) / 2; };
+  auto k_of = [h](const std::string& scope) { return find_layer(h, scope)->k; };
+  int r = 0;
+  for (int i = 0; i < h->cfg.layers; ++i) r += half(k_of("CNN" + std::to_string(i + 1)));
+  r += half(k_of("B1")) + half(k_of("B2")) + half(k_of("Up-PS/Up-PS_CNN"));
+  const int hr = half(k_of("R-CNN1"));
+  if (h->cfg.scale == 4) r += (half(k_of("Up-PS2/Up-PS2_CNN")) + (hr + 1) / 2 + 1) / 2;
+  else r += (hr + h->cfg.scale - 1) / h->cfg.scale;
+  return r;
+}
+
+constexpr int kTileMinCore = 16;   // smallest window core (LR pixels per side) the planner uses
+
+struct TilePlan {
+  int th = 0, tw = 0;   // window, LR pixels
+  int my = 0, mx = 0;   // windows per image along y / x
+  int batch = 0;        // windows per batch
+};
+
+// Windows of one size per forward, clamped inside the image.  Of the window shapes whose pixels fit the budget, the one
+// with the fewest window pixels per image is taken (a dimension that fits whole is spanned: no halo along it), ties going
+// to the larger window; then as many windows of all n images as still fit form one batch.  When the whole image would run
+// R-CNN1 on its four-pixel kernel, a window narrower than the image is a multiple of 4 wide so that its batch does too.
+static int plan_tiles(dcscn_handle* h, int n, int H, int W, size_t px_bytes, TilePlan* tp) {
+  const int r = tile_halo(h);
+  const long long max_px = (h->workspace_mb << 20) / (long long)px_bytes;
+  const int min_th = std::min(H, kTileMinCore + 2 * r);
+  const int min_tw = std::min(W, h->tile_vec4 ? (kTileMinCore + 2 * r + 3) & ~3 : kTileMinCore + 2 * r);
+  if ((long long)min_th * min_tw > max_px) {
+    const long long need = ((long long)min_th * min_tw * (long long)px_bytes + (1 << 20) - 1) >> 20;
+    return fail("forward: option workspace_mb = %lld cannot hold one %dx%d window (a %dx%d core plus a %d-pixel halo); this "
+                "graph needs at least workspace_mb = %lld for this image", (long long)h->workspace_mb, min_th, min_tw,
+                kTileMinCore, kTileMinCore, r, need);
+  }
+  long long best = -1, best_area = 0;
+  for (int th = min_th; th <= H && (long long)th * min_tw <= max_px; ++th) {
+    int tw = (int)std::min<long long>(W, max_px / th);
+    if (tw < W && h->tile_vec4) tw &= ~3;
+    if (tw < min_tw) continue;
+    const int my = tile_count(H, th, r), mx = tile_count(W, tw, r);
+    const long long cost = (long long)my * mx * th * tw, area = (long long)th * tw;
+    if (best < 0 || cost < best || (cost == best && area > best_area)) {
+      best = cost;
+      best_area = area;
+      tp->th = th; tp->tw = tw; tp->my = my; tp->mx = mx;
+    }
+  }
+  const long long windows = (long long)n * tp->my * tp->mx;
+  tp->batch = (int)std::max<long long>(1, std::min<long long>(windows, max_px / best_area));
+  return 0;
+}
+
+// Runs the forward as batches of windows (plan_tiles) through forward_impl on the staging buffers: every full batch
+// shares one (batch, th, tw) plan and one staging pointer, so its front launches are captured and replayed like any
+// repeated forward; the last, partial batch has a plan of its own.
+static int forward_tiled(dcscn_handle* h, const float* x, const float* x2, float* y, int n, int H, int W,
+                         const TilePlan& tp, cudaStream_t st) {
+  const int s = h->cfg.scale;
+  const size_t lr_px = (size_t)tp.batch * tp.th * tp.tw, hr_px = lr_px * s * s;
+  if (lr_px > h->tile_cap) {
+    cudaFree(h->tile_x); cudaFree(h->tile_x2); cudaFree(h->tile_y);
+    h->tile_x = h->tile_x2 = h->tile_y = nullptr;
+    h->tile_cap = 0;
+    h->tile_bytes = 0;
+    CUDA_TRY(cudaMalloc((void**)&h->tile_x, lr_px * sizeof(float)));
+    CUDA_TRY(cudaMalloc((void**)&h->tile_x2, hr_px * sizeof(float)));
+    CUDA_TRY(cudaMalloc((void**)&h->tile_y, hr_px * sizeof(float)));
+    h->tile_cap = lr_px;
+    h->tile_bytes = (int64_t)((lr_px + 2 * hr_px) * sizeof(float));
+  }
+  struct Scope {
+    dcscn_handle* h;
+    ~Scope() { h->tiling = false; }
+  } scope{h};
+  h->tiling = true;
+  h->ev_used = 0;
+  if (mark(h, st)) return 1;
+  if (h->wait_x2) {  // forward_host: x2 was copied on the side stream, and the first gather reads it
+    CUDA_TRY(cudaStreamWaitEvent(st, h->x2_ready, 0));
+    h->wait_x2 = false;
+  }
+  const long long windows = (long long)n * tp.my * tp.mx;
+  int batches = 0;
+  for (long long first = 0; first < windows; first += tp.batch, ++batches) {
+    const int count = (int)std::min<long long>(tp.batch, windows - first);
+    const TileGeom g{n, H, W, s, tp.th, tp.tw, tile_halo(h), tp.my, tp.mx, first, count};
+    const long long elems = (long long)count * tp.th * tp.tw * (1 + s * s);
+    tile_gather_kernel<<<(int)std::min<long long>((elems + 255) / 256, (long long)h->sm_count * 8), 256, 0, st>>>(
+        g, x, x2, h->tile_x, h->tile_x2);
+    CUDA_TRY(cudaGetLastError());
+    h->launches++;
+    if (mark(h, st)) return 1;
+    if (forward_impl(h, h->tile_x, h->tile_x2, h->tile_y, count, tp.th, tp.tw, st)) return 1;
+    const long long hr_elems = (long long)count * tp.th * tp.tw * s * s;
+    tile_stitch_kernel<<<(int)std::min<long long>((hr_elems + 255) / 256, (long long)h->sm_count * 8), 256, 0, st>>>(
+        g, h->tile_y, y);
+    CUDA_TRY(cudaGetLastError());
+    h->launches++;
+    if (mark(h, st)) return 1;
+  }
+  h->tiled_last = true;
+  h->tiled_batches = batches;
+  return 0;
+}
+
+// Every inference forward: whole-image (forward_impl) unless option workspace_mb is set and the image's workspace
+// would exceed it.
+static int forward_any(dcscn_handle* h, const float* x, const float* x2, float* y, int n, int H, int W, cudaStream_t st) {
+  if (h->workspace_mb <= 0) return forward_impl(h, x, x2, y, n, H, W, st);
+  if (n <= 0 || H <= 0 || W <= 0) return fail("forward: bad shape n=%d h=%d w=%d", n, H, W);
+  CUDA_TRY(cudaSetDevice(h->cfg.device_id));
+  if (h->params_dirty && finalize_params(h)) return 1;
+  const bool ds = h->cfg.depthwise_separable != 0;
+  const size_t ws_px = workspace_shape(h).bytes_per_px(ds);
+  const long long budget = h->workspace_mb << 20;
+  const long long lr_total = (long long)n * H * W;
+  if (lr_total <= budget / (long long)ws_px) return forward_impl(h, x, x2, y, n, H, W, st);
+  const int s = h->cfg.scale;
+  h->tile_vec4 = find_layer(h, "R-CNN1")->k == 3 && (((long long)s * W) & 3) == 0 &&
+                 ((reinterpret_cast<uintptr_t>(x2) | reinterpret_cast<uintptr_t>(y)) & 15) == 0 &&
+                 (!ds || lr_total * s * s < (1ll << 32));
+  TilePlan tp;
+  if (plan_tiles(h, n, H, W, ws_px + sizeof(float) * (1 + 2 * (size_t)s * s), &tp)) return 1;
+  return forward_tiled(h, x, x2, y, n, H, W, tp, st);
 }
 
 // ------------------------------------------------------------------------- Pillow bicubic on the device ----
@@ -1428,6 +1612,7 @@ int dcscn_destroy(dcscn_handle* h) {
   cudaFree(h->io_x);
   cudaFree(h->io_x2);
   cudaFree(h->io_y);
+  cudaFree(h->tile_x); cudaFree(h->tile_x2); cudaFree(h->tile_y);
   for (auto& pt : h->pil_tables) { cudaFree(pt.k); cudaFree(pt.bounds); }
   cudaFree(h->pil_tmp);
   cudaFree(h->ps_lr); cudaFree(h->ps_bic); cudaFree(h->ps_true); cudaFree(h->ps_idx);
@@ -1478,7 +1663,7 @@ int dcscn_get_param(dcscn_handle* h, const char* name, float* host_data, int64_t
 int dcscn_forward(dcscn_handle* h, const float* x_dev, const float* x2_dev, float* y_dev, int n, int height, int width,
                   void* stream) {
   if (!h || !x_dev || !x2_dev || !y_dev) return fail("dcscn_forward: null argument");
-  return forward_impl(h, x_dev, x2_dev, y_dev, n, height, width, (cudaStream_t)stream);
+  return forward_any(h, x_dev, x2_dev, y_dev, n, height, width, (cudaStream_t)stream);
 }
 
 int dcscn_bicubic_resize(dcscn_handle* h, const float* src_dev, float* dst_dev, int n, int height, int width, int out_height,
@@ -1520,7 +1705,7 @@ int dcscn_forward_host(dcscn_handle* h, const float* x, const float* x2, float* 
     const int s = h->cfg.scale;
     if (pil_resize_impl(h, h->io_x, h->io_x2, n, height, width, s * height, s * width, st)) return 1;
   }
-  const int rc = forward_impl(h, h->io_x, h->io_x2, h->io_y, n, height, width, st);
+  const int rc = forward_any(h, h->io_x, h->io_x2, h->io_y, n, height, width, st);
   h->wait_x2 = false;
   if (rc) {
     cudaStreamSynchronize(h->copy_stream);
@@ -1563,7 +1748,7 @@ static int ensemble_impl(dcscn_handle* h, const float* x, const float* x2, doubl
     CUDA_TRY(cudaGetLastError());
     h->launches += 2;
     const int fh = grp == 0 ? height : width, fw = grp == 0 ? width : height;
-    if (forward_impl(h, h->ens_x, h->ens_x2, h->ens_y + (size_t)grp * 4 * hr, sel.count, fh, fw, st)) return 1;
+    if (forward_any(h, h->ens_x, h->ens_x2, h->ens_y + (size_t)grp * 4 * hr, sel.count, fh, fw, st)) return 1;
   }
   ensemble_reduce_kernel<<<(int)std::min<size_t>((hr + 255) / 256, (size_t)h->sm_count * 8), 256, 0, st>>>(
       h->ens_y, h->ens_y + 4 * hr, y, s * height, s * width, mask, divisor);
@@ -1616,6 +1801,9 @@ int dcscn_forward_ensemble_host(dcscn_handle* h, const float* x, const float* x2
 
 int dcscn_get_activation(dcscn_handle* h, const char* tensor, float* host_data, int64_t numel) {
   if (!h || !tensor || !host_data) return fail("dcscn_get_activation: null argument");
+  if (h->tiled_last)
+    return fail("dcscn_get_activation: the last forward ran tiled (option workspace_mb): the buffers hold its last batch "
+                "of windows, not the image");
   if (h->cfg.depthwise_separable) {
     if (h->ds_n == 0) return fail("dcscn_get_activation: no forward has run yet");
     CUDA_TRY(cudaSetDevice(h->cfg.device_id));
@@ -1713,6 +1901,9 @@ int dcscn_set_option(dcscn_handle* h, const char* key, int64_t value) {
   } else if (k == "act_grad_impl") {
     if (value < 0 || value > 1) return fail("act_grad_impl must be 0 or 1");
     h->act_grad_impl = (int)value;
+  } else if (k == "workspace_mb") {
+    if (value < 0 || value > (int64_t(1) << 40)) return fail("workspace_mb must be >= 0 MiB (0 = no limit), got %lld", (long long)value);
+    h->workspace_mb = value;
   } else if (k == "seg_chunks") {
     if (value < 0 || value > 4096) return fail("seg_chunks must be >= 0 (0 = automatic)");
     h->seg_chunks = (int)value;
@@ -1746,6 +1937,11 @@ int dcscn_get_timings(dcscn_handle* h, float* ms, int capacity, int* count, char
     } else {
       for (const TcLayer& t : h->tcl) s += "," + t.name;
       s += ",R-CNN1";
+    }
+    if (h->tiled_last) {   // every batch of windows: gather, the layers, stitch
+      const std::string layers = s;
+      s = "";
+      for (int b = 0; b < h->tiled_batches; ++b) s += (b ? "," : "") + std::string("tile_gather,") + layers + ",tile_stitch";
     }
     snprintf(names, names_len, "%s", s.c_str());
   }
@@ -1975,7 +2171,13 @@ int dcscn_dropout_mask(dcscn_handle* h, const char* tensor, uint32_t seed, int n
 }
 
 int64_t dcscn_launch_count(dcscn_handle* h) { return h ? h->launches : 0; }
-int64_t dcscn_device_bytes(dcscn_handle* h) { return h ? h->device_bytes : 0; }
+int64_t dcscn_device_bytes(dcscn_handle* h) { return h ? h->device_bytes + h->tile_bytes : 0; }
+
+int dcscn_tile_halo(dcscn_handle* h, int* lr_pixels) {
+  if (!h || !lr_pixels) return fail("dcscn_tile_halo: null argument");
+  *lr_pixels = tile_halo(h);
+  return 0;
+}
 int64_t dcscn_graph_replays(dcscn_handle* h) { return h ? h->graph_replays : 0; }
 
 }  // extern "C"

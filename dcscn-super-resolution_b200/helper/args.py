@@ -210,6 +210,8 @@ _REFERENCE_FLAGS = [
     # --- additions of this engine; the defaults reproduce the reference's fp32 results ---
     ("precision", "f16x3", "tensor-core arithmetic: f16x3 (fp32-equivalent) or f16x1 (single pass, PSNR-neutral)"),
     ("gpus", 1, "GPUs the self-ensemble / training batch is spread over (one process each)"),
+    ("workspace_mb", 0, "MiB of GPU workspace one inference batch may use; larger images run as overlapping windows, "
+                        "bit-identical to the whole image (0 = no limit)"),
 ]
 
 for _name, _default, _help in _REFERENCE_FLAGS:

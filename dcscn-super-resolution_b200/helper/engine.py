@@ -56,6 +56,7 @@ EXPORTED_SYMBOLS = [
     "dcscn_train_step", "dcscn_train_step_host", "dcscn_get_grad", "dcscn_get_adam_slot", "dcscn_set_adam_slot", "dcscn_get_adam_step",
     "dcscn_set_adam_step", "dcscn_last_grad_norm",
     "dcscn_patch_store_set", "dcscn_train_step_indexed", "dcscn_patch_gather", "dcscn_dropout_mask", "dcscn_grad_buffer", "dcscn_apply_gradients", "dcscn_apply_gradients_avg", "dcscn_reset_optimizer", "dcscn_graph_replays",
+    "dcscn_tile_halo",
 ]
 
 _lib = None
@@ -118,6 +119,7 @@ def load_library(path=None):
     lib.dcscn_device_bytes.restype = c64
     lib.dcscn_graph_replays.argtypes = [vp]
     lib.dcscn_graph_replays.restype = c64
+    lib.dcscn_tile_halo.argtypes = [vp, ctypes.POINTER(ci)]
     _lib = lib
     return lib
 
@@ -453,12 +455,23 @@ class Engine:
     def set_option(self, key, value):
         self._check(self.lib.dcscn_set_option(self.handle, key.encode(), int(value)))
 
+    def tile_halo(self):
+        """LR pixels of context around each window core of a tiled forward (option "workspace_mb")."""
+        r = ctypes.c_int()
+        self._check(self.lib.dcscn_tile_halo(self.handle, ctypes.byref(r)))
+        return int(r.value)
+
     def timings(self):
         """[(launch name, ms)] of the last forward (needs set_option("timing", 1) before it)."""
-        ms = (ctypes.c_float * 64)()
-        cnt = ctypes.c_int()
-        names = ctypes.create_string_buffer(1024)
-        self._check(self.lib.dcscn_get_timings(self.handle, ms, 64, ctypes.byref(cnt), names, 1024))
+        cap = 64
+        while True:   # a tiled forward has one sequence of launches per batch of windows
+            ms = (ctypes.c_float * cap)()
+            cnt = ctypes.c_int()
+            names = ctypes.create_string_buffer(32 * cap)
+            self._check(self.lib.dcscn_get_timings(self.handle, ms, cap, ctypes.byref(cnt), names, 32 * cap))
+            if cnt.value <= cap:
+                break
+            cap = cnt.value
         return list(zip(names.value.decode().split(","), [float(ms[i]) for i in range(cnt.value)]))
 
     @property

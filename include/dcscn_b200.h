@@ -161,6 +161,7 @@ int dcscn_dropout_mask(dcscn_handle* h, const char* tensor, uint32_t seed, int n
 /*
  * Parity / debug: output of one layer of the LAST forward as fp32 NHWC [n, H_l, W_l, cout_l]
  * (`tensor` is the reference's self.H entry: "CNN1".."CNNL", "A1", "B1", "B2", "Up-PS", "Up-PS2").
+ * Fails after a forward that ran tiled (option "workspace_mb"): the buffers then hold its last batch of windows.
  */
 int dcscn_get_activation(dcscn_handle* h, const char* tensor, float* host_data, int64_t numel);
 
@@ -173,11 +174,26 @@ int dcscn_get_activation(dcscn_handle* h, const char* tensor, float* host_data, 
  *          the same input pointer has been seen twice in a row (default 1; off while "timing" = 1 or "conv_impl" = 1);
  *          "l1_loss" 0 | 1 = image_loss of the train step is mean |y_ - y| instead of the MSE (--use_l1_loss,
  *          DCSCN.py:342-344; the returned mse stays the MSE);
- *          "wgrad_impl" 0 | 1 = filter gradients on wgmma tensor cores (default) or on CUDA cores (cross-check). */
+ *          "wgrad_impl" 0 | 1 = filter gradients on wgmma tensor cores (default) or on CUDA cores (cross-check);
+ *          "workspace_mb" = MiB an inference forward may allocate per batch (default 0 = no limit: the whole batch runs
+ *          at once).  Covers dcscn_forward, dcscn_forward_host and the dcscn_forward_ensemble* calls.  The limit counts
+ *          the activation workspace and the staging buffers of one batch of windows; an image whose workspace fits runs
+ *          exactly as without the option, a larger one runs as batches of overlapping windows (each with
+ *          dcscn_tile_halo pixels of context), bit-identical to the whole-image forward.  A limit too small for one
+ *          window of a 16 x 16 core plus its halo fails the forward, naming the minimum.  Not counted: the whole-image
+ *          buffers of the host-buffer and ensemble calls (their x / x2 / y copies and transformed images, tens of bytes
+ *          per LR pixel) and the bicubic scratch.  The workspace only grows: set the option before the first forward.
+ *          The train step does not read it (its batches are patches).  Negative values are refused. */
 int dcscn_set_option(dcscn_handle* h, const char* key, int64_t value);
 /* With option "timing" = 1 every launch of a forward is bracketed by CUDA events on its stream; this returns the
- * device time in ms of each launch of the LAST forward (in launch order) and their comma-separated names. */
+ * device time in ms of each launch of the LAST forward (in launch order) and their comma-separated names.  A tiled
+ * forward lists tile_gather, its layers and tile_stitch once per batch of windows. */
 int dcscn_get_timings(dcscn_handle* h, float* ms, int capacity, int* count, char* names, int names_len);
+/* LR pixels of context a window of a tiled forward carries around its core (option "workspace_mb"): the receptive
+ * radius of the graph, walked back from R-CNN1 at HR resolution (15 for the 12-layer 3x3 graphs, 10 for 7 layers).
+ * A core computed with this much context is bit-identical to the same pixels of the whole-image forward, which also
+ * lets a caller split one image over several GPUs. */
+int dcscn_tile_halo(dcscn_handle* h, int* lr_pixels);
 /* Number of kernels this handle has launched so far (bench.py "gpu_launches"). */
 int64_t dcscn_launch_count(dcscn_handle* h);
 /* Forwards served by a CUDA-graph replay so far (option "graph"). */
