@@ -182,6 +182,40 @@ def test_depthwise_separable_odd_hr_width():
     check_depthwise_separable_layers(DS2, O.he_init_weights(O.OracleConfig(**DS2), seed=4), 3, 17, 23)
 
 
+@pytest.mark.parametrize("model", ["dcscn_L12_F196to48_NIN_A64_PS_R1F32", "dcscn_L12_F196to48_Sc4_NIN_A64_PS_R1F32"],
+                         ids=["L12x2", "L12x4"])
+def test_unfused_last_layer_every_layer(model):
+    """Option fuse_last = 0 on the full-width checkpoints: R-CNN1 runs as its own kernel on the materialised Up-PS
+    (x2) / Up-PS2 (x4) output, which the fused path never writes.  On a Set5 crop every layer, the pixel-shuffler
+    outputs included, matches the fp64 oracle at the fp32-level bar of test_small_graph_every_layer, and the fused and
+    unfused outputs are both within 1e-3 of fp64."""
+    kw = MODEL_FLAGS[model]
+    s = kw.get("scale", 2)
+    w = load_golden_weights(model)
+    f = sorted(glob.glob(os.path.join(GOLDEN, "data", "set5", "*.png")))[1]
+    lr, bic, _ = O.build_inputs_for_evaluate(f, s)
+    r0, c0, h, wd = 8, 12, 36, 44
+    x = np.ascontiguousarray(lr[r0:r0 + h, c0:c0 + wd].reshape(1, h, wd, 1)).astype(np.float32)
+    x2 = np.ascontiguousarray(bic[s * r0:s * (r0 + h), s * c0:s * (c0 + wd)].reshape(1, s * h, s * wd, 1)).astype(np.float32)
+    y64, inter = O.Oracle(O.OracleConfig(**kw), w, torch.float64).forward(x.astype(np.float64), x2.astype(np.float64),
+                                                                         return_intermediates=True)
+    eng = make_engine(kw, w)
+    y_fused = gpu_forward(eng, x, x2)
+    eng.set_option("fuse_last", 0)
+    y = gpu_forward(eng, x, x2)
+    assert np.abs(y_fused - y64).max() <= TOL
+    assert np.abs(y - y64).max() <= TOL
+    bad = []
+    for name, ref in inter.items():
+        if name == "R-CNN":
+            continue
+        err = float(np.abs(eng.get_activation(name, ref.shape) - ref).max())
+        if not err <= 4e-6 * max(1.0, np.abs(ref).max()) + 1e-4:
+            bad.append((name, err, float(np.abs(ref).max())))
+    eng.close()
+    assert not bad, bad
+
+
 def test_l12_stress_noise_tiles():
     """BASELINE configs[1] shape: uniform-noise 48x48 tiles through the L12 x2 checkpoint."""
     model = "dcscn_L12_F196to48_NIN_A64_PS_R1F32"

@@ -7,17 +7,28 @@ import pytest
 import torch
 
 import dcscn_oracle as O
+from conftest import MODEL_FLAGS, load_golden_weights
 
 pytestmark = pytest.mark.gpu
 
 SMALL = dict(scale=2, layers=3, filters=24, min_filters=16, filters_decay_gamma=1.5, nin_filters=16, nin_filters2=16)
 SMALL4 = dict(scale=4, layers=3, filters=20, min_filters=16, filters_decay_gamma=1.5, nin_filters=16, nin_filters2=16)
+SMALL3 = dict(SMALL, scale=3)
+K5 = dict(SMALL, cnn_size=5)
+# the shipped c-DCSCN checkpoints: --pixel_shuffler_filters=1, so R-CNN1 reads a single channel (C = 1)
+CDCSCN = {2: "dcscn_L7_F32to8_G1.20_NIN_A24_B8_PS_R1F32", 3: "dcscn_L7_F32to8_G1.20_Sc3_NIN_A24_B8_PS_R1F32",
+          4: "dcscn_L7_F32to8_G1.20_Sc4_NIN_A24_B8_PS_R1F32"}
 
 
-def setup(kw, keep, n, h, w, seed=0):
+def setup(kw, keep, n, h, w, seed=0, weights="he"):
+    """`weights` is "he" (He-init with `seed`) or the name of a checkpoint under tests/golden/models, whose MODEL_FLAGS
+    then replace `kw`."""
     from helper import engine as E
+    if weights != "he":
+        kw = MODEL_FLAGS[weights]
     cfg = O.OracleConfig(**kw)
-    wts = {k: v.astype(np.float64) for k, v in O.he_init_weights(cfg, seed=seed).items()}
+    src = O.he_init_weights(cfg, seed=seed) if weights == "he" else load_golden_weights(weights)
+    wts = {k: v.astype(np.float64) for k, v in src.items()}
     eng = E.Engine(E.make_config(dropout_keep=keep, **kw))
     eng.set_params({k: v.astype(np.float32) for k, v in wts.items()})
     g = np.random.RandomState(seed + 1)
@@ -37,28 +48,102 @@ def oracle_masks(eng, cfg, seed, n, h, w):
     return masks
 
 
-@pytest.mark.parametrize("kw,keep,shape", [(SMALL, 1.0, (2, 12, 10)), (SMALL, 0.8, (2, 16, 24)), (SMALL4, 0.8, (1, 9, 11)),
-                                           (SMALL, 1.0, (1, 1, 1)), (SMALL4, 1.0, (3, 2, 1)), (SMALL, 0.8, (1, 1, 37)),
-                                           (SMALL, 1.0, (2, 33, 3))],
-                         ids=["x2-nodrop", "x2-drop", "x4-drop", "x2-1x1", "x4-2x1", "x2-row", "x2-narrow"])
-def test_gradients_match_oracle(kw, keep, shape):
+def launched_kernels(fn):
+    """Runs fn() under torch.profiler and returns (its result, the names of the CUDA kernels launched meanwhile).  CUPTI
+    records every kernel of the process, so the engine's launches from libdcscn_b200.so show up with demangled names
+    ("void dcscn::last_wgrad_kernel<9>(dcscn::LastWgradParams)")."""
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.init()
+    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+        out = fn()
+        torch.cuda.synchronize()
+    return out, {e.name for e in prof.events()}
+
+
+def assert_kernels_ran(names, kernels):
+    """Every entry of `kernels` was launched: "foo" matches dcscn::foo( or dcscn::foo< (so last_wgrad_kernel does not
+    match last_wgrad_scalar_kernel), "foo<25>" matches that instantiation only."""
+    ours = sorted(n for n in names if "dcscn::" in n)
+    assert ours, ("the profiler recorded no dcscn:: kernel among %d events: CUPTI did not trace the engine's launches, "
+                  "so which kernels a case reaches cannot be checked" % len(names))
+
+    def ran(k):
+        pats = ["dcscn::" + k] if "<" in k else ["dcscn::%s(" % k, "dcscn::%s<" % k]
+        return any(p in n for n in ours for p in pats)
+    missing = [k for k in kernels if not ran(k)]
+    assert not missing, ("not launched", missing, ours)
+
+
+# The fast kernels of the train step, and what each general case must reach instead (train_engine.inc, train_step_impl:
+# the selection predicates of CNN1, R-CNN1 forward / filter gradient / data gradient + space_to_depth, x4 space_to_depth).
+FAST = ["conv_tc_kernel", "wgrad_tc_kernel", "conv_first3x3_kernel", "first_wgrad_kernel", "conv_last_direct_kernel",
+        "last_wgrad_kernel<9>", "last_dgrad_s2d_rows_kernel"]
+C1 = ["conv_last_kernel", "last_wgrad_scalar_kernel", "last_dgrad_s2d_kernel"]     # R-CNN1 on one input channel
+GENERAL_K = ["conv_first_kernel", "wgrad_kernel", "conv_last_kernel", "last_dgrad_s2d_kernel", "wgrad_tc_kernel"]
+
+GRADIENT_CASES = [
+    # id, config, weights, keep, (n, h, w), kernels that must run
+    ("x2-nodrop", SMALL, "he", 1.0, (2, 12, 10), FAST),
+    ("x2-drop", SMALL, "he", 0.8, (2, 16, 24), FAST),
+    ("x4-drop", SMALL4, "he", 0.8, (1, 9, 11), FAST + ["s2d_planes_kernel"]),
+    ("x2-1x1", SMALL, "he", 1.0, (1, 1, 1), FAST),
+    ("x4-2x1", SMALL4, "he", 1.0, (3, 2, 1), FAST + ["s2d_planes_kernel"]),
+    ("x2-row", SMALL, "he", 0.8, (1, 1, 37), FAST),
+    ("x2-narrow", SMALL, "he", 1.0, (2, 33, 3), FAST),
+    # depth_to_space gradient at r = 3; Up-PS has 9 * 32 = 288 columns: three wgmma column tiles in its filter gradient
+    # and a partial last K chunk in its data-gradient twin
+    ("x3", SMALL3, "he", 0.8, (2, 9, 11), FAST),
+    ("cdcscn-x2", None, CDCSCN[2], 0.8, (2, 12, 10), C1),
+    ("cdcscn-x3", None, CDCSCN[3], 0.8, (2, 12, 10), C1),
+    ("cdcscn-x4", None, CDCSCN[4], 0.8, (2, 12, 10), C1 + ["s2d_planes_kernel"]),
+    # 5x5 everywhere but A1 / B1 / B2: CNN1 stores min(z, 0) from the general kernel, CNN1's filter gradient reads the fp32
+    # image, wgmma filter gradients at 25 taps, R-CNN1 C = 32 on the vector branch of the data-gradient kernel
+    ("k5-x2", K5, "he", 0.8, (2, 12, 10), GENERAL_K + ["last_wgrad_kernel<25>"]),
+    # nin 12 + 8 = 20 channels (not a multiple of 8): per-element space_to_depth and the per-channel data-gradient branch
+    ("k5-x4-c20", dict(SMALL4, cnn_size=5, nin_filters=12, nin_filters2=8), "he", 0.8, (1, 9, 7),
+     GENERAL_K + ["last_wgrad_kernel<25>", "s2d_planes_kernel"]),
+    ("k1-x3", dict(SMALL3, cnn_size=1), "he", 0.8, (2, 8, 9), GENERAL_K + ["last_wgrad_kernel<1>"]),
+    # R-CNN1 C = 12: a multiple of 4 but not of 8, still on the vector kernels
+    ("ps12-x2", dict(SMALL, pixel_shuffler_filters=12), "he", 0.8, (2, 10, 13), FAST),
+    # R-CNN1 C = 144 > 128: general forward and data gradient; Up-PS has 576 columns
+    ("ps144-x2", dict(SMALL, nin_filters=96, nin_filters2=48), "he", 0.8, (1, 8, 9),
+     ["conv_last_kernel", "last_wgrad_kernel<9>", "last_dgrad_s2d_kernel", "wgrad_tc_kernel"]),
+    # CNN1 with 272 filters (n_pad > 256) on the general kernels; CNN2 has a 16-channel partial K chunk (272 = 4 * 64 + 16)
+    ("cnn1-272", dict(SMALL, layers=2, filters=272, min_filters=32), "he", 0.8, (1, 8, 8),
+     ["conv_first_kernel", "wgrad_kernel", "conv_tc_kernel", "wgrad_tc_kernel"]),
+]
+
+
+@pytest.mark.parametrize("kw,weights,keep,shape,kernels", [c[1:] for c in GRADIENT_CASES], ids=[c[0] for c in GRADIENT_CASES])
+def test_gradients_match_oracle(kw, weights, keep, shape, kernels):
+    """Loss, mse, global norm and every gradient of one train step against fp64 autograd, on graphs chosen so that each
+    kernel the train step can select (fast or general path) runs in at least one case; the profiler trace of the step
+    proves it.  All mismatches of a case are reported at once."""
     n, h, w = shape
-    cfg, wts, eng, x, x2, y = setup(kw, keep, n, h, w)
+    cfg, wts, eng, x, x2, y = setup(kw, keep, n, h, w, weights=weights)
     seed = 1234
-    loss, mse = eng.train_step_host(x, x2, y, lr=0.002, seed=seed, apply_update=False)
+    (loss, mse), names = launched_kernels(lambda: eng.train_step_host(x, x2, y, lr=0.002, seed=seed, apply_update=False))
+    assert_kernels_ran(names, kernels)
     orc = O.Oracle(cfg, wts, torch.float64)
     masks = oracle_masks(eng, cfg, seed, n, h, w) if keep < 1.0 else None
     mse_ref, loss_ref, grads_ref = orc.loss_and_grads(x.astype(np.float64), x2.astype(np.float64), y.astype(np.float64),
                                                       keep_prob=keep, masks=masks)
-    assert mse == pytest.approx(mse_ref, rel=2e-5)
-    assert loss == pytest.approx(mse_ref, rel=2e-5)          # image_loss == mse (DCSCN.py:346-347)
+    bad = []
+    if not mse == pytest.approx(mse_ref, rel=2e-5):
+        bad.append(("mse", mse, mse_ref))
+    if not loss == pytest.approx(mse_ref, rel=2e-5):          # image_loss == mse (DCSCN.py:346-347)
+        bad.append(("loss", loss, mse_ref))
     norm_ref = np.sqrt(sum(np.sum(v ** 2) for v in grads_ref.values()))
-    assert eng.last_grad_norm == pytest.approx(norm_ref, rel=2e-3)
+    if not eng.last_grad_norm == pytest.approx(norm_ref, rel=2e-3):
+        bad.append(("grad norm", eng.last_grad_norm, norm_ref))
     for name, gref in grads_ref.items():
         g = eng.get_grad(name)
         tol = 2e-3 * np.abs(gref).max() + 1e-7
-        assert np.abs(g - gref).max() <= tol, (name, float(np.abs(g - gref).max()), float(np.abs(gref).max()))
+        err = float(np.abs(g - gref).max())
+        if not err <= tol:
+            bad.append((name, err, float(np.abs(gref).max())))
     eng.close()
+    assert not bad, bad
 
 
 def test_adam_step_matches_oracle_and_loss_decreases():
@@ -98,14 +183,18 @@ def test_adam_step_matches_oracle_and_loss_decreases():
     eng.close()
 
 
-@pytest.mark.parametrize("kw", [SMALL, SMALL4], ids=["x2", "x4"])
-def test_device_refresh_equals_host_repack(kw):
+@pytest.mark.parametrize("kw,weights", [(SMALL, "he"), (SMALL4, "he"), (SMALL3, "he"), (K5, "he"), (None, CDCSCN[3])],
+                         ids=["x2", "x4", "x3", "k5-x2", "cdcscn-x3"])
+def test_device_refresh_equals_host_repack(kw, weights):
     """After an optimizer step the packed tensor-core weight images (forward layers and dgrad twins), fused bias / PReLU
     vectors and the CNN1 / R-CNN1 filters are refreshed on the device through index maps derived from the host packing
     code.  A fresh engine that packs the same weights on the host must give the same forward output and the same
-    gradients (only the power-of-two weight scale may differ, which is exact)."""
+    gradients (only the power-of-two weight scale may differ, which is exact).  The cases cover 3x3 and 5x5 twins, a
+    9-column Up-PS (x3 with one R-CNN1 input channel) and a one-channel R-CNN1 filter."""
     from helper import engine as E
-    cfg, wts, eng, x, x2, y = setup(kw, 0.8, 2, 12, 14, seed=3)
+    if weights != "he":
+        kw = MODEL_FLAGS[weights]
+    cfg, wts, eng, x, x2, y = setup(kw, 0.8, 2, 12, 14, seed=3, weights=weights)
     for i in range(4):
         eng.train_step_host(x, x2, y, lr=0.01, seed=50 + i)
     y_dev = eng.forward_host(x, x2)
@@ -123,6 +212,27 @@ def test_device_refresh_equals_host_repack(kw):
         assert np.abs(g - grads_dev[n]).max() <= 1e-4 * np.abs(g).max() + 1e-9, n   # fp32 atomics reorder sums
     eng.close()
     fresh.close()
+
+
+def test_train_step_refuses_f16x1_and_handle_keeps_working():
+    """The train step needs the fp16x3 operand planes of the tensor-core graph: an f16x1 engine refuses it with
+    EngineError, and the refusal leaves the handle as it was, so the forward still runs and gives the same output."""
+    from helper import engine as E
+    cfg = O.OracleConfig(**SMALL)
+    wts = O.he_init_weights(cfg, seed=2)
+    eng = E.Engine(E.make_config(dropout_keep=0.8, precision=1, **SMALL))
+    eng.set_params(wts)
+    g = np.random.RandomState(8)
+    x = (g.rand(1, 10, 12, 1) * 255).astype(np.float32)
+    x2 = (g.rand(1, 20, 24, 1) * 255).astype(np.float32)
+    y_before = eng.forward_host(x, x2)
+    with pytest.raises(E.EngineError, match="f16x3"):
+        eng.train_step_host(x, x2, x2, lr=0.002, seed=1)
+    y_after = eng.forward_host(x, x2)
+    assert np.array_equal(y_before, y_after)
+    ref = O.Oracle(cfg, {k: v.astype(np.float64) for k, v in wts.items()}, torch.float64).forward(x.astype(np.float64), x2.astype(np.float64))
+    assert np.abs(y_after - ref).max() < 1.0          # single-pass fp16 operands: the bar of test_fast_mode_is_psnr_neutral
+    eng.close()
 
 
 def test_tensor_core_wgrad_matches_cuda_core_wgrad_full_model():
@@ -263,9 +373,13 @@ DS4W = dict(scale=4, layers=3, filters=10, min_filters=6, filters_decay_gamma=1.
             pixel_shuffler_filters=0, depthwise_separable=True)    # pixel shuffler keeps all 12 channels: R-CNN1 12 -> 1
 
 
+DS3 = dict(scale=3, layers=3, filters=12, min_filters=6, filters_decay_gamma=1.5, nin_filters=10, nin_filters2=6,
+           pixel_shuffler_filters=1, depthwise_separable=True)
+
+
 @pytest.mark.parametrize("kw,keep,shape", [(DS2, 1.0, (2, 9, 7)), (DS2, 0.8, (2, 12, 10)), (DS4, 0.8, (2, 8, 11)),
-                                           (DS4, 1.0, (1, 1, 1)), (DS4W, 0.8, (1, 6, 5))],
-                         ids=["ds-x2-nodrop", "ds-x2-drop", "ds-x4-drop", "ds-x4-1x1", "ds-x4-wide"])
+                                           (DS4, 1.0, (1, 1, 1)), (DS4W, 0.8, (1, 6, 5)), (DS3, 0.8, (2, 7, 9))],
+                         ids=["ds-x2-nodrop", "ds-x2-drop", "ds-x4-drop", "ds-x4-1x1", "ds-x4-wide", "ds-x3-oddw"])
 def test_depthwise_separable_gradients_match_oracle(kw, keep, shape):
     """The train step of --depthwise_separable graphs: loss, mse and EVERY gradient (depthwise_W, pointwise_W, conv_B, PReLU
     slopes, and the dead conv_W whose only gradient is its L2 decay, tf_graph.py:183,212) against fp64 autograd with
