@@ -8,7 +8,7 @@ by the CLIs (`build_graph` -> [`build_optimizer`] -> `build_summary_saver` -> `i
 `load_model`), `do` / `do_for_file` / `do_for_evaluate[_with_output]` / `evaluate` / `evaluate_bicubic`,
 `train_batch` / `build_input_batch` and the learning-rate / status bookkeeping, and the log lines.
 Replaced: everything `sess.run` did.  Not carried over (TensorFlow-specific, SURVEY.md section 2 rows 15-17):
-tensorboard summaries, frozen-graph loading, transposed-conv upsampler, batch-norm, non-PReLU activators.
+tensorboard summaries, frozen-graph loading, transposed-conv upsampler, batch-norm.
 """
 
 import logging
@@ -219,8 +219,6 @@ class SuperResolution:
     def _check_supported(self):
         """Flag values the reference accepts but no shipped checkpoint uses are rejected with a clear message."""
         problems = []
-        if self.activator != "prelu":
-            problems.append("--activator=%s (only prelu)" % self.activator)
         if self.batch_norm:
             problems.append("--batch_norm")
         if not self.pixel_shuffler:
@@ -238,6 +236,8 @@ class SuperResolution:
 
     # ------------------------------------------------------------------ graph ----
     def _engine_config(self):
+        if self.activator not in eng.ACTIVATORS:
+            raise NameError("Not implemented activator:%s" % self.activator)   # tf_graph.py:98, at build_graph
         prec = {"f16x3": eng.PRECISION_F16X3, "f16x1": eng.PRECISION_F16X1}[self.precision]
         return eng.make_config(
             scale=self.scale, layers=self.layers, filters=self.filters, min_filters=self.min_filters,
@@ -246,7 +246,7 @@ class SuperResolution:
             reconstruct_filters=self.reconstruct_filters, pixel_shuffler_filters=self.pixel_shuffler_filters,
             depthwise_separable=self.depthwise_separable, channels=self.channels, dropout_keep=self.dropout_rate,
             l2_decay=self.l2_decay, clipping_norm=self.clipping_norm, beta1=self.beta1, beta2=self.beta2,
-            epsilon=self.epsilon, device_id=self.gpu_device_id, precision=prec)
+            epsilon=self.epsilon, device_id=self.gpu_device_id, precision=prec, activator=self.activator)
 
     def build_graph(self):
         """DCSCN.py:222-332: creates the engine (variables at their initial values) and the bookkeeping strings."""
@@ -270,7 +270,7 @@ class SuperResolution:
             self.complexity += pix * k * k * cin * cout
             if (scope + "/conv_B") in shapes:
                 self.complexity += pix * cout
-            if any(n.startswith(scope + "/prelu/") for n in shapes):
+            if scope.startswith("CNN") or scope in ("A1", "B1", "B2"):   # build_activator, whatever the activator
                 self.complexity += pix * cout
             if scope == "B1":
                 pass  # A1 and B1 are parallel: DCSCN.py:275 takes the 1x1 back out

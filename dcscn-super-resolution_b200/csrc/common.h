@@ -24,6 +24,19 @@ enum EpilogueMode : int {
                        // writes, per HR pixel and filter tap, dot(h[pixel, :], w_last[tap, :])
 };
 
+// Point-wise activation of CNN1..CNNL, A1, B1 and B2 (--activator, tf_graph.py:77-102); values of DCSCN_ACTIVATOR_*.
+// The forward kernels apply prelu, relu and leaky_relu as z > 0 ? z : a * z with a per-channel slope vector a (the
+// PReLU variable, 0, or 0.1f; linear layers carry act = ACT_PRELU with a = 1) and evaluate the others as functions.
+enum Activation : int {
+  ACT_NONE = -1,       // linear layer without dropout (train kernels only)
+  ACT_PRELU = 0,
+  ACT_RELU = 1,
+  ACT_LEAKY_RELU = 2,
+  ACT_SIGMOID = 3,
+  ACT_TANH = 4,
+  ACT_SELU = 5,
+};
+
 struct EpiSegment {
   int col_begin;       // first GEMM column of this segment (multiple of 16)
   int col_end;         // one past the last column written (multiple of 16)
@@ -39,6 +52,7 @@ struct EpiParams {
   const float* bias;   // [n_total_pad]  (zeros where the layer has no bias / padding)
   const float* alpha;  // [n_total_pad]  PReLU slope; 1.0 == linear layer
   float out_scale;     // 1 / weight_scale (exact power of two)
+  int act;             // Activation: ACT_SIGMOID / ACT_TANH / ACT_SELU apply that function (their slope vector is 1)
   int mode;
   int n_valid;         // real output channels (cout) - columns >= n_valid are dropped for D2S
   EpiSegment seg[kMaxSegments];

@@ -95,6 +95,7 @@ __global__ void __launch_bounds__(256, 2) conv_first3x3_kernel(const ConvFirstPa
   }
   const EpiSegment seg = p.epi.seg[0];
   const float keep = p.epi.keep_prob, inv_keep = 1.0f / keep;
+  const int act = p.epi.act;
   const long long total = (long long)p.g.n_img * p.g.H * p.g.W;
   const long long warp0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
@@ -135,6 +136,11 @@ __global__ void __launch_bounds__(256, 2) conv_first3x3_kernel(const ConvFirstPa
         if (ZNEG) pz[i >> 1] = pack_h2(__float2half_rn(fmaxf(fminf(t0, 0.f), -65504.f)), __float2half_rn(fmaxf(fminf(t1, 0.f), -65504.f)));
         t0 = t0 > 0.f ? t0 : alpha[i] * t0;
         t1 = t1 > 0.f ? t1 : alpha[i + 1] * t1;
+        if (!ZNEG && act >= ACT_SIGMOID) {             // slope 1 on these layers: t0, t1 are still z (their training
+                                                       // forward writes no min(z, 0) plane, so ZNEG excludes them)
+          t0 = act_curve_call(act, t0);
+          t1 = act_curve_call(act, t1);
+        }
         if (keep < 1.0f) {
           const uint64_t base = (uint64_t)pix * (uint64_t)p.n_pad + c0 + i;
           t0 = dropout_keep(p.epi.drop_seed, p.epi.drop_layer, base, keep) ? t0 * inv_keep : 0.f;

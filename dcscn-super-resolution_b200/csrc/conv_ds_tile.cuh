@@ -21,6 +21,7 @@
 // fp32 throughout (CUDA cores): the contraction depth is <= 140 and the layers are HBM / issue bound, not FLOP bound.
 #pragma once
 #include <cstdint>
+#include "epilogue.cuh"
 
 namespace dcscn {
 
@@ -270,6 +271,19 @@ __global__ void __launch_bounds__(kDtThreads) ds_tile_kernel(const DsTileParams 
         }
       }
     }
+  }
+}
+
+// sigmoid / tanh / selu of an activated layer's output, in place: channels [off, off + C) of a [px][pitch] buffer.
+// prelu, relu and leaky_relu run inside ds_tile_kernel's epilogue through its slope vector; evaluating the other three
+// there as well changed the register allocation of every ds_tile_kernel instantiation and cost the PReLU graph 1.3 %
+// (bench.py `ds`), so they take this one extra pass over the layer's output instead.
+__global__ void __launch_bounds__(256) ds_act_kernel(float* buf, long long npx, int pitch, int off, int C, int act) {
+  const long long total = npx * C;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long px = i / C;
+    float* q = buf + px * pitch + off + (int)(i - px * C);
+    *q = act_curve(act, *q);
   }
 }
 

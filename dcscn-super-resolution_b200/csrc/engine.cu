@@ -54,7 +54,8 @@ static inline int pad16(int v) { return (v + 15) & ~15; }
 struct LayerDef {
   std::string scope;  // TF variable scope, e.g. "CNN3", "Up-PS/Up-PS_CNN"
   int k, cin, cout;
-  bool bias, prelu;
+  bool bias;
+  bool act;           // activated (--activator, then dropout): CNN1..CNNL, A1, B1, B2
 };
 
 struct ParamDef {
@@ -257,8 +258,32 @@ static void add_param(dcscn_handle* h, const std::string& name, std::vector<int6
   h->params.push_back(std::move(p));
 }
 
+// Name of an activated layer's PReLU slope variable (tf_graph.py:89-91); only --activator=prelu creates it.
+static std::string prelu_name(const std::string& scope) {
+  const size_t k = scope.find_last_of('/');
+  return scope + "/prelu/" + (k == std::string::npos ? scope : scope.substr(k + 1)) + "_prelu";
+}
+static bool has_slope_variable(const dcscn_handle* h, const LayerDef& l) {
+  return l.act && h->cfg.activator == DCSCN_ACTIVATOR_PRELU;
+}
+static const std::vector<float>& P(const dcscn_handle* h, const std::string& name);
+
+// The slope below zero that the forward kernels apply to an activated layer's channels: the PReLU variable, relu's 0 or
+// leaky_relu's 0.1f (whose product 0.1f * z is the value tf.maximum(z, 0.1 * z) returns).  sigmoid, tanh and selu use
+// no slope (EpiParams::act); their entries keep the linear 1.
+static void layer_slopes(const dcscn_handle* h, const LayerDef& l, float* dst) {
+  const int a = h->cfg.activator;
+  for (int co = 0; co < l.cout; ++co)
+    dst[co] = a == DCSCN_ACTIVATOR_RELU ? 0.f : a == DCSCN_ACTIVATOR_LEAKY_RELU ? 0.1f : 1.f;
+  if (a == DCSCN_ACTIVATOR_PRELU) {
+    const std::vector<float>& A = P(h, prelu_name(l.scope));
+    std::copy(A.begin(), A.begin() + l.cout, dst);
+  }
+}
+
 static int build_graph(dcscn_handle* h) {
   const dcscn_config& c = h->cfg;
+  if (c.activator < DCSCN_ACTIVATOR_PRELU || c.activator > DCSCN_ACTIVATOR_SELU) return fail("activator %d is not one of DCSCN_ACTIVATOR_*", c.activator);
   if (!c.use_nin) return fail("use_nin=false is not supported (no shipped checkpoint uses it)");
   if (c.channels != 1) return fail("channels must be 1 (helper/args.py: 'Now it should be 1')");
   if (std::max(c.reconstruct_layers, 1) != 1) return fail("reconstruct_layers > 1 is not supported");
@@ -294,7 +319,7 @@ static int build_graph(dcscn_handle* h) {
       add_param(h, l.scope + "/pointwise_W", {1, 1, l.cin, l.cout}, 0.f);
     }
     if (l.bias) add_param(h, l.scope + "/conv_B", {l.cout}, 0.f);                 // util.bias: zeros
-    if (l.prelu) add_param(h, l.scope + "/prelu/" + base + "_prelu", {l.cout}, 0.1f);  // tf_graph.py:91
+    if (has_slope_variable(h, l)) add_param(h, prelu_name(l.scope), {l.cout}, 0.1f);  // tf_graph.py:91
   }
 
   // channel layout of the shared feature ("concat") buffer: 16-aligned slot per CNN layer
@@ -365,16 +390,12 @@ static void fuse_columns(const dcscn_handle* h, TcLayer& t, const std::string& s
     for (int ci = 0; ci < l->cin; ++ci)
       for (int co = 0; co < l->cout; ++co)
         t.w_host[((size_t)tp * t.cin + ci) * t.cout + col0 + co] = W[((size_t)tp * l->cin + ci) * l->cout + co];
-  std::string base = scope.substr(scope.find_last_of('/') == std::string::npos ? 0 : scope.find_last_of('/') + 1);
   (void)n_total_pad;
   if (l->bias) {
     const std::vector<float>& B = P(h, scope + "/conv_B");
     for (int co = 0; co < l->cout; ++co) t.bias_host[col0 + co] = B[co];
   }
-  if (l->prelu) {
-    const std::vector<float>& A = P(h, scope + "/prelu/" + base + "_prelu");
-    for (int co = 0; co < l->cout; ++co) t.alpha_host[col0 + co] = A[co];
-  }
+  if (l->act) layer_slopes(h, *l, t.alpha_host.data() + col0);
 }
 
 static void choose_tiling(int n_total_pad16, int* n_tiles, int* n_pad, int cap = kMaxTileN) {
@@ -517,9 +538,10 @@ static int finalize_params_ds(dcscn_handle* h) {
   ab_pw.assign((size_t)T * (na + nb), 0.f);
   ab_bias.assign(na + nb, 0.f);
   ab_alpha.assign(na + nb, 1.f);
+  // slope vectors for prelu / relu / leaky_relu; sigmoid, tanh and selu have none (ds_activate)
+  const bool slopes = h->cfg.activator <= DCSCN_ACTIVATOR_LEAKY_RELU;
   for (size_t i = 0; i < h->layers.size(); ++i) {
     const LayerDef& l = h->layers[i];
-    std::string base = l.scope.substr(l.scope.find_last_of('/') == std::string::npos ? 0 : l.scope.find_last_of('/') + 1);
     const std::vector<float>& dwv = P(h, l.scope + "/depthwise_W");   // [k,k,cin,1] == [taps][cin]
     const std::vector<float>& pwv = P(h, l.scope + "/pointwise_W");   // [1,1,cin,cout] == [cin][cout]
     if (l.scope == "A1" || l.scope == "B1") {
@@ -534,18 +556,20 @@ static int finalize_params_ds(dcscn_handle* h) {
             if (l.k == 1) ab_pw[(size_t)pos * (na + nb) + col0 + co] = dwv[ci] * pwv[(size_t)ci * l.cout + co];
         }
       const auto& B = P(h, l.scope + "/conv_B");
-      const auto& A = P(h, l.scope + "/prelu/" + base + "_prelu");
-      for (int co = 0; co < l.cout; ++co) {
-        ab_bias[col0 + co] = B[co];
-        ab_alpha[col0 + co] = A[co];
-      }
+      for (int co = 0; co < l.cout; ++co) ab_bias[col0 + co] = B[co];
+      layer_slopes(h, l, ab_alpha.data() + col0);
       continue;
     }
     if (upload(&h->ds[i].dw, dwv, h) || upload(&h->ds[i].pw, pwv, h)) return 1;
     if (l.bias && upload(&h->ds[i].bias, P(h, l.scope + "/conv_B"), h)) return 1;
-    if (l.prelu && upload(&h->ds[i].alpha, P(h, l.scope + "/prelu/" + base + "_prelu"), h)) return 1;
+    if (l.act) {
+      std::vector<float> a(l.cout);
+      layer_slopes(h, l, a.data());
+      if (slopes && upload(&h->ds[i].alpha, a, h)) return 1;
+    }
   }
-  if (upload(&h->ds_ab.pw, ab_pw, h) || upload(&h->ds_ab.bias, ab_bias, h) || upload(&h->ds_ab.alpha, ab_alpha, h)) return 1;
+  if (upload(&h->ds_ab.pw, ab_pw, h) || upload(&h->ds_ab.bias, ab_bias, h)) return 1;
+  if (slopes && upload(&h->ds_ab.alpha, ab_alpha, h)) return 1;
   h->params_dirty = false;
   return 0;
 }
@@ -553,7 +577,7 @@ static int finalize_params_ds(dcscn_handle* h) {
 static int build_bwd_layers(dcscn_handle* h);
 static int sync_host_params(dcscn_handle* h);   // train_engine.inc: device master copy -> host, when newer
 
-// CNN1's device vectors (CUDA cores): filter [taps][n_pad], bias, PReLU slope, padded to the slot width.
+// CNN1's device vectors (CUDA cores): filter [taps][n_pad], bias, slope (layer_slopes), padded to the slot width.
 static void first_layer_vectors(const dcscn_handle* h, std::vector<float>& w, std::vector<float>& b, std::vector<float>& a) {
   const LayerDef* l = find_layer(h, "CNN1");
   const int taps = l->k * l->k, np = h->feat_w[0];
@@ -564,11 +588,8 @@ static void first_layer_vectors(const dcscn_handle* h, std::vector<float>& w, st
   for (int tp = 0; tp < taps; ++tp)
     for (int co = 0; co < l->cout; ++co) w[(size_t)tp * np + co] = W[(size_t)tp * l->cout + co];
   const auto& B = P(h, "CNN1/conv_B");
-  const auto& A = P(h, "CNN1/prelu/CNN1_prelu");
-  for (int co = 0; co < l->cout; ++co) {
-    b[co] = B[co];
-    a[co] = A[co];
-  }
+  for (int co = 0; co < l->cout; ++co) b[co] = B[co];
+  layer_slopes(h, *l, a.data());
 }
 
 // Fills h->tcl (forward tensor-core layers) and, when training, h->bwd (their dgrad twins) from the parameters P().
@@ -923,11 +944,13 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
   pl->first.epi = epi_planes(h->feat_hi, lo(h->feat_lo, 0), h->feat_pitch, 0, h->feat_w[0]);
   pl->first.epi.bias = h->d_first_bias;
   pl->first.epi.alpha = h->d_first_alpha;
+  pl->first.epi.act = c.activator;
   pl->first.epi.n_valid = h->filters[0];
 
   size_t ti = 0;
   for (int i = 1; i < c.layers; ++i, ++ti) {
     EpiParams e = epi_planes(h->feat_hi + h->feat_off[i], lo(h->feat_lo, h->feat_off[i]), h->feat_pitch, 0, h->feat_w[i]);
+    e.act = c.activator;
     if (add_tc_launch(h, pl.get(), h->tcl[ti], h->feat_hi + h->feat_off[i - 1], lo(h->feat_lo, h->feat_off[i - 1]),
                       h->feat_pitch, n, H, W, e))
       return nullptr;
@@ -936,10 +959,12 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
     EpiParams e = epi_planes(h->nin_hi + h->b1_w, lo(h->nin_lo, h->b1_w), h->nin_pitch, 0, h->a1_w);
     e.num_seg = 2;
     e.seg[1] = {h->a1_w, h->a1_w + h->b1_w, h->b1_hi, two ? h->b1_lo : nullptr, h->b1_w};
+    e.act = c.activator;
     if (add_tc_launch(h, pl.get(), h->tcl[ti++], h->feat_hi, lo(h->feat_lo, 0), h->feat_pitch, n, H, W, e)) return nullptr;
   }
   {  // B2 -> nin[:, 0:b1_w]
     EpiParams e = epi_planes(h->nin_hi, lo(h->nin_lo, 0), h->nin_pitch, 0, h->b1_w);
+    e.act = c.activator;
     if (add_tc_launch(h, pl.get(), h->tcl[ti++], h->b1_hi, two ? h->b1_lo : nullptr, h->b1_w, n, H, W, e)) return nullptr;
   }
   int HR_H = H, HR_W = W;
@@ -1138,6 +1163,17 @@ static DsTileParams ds_tile_params(const LayerDef& l, const dcscn_handle::DsDev&
   return p;
 }
 
+// sigmoid / tanh / selu of an activated depthwise-separable layer (see ds_act_kernel); nothing for the other activators.
+static int ds_activate(dcscn_handle* h, float* buf, long long npx, int pitch, int off, int C, cudaStream_t st) {
+  if (h->cfg.activator < DCSCN_ACTIVATOR_SIGMOID) return 0;
+  const long long total = npx * C;
+  ds_act_kernel<<<(int)std::min<long long>((total + 255) / 256, (long long)h->sm_count * 16), 256, 0, st>>>(buf, npx, pitch, off, C,
+                                                                                                          h->cfg.activator);
+  CUDA_TRY(cudaGetLastError());
+  h->launches++;
+  return 0;
+}
+
 // Depthwise-separable graph (DCSCN.py:246-249, 264-271, 318-320; tf_graph.py:240-243): fp32 NHWC, CUDA cores.
 static int forward_ds_tile(dcscn_handle* h, const float* x, const float* x2, float* y, int n, int H, int W, cudaStream_t st) {
   const dcscn_config& c = h->cfg;
@@ -1151,6 +1187,7 @@ static int forward_ds_tile(dcscn_handle* h, const float* x, const float* x2, flo
     const float* src = i == 0 ? x : h->ds_feat + h->ds_off[i - 1];
     DsTileParams p = ds_tile_params(h->layers[li], h->ds[li], src, i == 0 ? c.channels : T, h->ds_feat, T, h->ds_off[i], n, H, W);
     if (launch_ds_tile(h, p, h->layers[li].k, st)) return 1;
+    if (ds_activate(h, h->ds_feat, (long long)n * H * W, T, h->ds_off[i], h->filters[i], st)) return 1;
   }
   {  // A1 | B1: both are 1x1 over the whole concat buffer -> ONE pass; the per-channel depthwise scales are folded into the
      // pointwise rows.  Columns [0, na) = A1 -> [B2 | A1] buffer at channel nb; columns [na, na+nb) = B1 -> B1 buffer.
@@ -1163,11 +1200,14 @@ static int forward_ds_tile(dcscn_handle* h, const float* x, const float* x2, flo
     p.dst2 = h->ds_b1; p.dst2_pitch = nb; p.dst2_off = 0;
     if (cps > 32) return fail("depthwise-separable graph: nin_filters + nin_filters2 = %d > 32 is not supported by the fused A1|B1 kernel", cps);
     if (launch_ds_tile(h, p, 1, st)) return 1;
+    if (ds_activate(h, h->ds_nin, (long long)n * H * W, cps, nb, na, st) || ds_activate(h, h->ds_b1, (long long)n * H * W, nb, 0, nb, st))
+      return 1;
     li += 2;
   }
   {  // B2
     DsTileParams p = ds_tile_params(h->layers[li], h->ds[li], h->ds_b1, nb, h->ds_nin, cps, 0, n, H, W);
     if (launch_ds_tile(h, p, h->layers[li].k, st)) return 1;
+    if (ds_activate(h, h->ds_nin, (long long)n * H * W, cps, 0, nb, st)) return 1;
     ++li;
   }
   int HH = H, WW = W;

@@ -27,6 +27,36 @@ __host__ __device__ __forceinline__ bool dropout_keep(uint32_t seed, uint32_t la
   return (float)(dropout_hash(seed, layer, idx) >> 8) * (1.0f / 16777216.0f) < keep_prob;
 }
 
+// TensorFlow's selu constants: lambda and lambda * alpha (tf.nn.selu, SeluGrad).
+constexpr float kSeluScale = 1.0507009873554805f;
+constexpr float kSeluScaleAlpha = 1.7580993408473766f;
+constexpr float kLeakySlope = 0.1f;   // build_activator's leaky_relu_alpha (tf_graph.py:77)
+
+// sigmoid, tanh or selu of z in fp32 with the accurate libdevice functions (the build has no --use_fast_math).
+__device__ __forceinline__ float act_curve(int act, float z) {
+  if (act == ACT_SIGMOID) return 1.0f / (1.0f + expf(-z));
+  if (act == ACT_TANH) return tanhf(z);
+  return z < 0.f ? kSeluScaleAlpha * expm1f(z) : kSeluScale * z;
+}
+
+// The same as an out-of-line call: inlined at every epilogue site, the libdevice code grew conv_tc_kernel enough to
+// slow the PReLU graph by 4 % (bench.py headline), with unchanged registers.
+__device__ __noinline__ float act_curve_call(int act, float z) { return act_curve(act, z); }
+
+// f(z) of an activated layer; `a` is the slope below zero of prelu / relu / leaky_relu.
+__device__ __forceinline__ float act_apply(int act, float z, float a) {
+  return act >= ACT_SIGMOID ? act_curve(act, z) : (z > 0.f ? z : a * z);
+}
+
+// f'(z) of relu, sigmoid, tanh and selu from the output h = f(z), the rule of TensorFlow's ReluGrad, SigmoidGrad,
+// TanhGrad and SeluGrad: relu' = [h > 0] (0 at z = 0), selu' = lambda at z = 0.
+__device__ __forceinline__ float act_deriv_from_output(int act, float h) {
+  if (act == ACT_RELU) return h > 0.f ? 1.f : 0.f;
+  if (act == ACT_SIGMOID) return h * (1.f - h);
+  if (act == ACT_TANH) return 1.f - h * h;
+  return h < 0.f ? h + kSeluScaleAlpha : kSeluScale;
+}
+
 __device__ __forceinline__ uint32_t pack_h2(__half a, __half b) {
   return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
 }
@@ -63,8 +93,8 @@ __device__ __forceinline__ void store_planes16(__half* dst_hi, __half* dst_lo, s
   if (dst_lo != nullptr) store_words8(dst_lo + off, pl);
 }
 
-// acc * out_scale + bias -> PReLU -> [inverted dropout] of 16 consecutive GEMM columns starting at `cg`; zn = fp16 pairs of
-// min(z, 0), only formed when `want_zneg`.
+// acc * out_scale + bias -> activation -> [inverted dropout] of 16 consecutive GEMM columns starting at `cg`; zn = fp16
+// pairs of min(z, 0), only formed when `want_zneg`.
 __device__ __forceinline__ void epilogue_values16(const EpiParams& e, const ConvGeom& g, int n_total, int img, int y, int x,
                                                   int cg, const float (&acc)[16], float (&v)[16], uint32_t (&zn)[8],
                                                   bool want_zneg) {
@@ -88,6 +118,10 @@ __device__ __forceinline__ void epilogue_values16(const EpiParams& e, const Conv
       zn[2 * q] = *reinterpret_cast<const uint32_t*>(&z01);
       zn[2 * q + 1] = *reinterpret_cast<const uint32_t*>(&z23);
     }
+  }
+  if (e.act >= ACT_SIGMOID) {   // these layers carry slope 1, so v == z here; an out-of-line call keeps the code small
+#pragma unroll
+    for (int i = 0; i < 16; ++i) v[i] = act_curve_call(e.act, v[i]);
   }
   if (e.keep_prob < 1.0f) {
     const float inv_keep = 1.0f / e.keep_prob;

@@ -346,11 +346,12 @@ __global__ void __launch_bounds__(256) s2d_planes_kernel(const S2dParams p) {
 }
 
 // -------------------------------------------------------------- PReLU + dropout gradient, bias / alpha sums ----
-// out = dropout(prelu(z)) (tf_graph.py:126-130).  g = dL/d out (sum of up to two plane tensors).
-//   dZ     = g * keepmask/keep * (z > 0 ? 1 : alpha)
-//   dalpha = sum g * keepmask/keep * min(z, 0)          db = sum dZ
-// z is recovered from the stored forward output (alpha > 0 is required): z < 0 <=> out < 0, z = out * keep / alpha.
-// Layers without activation (alpha == nullptr): dZ = g.
+// out = dropout(f(z)) (tf_graph.py:126-130).  g = dL/d out (sum of up to two plane tensors), dh = g * keepmask/keep.
+//   prelu:       dZ = dh * (z < 0 ? alpha : 1)      dalpha = sum dh * min(z, 0)        (from the min(z, 0) plane)
+//   leaky_relu:  dZ = dh * (z < 0 ? 0.1f : 1)       (from the min(z, 0) plane: slope 1 at z = 0, like Maximum's gradient)
+//   relu, sigmoid, tanh, selu: dZ = dh * f'(z) from the stored forward output y = h / keep of a kept element,
+//                h = y * keep, as TensorFlow's ReluGrad / SigmoidGrad / TanhGrad / SeluGrad take it from h
+//   db = sum dZ.  Layers without activation (act == ACT_NONE): dZ = g.
 struct ActGradParams {
   size_t pixels;
   int C;                 // logical channels
@@ -359,12 +360,14 @@ struct ActGradParams {
   const __half *g1_hi, *g1_lo; int g1_pitch;   // gradient source 1 (already offset to channel 0 of this tensor)
   const __half *g2_hi, *g2_lo; int g2_pitch;   // optional source 2 (nullptr: none)
   const __half* zneg; int zneg_pitch;          // min(z, 0) of the forward pre-activation (EpiSegment::dst_zneg), fp16
-  const float* alpha;    // [C] or nullptr
+  const __half *y_hi, *y_lo; int y_pitch;      // the layer's stored forward output (relu, sigmoid, tanh, selu)
+  int act;               // Activation
+  const float* alpha;    // [C] PReLU slope (prelu only)
   float keep;
   uint32_t seed, layer;
   __half *dz_hi, *dz_lo; int dz_pitch;         // result planes (pad channels must stay zero)
   float* dbias;          // [C] accumulators (scaled by grad_scale) or nullptr
-  float* dalpha;         // [C] or nullptr
+  float* dalpha;         // [C] or nullptr (prelu only)
   int px_per_block;
 };
 
@@ -389,7 +392,8 @@ __global__ void __launch_bounds__(256) act_grad_kernel(const ActGradParams p) {
   const float inv_keep = 1.0f / p.keep;
   const int c = 2 * threadIdx.x;
   const bool v0 = c < p.C, v1 = c + 1 < p.C;
-  float a0 = 1.f, a1 = 1.f;
+  const bool by_zneg = p.act == ACT_PRELU || p.act == ACT_LEAKY_RELU;
+  float a0 = kLeakySlope, a1 = kLeakySlope;
   if (p.alpha) {
     if (v0) a0 = __ldg(p.alpha + c);
     if (v1) a1 = __ldg(p.alpha + c + 1);
@@ -405,12 +409,12 @@ __global__ void __launch_bounds__(256) act_grad_kernel(const ActGradParams p) {
         g.y += g2.y;
       }
       float2 dz = g;
-      if (p.alpha != nullptr) {
-        if (p.keep < 1.0f) {
-          const uint64_t e = (uint64_t)q * (uint64_t)p.n_total + p.col0 + c;
-          g.x = dropout_keep(p.seed, p.layer, e, p.keep) ? g.x * inv_keep : 0.f;
-          g.y = dropout_keep(p.seed, p.layer, e + 1, p.keep) ? g.y * inv_keep : 0.f;
-        }
+      if (p.act != ACT_NONE && p.keep < 1.0f) {
+        const uint64_t e = (uint64_t)q * (uint64_t)p.n_total + p.col0 + c;
+        g.x = dropout_keep(p.seed, p.layer, e, p.keep) ? g.x * inv_keep : 0.f;
+        g.y = dropout_keep(p.seed, p.layer, e + 1, p.keep) ? g.y * inv_keep : 0.f;
+      }
+      if (by_zneg) {
         // PReLU backward from the pre-activation itself: z < 0 -> dz = g * alpha and d alpha += g * z.  (Deciding by the
         // sign of the OUTPUT is wrong for alpha <= 0 - alpha * z is then >= 0 - and shipped checkpoints have many
         // negative slopes; recovering z as output / alpha also breaks down as alpha -> 0.)
@@ -424,6 +428,10 @@ __global__ void __launch_bounds__(256) act_grad_kernel(const ActGradParams p) {
           sa1 = fmaf(g.y, zn.y, sa1);
           dz.y = g.y * a1;
         }
+      } else if (p.act != ACT_NONE) {
+        const float2 y = load_planes2(p.y_hi, p.y_lo, q * p.y_pitch + c);
+        dz.x = g.x * act_deriv_from_output(p.act, y.x * p.keep);
+        dz.y = g.y * act_deriv_from_output(p.act, y.y * p.keep);
       }
       if (!v1) dz.y = 0.f;                          // pad channels of the result stay zero
       sb0 += dz.x;
@@ -478,7 +486,7 @@ __global__ void __launch_bounds__(256) act_grad8_kernel(const ActGradParams p) {
   float a[8], sb[8], sa[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
-    a[i] = (p.alpha != nullptr && c + i < p.C) ? __ldg(p.alpha + c + i) : 1.f;
+    a[i] = (p.alpha != nullptr && c + i < p.C) ? __ldg(p.alpha + c + i) : kLeakySlope;
     sb[i] = 0.f;
     sa[i] = 0.f;
   }
@@ -504,7 +512,7 @@ __global__ void __launch_bounds__(256) act_grad8_kernel(const ActGradParams p) {
         for (int i = 0; i < 8; ++i) g[i] += u[i];          // same association as the pair kernel: (g1h + g1l) + (g2h + g2l)
       }
       float dz[8];
-      if (p.alpha != nullptr) {
+      if (p.act == ACT_PRELU || p.act == ACT_LEAKY_RELU) {
         float zn[8];
         unpack8(__ldg(reinterpret_cast<const uint4*>(p.zneg + q * p.zneg_pitch + c)), zn);
         const uint64_t e = (uint64_t)q * (uint64_t)p.n_total + p.col0 + c;
@@ -517,6 +525,21 @@ __global__ void __launch_bounds__(256) act_grad8_kernel(const ActGradParams p) {
             sa[i] = fmaf(gi, zn[i], sa[i]);
             dz[i] = gi * a[i];
           }
+        }
+      } else if (p.act != ACT_NONE) {                      // derivative from the stored output (see above)
+        float y[8];
+        unpack8(__ldg(reinterpret_cast<const uint4*>(p.y_hi + q * p.y_pitch + c)), y);
+        if (p.y_lo != nullptr) {
+          unpack8(__ldg(reinterpret_cast<const uint4*>(p.y_lo + q * p.y_pitch + c)), t);
+#pragma unroll
+          for (int i = 0; i < 8; ++i) y[i] += t[i];
+        }
+        const uint64_t e = (uint64_t)q * (uint64_t)p.n_total + p.col0 + c;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          float gi = g[i];
+          if (p.keep < 1.0f) gi = dropout_keep(p.seed, p.layer, e + i, p.keep) ? gi * inv_keep : 0.f;
+          dz[i] = gi * act_deriv_from_output(p.act, y[i] * p.keep);
         }
       } else {
 #pragma unroll

@@ -3,8 +3,10 @@
 // gradient ops of DCSCN.py:334-413).  fp32 on CUDA cores: a depthwise-separable c-DCSCN has 14 kMAC per LR pixel and at
 // most 131 x 32 pointwise filters; the step is bound by memory traffic and launch count, not by arithmetic.
 //
-// One layer, forward:   u = depthwise(x, dw);  z = u . pw + b;  h = PReLU(z);  out = dropout(h)
-//            backward:  g = d out;  dh = g * mask / keep;  dz = dh * (z > 0 ? 1 : alpha);  d alpha += dh * min(z, 0);  d b += dz
+// One layer, forward:   u = depthwise(x, dw);  z = u . pw + b;  h = f(z);  out = dropout(h)
+//            backward:  g = d out;  dh = g * mask / keep;  dz = dh * f'(z);  d b += dz;  with PReLU f'(z) = z > 0 ? 1 : alpha
+//                       and d alpha += dh * min(z, 0); the other activators take f' at z = 0 as TensorFlow's gradient ops
+//                       do (act_grad_kernel, train.cuh)
 //                       d pw[c][co] = sum_px u[px][c] dz[px][co];   du[px][c] = sum_co dz[px][co] pw[c][co]
 //                       d dw[t][c] = sum_px x[px + t][c] du[px][c];  dx[px][c] (+)= sum_t du[px - t][c] dw[t][c]
 // u is recomputed in the backward pass (one cheap kernel) instead of being kept; z (the pre-activation) is kept per layer.
@@ -46,14 +48,15 @@ struct DsPwParams {
   const float* u;        // [px][cin]
   const float* pw;       // [cin][cout]
   const float* bias;     // [cout] or null
-  const float* alpha;    // [cout] or null (no activation)
+  const float* alpha;    // [cout] PReLU slope, or null
   float* z;              // [px][cout] pre-activation, kept for the backward pass
   float* dst;            // layer output: (px, co) at dst[px * dst_pitch + dst_off + co], or depth_to_space scattered
   int dst_pitch, dst_off;
   int d2s_r, d2s_C;      // DCR: column (i*r + j)*C + c -> pixel (y*r + i, x*r + j), channel c
   const float* add;      // + x2 (cout == 1), or null
-  float keep;            // dropout keep probability (only applied when alpha != null, tf_graph.py:129-130)
+  float keep;            // dropout keep probability (only applied to activated layers, tf_graph.py:129-130)
   uint32_t seed, layer;
+  int act;               // Activation; ACT_NONE = linear layer
 };
 
 __global__ void __launch_bounds__(256) ds_pw_fwd_kernel(const DsPwParams p) {
@@ -66,8 +69,8 @@ __global__ void __launch_bounds__(256) ds_pw_fwd_kernel(const DsPwParams p) {
     for (int c = 0; c < p.cin; ++c) acc = fmaf(__ldg(ur + c), __ldg(p.pw + (size_t)c * p.cout + co), acc);
     p.z[i] = acc;
     float hv = acc;
-    if (p.alpha) {
-      hv = acc > 0.f ? acc : __ldg(p.alpha + co) * acc;
+    if (p.act != ACT_NONE) {
+      hv = act_apply(p.act, acc, p.alpha ? __ldg(p.alpha + co) : (p.act == ACT_LEAKY_RELU ? kLeakySlope : 0.f));
       if (p.keep < 1.0f) hv = dropout_keep(p.seed, p.layer, (uint64_t)i, p.keep) ? hv * (1.0f / p.keep) : 0.f;
     }
     if (p.d2s_r == 0) {
@@ -92,11 +95,12 @@ struct DsActBwdParams {
   int g_pitch, g_off;
   int d2s_r, d2s_C;
   const float* z;        // [px][cout]
-  const float* alpha;    // or null
+  const float* alpha;    // PReLU slope, or null
   float keep;
   uint32_t seed, layer;
   float* dz;             // [px][cout]
-  float* e;              // [px][cout]: dh * min(z, 0) (column sums = d alpha); only written when alpha != null
+  float* e;              // [px][cout]: dh * min(z, 0) (column sums = d alpha); only written for PReLU
+  int act;               // Activation; ACT_NONE = linear layer
 };
 
 __global__ void __launch_bounds__(256) ds_act_bwd_kernel(const DsActBwdParams p) {
@@ -115,11 +119,17 @@ __global__ void __launch_bounds__(256) ds_act_bwd_kernel(const DsActBwdParams p)
       const long long hp = (img * p.H * r + (long long)(y * r + ii)) * ((long long)p.W * r) + (x * r + jj);
       g = __ldg(p.gout + hp * p.g_pitch + p.g_off + c);
     }
-    if (p.alpha) {
+    if (p.act != ACT_NONE) {
       if (p.keep < 1.0f) g = dropout_keep(p.seed, p.layer, (uint64_t)i, p.keep) ? g * (1.0f / p.keep) : 0.f;
       const float zz = p.z[i];
-      p.e[i] = g * fminf(zz, 0.f);
-      g = zz > 0.f ? g : __ldg(p.alpha + co) * g;
+      if (p.act == ACT_PRELU) {
+        p.e[i] = g * fminf(zz, 0.f);
+        g = zz > 0.f ? g : __ldg(p.alpha + co) * g;
+      } else if (p.act == ACT_LEAKY_RELU) {
+        g = zz < 0.f ? kLeakySlope * g : g;        // Maximum's gradient: z >= 0.1 z takes the z branch, slope 1 at z = 0
+      } else {
+        g *= act_deriv_from_output(p.act, act_apply(p.act, zz, 0.f));
+      }
     }
     p.dz[i] = g;
   }

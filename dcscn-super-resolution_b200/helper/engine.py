@@ -19,6 +19,9 @@ LIB_PATH = os.environ.get("DCSCN_B200_LIB") or os.path.join(os.path.dirname(_HER
 PRECISION_F16X3 = 0
 PRECISION_F16X1 = 1
 
+# DCSCN_ACTIVATOR_* (--activator)
+ACTIVATORS = {"prelu": 0, "relu": 1, "leaky_relu": 2, "sigmoid": 3, "tanh": 4, "selu": 5}
+
 
 class DcscnConfig(ctypes.Structure):
     """Mirror of `struct dcscn_config` (include/dcscn_b200.h)."""
@@ -46,6 +49,7 @@ class DcscnConfig(ctypes.Structure):
         ("epsilon", ctypes.c_float),
         ("device_id", ctypes.c_int32),
         ("precision", ctypes.c_int32),
+        ("activator", ctypes.c_int32),
     ]
 
 
@@ -128,7 +132,7 @@ def make_config(scale=2, layers=12, filters=196, min_filters=48, filters_decay_g
                 nin_filters=64, nin_filters2=32, cnn_size=3, reconstruct_layers=1, reconstruct_filters=32,
                 pixel_shuffler_filters=0, depthwise_separable=False, channels=1, dropout_keep=0.8,
                 l2_decay=0.0001, clipping_norm=5.0, beta1=0.9, beta2=0.999, epsilon=1e-8, device_id=0,
-                precision=PRECISION_F16X3):
+                precision=PRECISION_F16X3, activator="prelu"):
     c = DcscnConfig()
     c.struct_size = ctypes.sizeof(DcscnConfig)
     c.scale, c.layers, c.filters, c.min_filters = scale, layers, filters, min_filters
@@ -139,6 +143,7 @@ def make_config(scale=2, layers=12, filters=196, min_filters=48, filters_decay_g
     c.dropout_keep, c.l2_decay, c.clipping_norm = dropout_keep, l2_decay, clipping_norm
     c.beta1, c.beta2, c.epsilon = beta1, beta2, epsilon
     c.device_id, c.precision = device_id, precision
+    c.activator = ACTIVATORS[activator]
     return c
 
 

@@ -27,6 +27,19 @@ enum {
   DCSCN_PRECISION_F16X1 = 1  /* single-pass fp16 operands (PSNR-neutral, not 1e-3-pixel exact) */
 };
 
+/* Point-wise activation of CNN1..CNNL, A1, B1 and B2 (--activator, helper/tf_graph.py:77-102).  Up-PS, Up-PS2 and R-CNN1
+ * stay linear.  Only prelu has a variable (a per-channel slope, initialised to 0.1); leaky_relu is max(z, 0.1 z); selu uses
+ * TensorFlow's lambda = 1.0507009873554805 and alpha = 1.6732632423543772.  Gradients follow TensorFlow's gradient ops,
+ * also at z = 0: relu' = 0, leaky_relu' = 1, selu' = lambda there. */
+enum {
+  DCSCN_ACTIVATOR_PRELU = 0,
+  DCSCN_ACTIVATOR_RELU = 1,
+  DCSCN_ACTIVATOR_LEAKY_RELU = 2,
+  DCSCN_ACTIVATOR_SIGMOID = 3,
+  DCSCN_ACTIVATOR_TANH = 4,
+  DCSCN_ACTIVATOR_SELU = 5
+};
+
 /*
  * Graph hyper-parameters: the subset of helper/args.py:16-98 flags that shape the graph built by
  * DCSCN.SuperResolution.__init__ (DCSCN.py:29-106) and build_graph (DCSCN.py:222-332).
@@ -53,6 +66,7 @@ typedef struct dcscn_config {
   float beta1, beta2, epsilon;    /* --beta1 --beta2 --epsilon (Adam) */
   int32_t device_id;              /* --gpu_device_id */
   int32_t precision;              /* DCSCN_PRECISION_* */
+  int32_t activator;              /* --activator: DCSCN_ACTIVATOR_* (0 = prelu) */
 } dcscn_config;
 
 /* SuperResolution(flags) + build_graph() + init_session (DCSCN.py:29, :222; tf_graph.py:65). */
@@ -65,6 +79,7 @@ const char* dcscn_last_error(void);
  * Variables of the graph, named exactly like the TF variables in the reference's checkpoints
  * (tf.train.Saver, tf_graph.py:263-296): "CNN1/conv_W" [k,k,cin,cout] HWIO, "CNN1/conv_B",
  * "CNN1/prelu/CNN1_prelu", "A1/...", "B1/...", "B2/...", "Up-PS/Up-PS_CNN/conv_W", "R-CNN1/conv_W" ...
+ * The "<scope>/prelu/<scope>_prelu" slopes exist only with DCSCN_ACTIVATOR_PRELU; the other activators have no variable.
  */
 int dcscn_num_params(dcscn_handle* h);
 int dcscn_param_info(dcscn_handle* h, int index, char* name_buf, int name_buf_len, int64_t* dims4, int* ndim);
