@@ -87,6 +87,10 @@ def _all_reduce_sum(array):
 
 
 class SuperResolution:
+    # defaults of --optimizer / --momentum, for instances whose attributes are set without the constructor
+    optimizer = "adam"
+    momentum = 0.9
+
     def __init__(self, flags, model_name=""):
         # ---- TensorflowGraph.__init__ (tf_graph.py:19-63) ----
         self.dropout_rate = flags.dropout_rate
@@ -229,8 +233,6 @@ class SuperResolution:
             problems.append("--channels=%d" % self.channels)
         if self.reconstruct_layers != 1:
             problems.append("--reconstruct_layers=%d" % self.reconstruct_layers)
-        if self.optimizer != "adam":
-            problems.append("--optimizer=%s (only adam)" % self.optimizer)
         if problems:
             raise NotImplementedError("not supported by the H100 engine: " + ", ".join(problems))
 
@@ -238,6 +240,8 @@ class SuperResolution:
     def _engine_config(self):
         if self.activator not in eng.ACTIVATORS:
             raise NameError("Not implemented activator:%s" % self.activator)   # tf_graph.py:98, at build_graph
+        if self.optimizer not in eng.OPTIMIZERS:   # the message of add_optimizer_op (DCSCN.py:391)
+            raise ValueError("Optimizer arg should be one of [gd, adadelta, adagrad, adam, momentum, rmsprop].")
         prec = {"f16x3": eng.PRECISION_F16X3, "f16x1": eng.PRECISION_F16X1}[self.precision]
         return eng.make_config(
             scale=self.scale, layers=self.layers, filters=self.filters, min_filters=self.min_filters,
@@ -246,7 +250,8 @@ class SuperResolution:
             reconstruct_filters=self.reconstruct_filters, pixel_shuffler_filters=self.pixel_shuffler_filters,
             depthwise_separable=self.depthwise_separable, channels=self.channels, dropout_keep=self.dropout_rate,
             l2_decay=self.l2_decay, clipping_norm=self.clipping_norm, beta1=self.beta1, beta2=self.beta2,
-            epsilon=self.epsilon, device_id=self.gpu_device_id, precision=prec, activator=self.activator)
+            epsilon=self.epsilon, device_id=self.gpu_device_id, precision=prec, activator=self.activator,
+            optimizer=self.optimizer, momentum=self.momentum)
 
     def build_graph(self):
         """DCSCN.py:222-332: creates the engine (variables at their initial values) and the bookkeeping strings."""
@@ -286,7 +291,7 @@ class SuperResolution:
             self.features, "{:,}".format(self.complexity), self.receptive_fields))
 
     def build_optimizer(self):
-        """DCSCN.py:334-369: the loss / clip / Adam step lives inside the engine's train_step."""
+        """DCSCN.py:334-369: the loss / clip / --optimizer step lives inside the engine's train_step."""
         self.optimizer_built = True
         if self.use_l1_loss:
             self.engine.set_option("l1_loss", 1)
@@ -315,8 +320,8 @@ class SuperResolution:
                 self.engine.set_param(name, np.zeros(shape, np.float32))
             else:
                 self.engine.set_param(name, np.full(shape, 0.1, np.float32))
-        # the reference re-runs tf.global_variables_initializer(), which also zeroes the Adam slots and resets the
-        # beta powers: trials of train.py (--tests > 1) must not inherit the previous trial's moments
+        # the reference re-runs tf.global_variables_initializer(), which also re-initialises the optimizer's slots and
+        # the beta powers: trials of train.py (--tests > 1) must not inherit the previous trial's moments
         self.engine.reset_optimizer()
         print("Model initialized.")
 
@@ -357,7 +362,8 @@ class SuperResolution:
     def load_model(self, name="", trial=0, output_log=False, restore_optimizer=False):
         """tf_graph.py:263-280: restore from the TF V2 bundle `<checkpoint_dir>/<name>.ckpt`.  With
         `restore_optimizer` (train.py resuming a run) the Adam slots `<var>/Adam`, `<var>/Adam_1` and the update count
-        behind `beta1_power` are restored too, as tf.train.Saver.restore does for the graph train.py builds."""
+        behind `beta1_power` are restored too, as tf.train.Saver.restore does for the graph train.py builds; for the
+        other optimizers, their slots (engine.OPTIMIZER_SLOTS) that the file holds."""
         filename = self._ckpt_filename(name, trial)
         if not os.path.isfile(filename + ".index"):
             print("Error. [%s] is not exist!" % filename)
@@ -371,12 +377,17 @@ class SuperResolution:
             weights[var] = reader.get_tensor(var)
         self.engine.set_params(weights)
         self.engine.reset_optimizer()   # weights from a file never keep moments of whatever was trained before
-        if restore_optimizer and reader.has_tensor("beta1_power"):
+        if restore_optimizer and self.optimizer == "adam" and reader.has_tensor("beta1_power"):
             for var in weights:
                 for slot, suffix in enumerate(("/Adam", "/Adam_1")):
                     if reader.has_tensor(var + suffix):
                         self.engine.set_adam_slot(var, slot, reader.get_tensor(var + suffix))
             self.engine.adam_step = self._adam_step_from_powers(reader)
+        elif restore_optimizer and self.optimizer != "adam":
+            for var in weights:
+                for slot, (suffix, _) in enumerate(eng.OPTIMIZER_SLOTS[self.optimizer]):
+                    if reader.has_tensor(var + suffix):
+                        self.engine.set_optimizer_slot(var, slot, reader.get_tensor(var + suffix))
         if output_log:
             logging.info("Model restored [ %s ]." % filename)
         else:
@@ -398,20 +409,26 @@ class SuperResolution:
 
     def save_model(self, name="", trial=0, output_log=False):
         """tf_graph.py:282-296: write `<name>.ckpt.index` + `.data-00000-of-00001` (TF V2 bundle) with everything the
-        reference's tf.train.Saver() writes: the trainables, their Adam slots and beta1_power / beta2_power - so the
-        file restores in the reference's sr.py / train.py graphs (which build the optimizer) as well as here."""
+        reference's tf.train.Saver() writes: the trainables, the --optimizer's slots (engine.OPTIMIZER_SLOTS) and, for
+        Adam, beta1_power / beta2_power - so the file restores in the reference's sr.py / train.py graphs (which build
+        the optimizer) as well as here."""
         filename = self._ckpt_filename(name, trial)
         if _dist_rank_world()[0] != 0:
             return      # data-parallel ranks hold identical weights: rank 0 writes the file
         shapes = self.engine.param_shapes()
         tensors = {var: self.engine.get_param(var) for var in shapes}
-        steps = self.engine.adam_step
-        for var, shape in shapes.items():
-            for slot, suffix in enumerate(("/Adam", "/Adam_1")):
-                tensors[var + suffix] = (self.engine.get_adam_slot(var, slot) if steps > 0
-                                         else np.zeros(shape, dtype=np.float32))
-        tensors["beta1_power"] = np.asarray(self.beta1 ** (steps + 1), dtype=np.float32)
-        tensors["beta2_power"] = np.asarray(self.beta2 ** (steps + 1), dtype=np.float32)
+        if self.optimizer != "adam":
+            for var in shapes:   # the engine returns a slot's initial value until the first step
+                for slot, (suffix, _) in enumerate(eng.OPTIMIZER_SLOTS[self.optimizer]):
+                    tensors[var + suffix] = self.engine.get_optimizer_slot(var, slot)
+        else:
+            steps = self.engine.adam_step
+            for var, shape in shapes.items():
+                for slot, suffix in enumerate(("/Adam", "/Adam_1")):
+                    tensors[var + suffix] = (self.engine.get_adam_slot(var, slot) if steps > 0
+                                             else np.zeros(shape, dtype=np.float32))
+            tensors["beta1_power"] = np.asarray(self.beta1 ** (steps + 1), dtype=np.float32)
+            tensors["beta2_power"] = np.asarray(self.beta2 ** (steps + 1), dtype=np.float32)
         tf_bundle.write_bundle(filename, tensors)
         if output_log:
             logging.info("Model saved [%s]." % filename)
@@ -479,7 +496,7 @@ class SuperResolution:
     def train_batch(self):
         """DCSCN.py:415-425: one optimisation step on the current mini-batch."""
         # data parallel: every rank holds its own batch_num / world patches (init_epoch_index); the gradients meet in
-        # one flat all-reduce before the (identical) clip + Adam update on every rank
+        # one flat all-reduce before the (identical) clip + optimizer update on every rank
         rank, world = _dist_rank_world()
         if getattr(self, "batch_indices", None) is not None:
             if world > 1:

@@ -284,6 +284,8 @@ static void layer_slopes(const dcscn_handle* h, const LayerDef& l, float* dst) {
 static int build_graph(dcscn_handle* h) {
   const dcscn_config& c = h->cfg;
   if (c.activator < DCSCN_ACTIVATOR_PRELU || c.activator > DCSCN_ACTIVATOR_SELU) return fail("activator %d is not one of DCSCN_ACTIVATOR_*", c.activator);
+  if (c.optimizer < DCSCN_OPTIMIZER_ADAM || c.optimizer > DCSCN_OPTIMIZER_RMSPROP) return fail("optimizer %d is not one of DCSCN_OPTIMIZER_*", c.optimizer);
+  if (!std::isfinite(c.momentum)) return fail("momentum must be finite");
   if (!c.use_nin) return fail("use_nin=false is not supported (no shipped checkpoint uses it)");
   if (c.channels != 1) return fail("channels must be 1 (helper/args.py: 'Now it should be 1')");
   if (std::max(c.reconstruct_layers, 1) != 1) return fail("reconstruct_layers > 1 is not supported");
@@ -2113,6 +2115,7 @@ int dcscn_get_grad(dcscn_handle* h, const char* name, float* host_data, int64_t 
 
 int dcscn_get_adam_slot(dcscn_handle* h, const char* name, int slot, float* host_data, int64_t numel) {
   if (!h || !name || !host_data) return fail("dcscn_get_adam_slot: null argument");
+  if (h->cfg.optimizer != DCSCN_OPTIMIZER_ADAM) return fail("dcscn_get_adam_slot: the optimizer is not adam (use dcscn_get_optimizer_slot)");
   if (!h->train || h->train->total == 0) return fail("dcscn_get_adam_slot: no train step has run yet");
   auto it = h->param_index.find(name);
   if (it == h->param_index.end()) return fail("dcscn_get_adam_slot: unknown variable '%s'", name);
@@ -2126,6 +2129,7 @@ int dcscn_get_adam_slot(dcscn_handle* h, const char* name, int slot, float* host
 
 int dcscn_set_adam_slot(dcscn_handle* h, const char* name, int slot, const float* host_data, int64_t numel) {
   if (!h || !name || !host_data) return fail("dcscn_set_adam_slot: null argument");
+  if (h->cfg.optimizer != DCSCN_OPTIMIZER_ADAM) return fail("dcscn_set_adam_slot: the optimizer is not adam (use dcscn_set_optimizer_slot)");
   CUDA_TRY(cudaSetDevice(h->cfg.device_id));
   if (train_init(h)) return 1;
   auto it = h->param_index.find(name);
@@ -2151,12 +2155,51 @@ int dcscn_set_adam_step(dcscn_handle* h, int64_t step) {
   return 0;
 }
 
+int dcscn_optimizer_slot_count(dcscn_handle* h) { return h ? optimizer_slot_count(h->cfg.optimizer) : 0; }
+
+// Resolves (variable, slot) of the configured optimizer to its offset in the flat slot buffers.
+static int optimizer_slot_view(dcscn_handle* h, const char* fn, const char* name, int slot, int64_t numel, size_t* off, float** buf) {
+  auto it = h->param_index.find(name);
+  if (it == h->param_index.end()) return fail("%s: unknown variable '%s'", fn, name);
+  const ParamDef& p = h->params[it->second];
+  if (numel != p.numel()) return fail("%s: '%s' has %lld elements, got %lld", fn, name, (long long)p.numel(), (long long)numel);
+  if (slot < 0 || slot >= optimizer_slot_count(h->cfg.optimizer))
+    return fail("%s: optimizer %d has no slot %d", fn, h->cfg.optimizer, slot);
+  *off = h->train ? h->train->off[it->second] : 0;
+  *buf = !h->train ? nullptr : slot == 0 ? h->train->d_m : h->train->d_v;
+  return 0;
+}
+
+int dcscn_get_optimizer_slot(dcscn_handle* h, const char* name, int slot, float* host_data, int64_t numel) {
+  if (!h || !name || !host_data) return fail("dcscn_get_optimizer_slot: null argument");
+  size_t off;
+  float* buf;
+  if (optimizer_slot_view(h, "dcscn_get_optimizer_slot", name, slot, numel, &off, &buf)) return 1;
+  if (!h->train || h->train->total == 0) {   // no state allocated yet: the slot holds its initial value
+    std::fill(host_data, host_data + numel, optimizer_slot_init(h->cfg.optimizer, slot));
+    return 0;
+  }
+  CUDA_TRY(cudaSetDevice(h->cfg.device_id));
+  CUDA_TRY(cudaMemcpy(host_data, buf + off, (size_t)numel * sizeof(float), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int dcscn_set_optimizer_slot(dcscn_handle* h, const char* name, int slot, const float* host_data, int64_t numel) {
+  if (!h || !name || !host_data) return fail("dcscn_set_optimizer_slot: null argument");
+  CUDA_TRY(cudaSetDevice(h->cfg.device_id));
+  if (train_init(h)) return 1;
+  size_t off;
+  float* buf;
+  if (optimizer_slot_view(h, "dcscn_set_optimizer_slot", name, slot, numel, &off, &buf)) return 1;
+  CUDA_TRY(cudaMemcpy(buf + off, host_data, (size_t)numel * sizeof(float), cudaMemcpyHostToDevice));
+  return 0;
+}
+
 int dcscn_reset_optimizer(dcscn_handle* h) {
   if (!h) return fail("dcscn_reset_optimizer: null argument");
-  if (!h->train || h->train->total == 0) return 0;   // no optimizer state exists yet: slots start at zero anyway
+  if (!h->train || h->train->total == 0) return 0;   // no optimizer state exists yet: train_init starts the slots right
   CUDA_TRY(cudaSetDevice(h->cfg.device_id));
-  CUDA_TRY(cudaMemset(h->train->d_m, 0, h->train->total * sizeof(float)));
-  CUDA_TRY(cudaMemset(h->train->d_v, 0, h->train->total * sizeof(float)));
+  if (reset_optimizer_slots(h)) return 1;
   h->train->step = 0;
   return 0;
 }

@@ -829,6 +829,51 @@ __global__ void __launch_bounds__(256) adam_kernel(const AdamParams p) {
   }
 }
 
+// The other TF1 optimizers of add_optimizer_op (DCSCN.py:380-391) at TF's defaults, on the same clipped gradient; the
+// update rules and slot orders are documented at DCSCN_OPTIMIZER_* (include/dcscn_b200.h).  One instantiation per
+// optimizer, so each reads and writes only its own slots: s0 is slot 0, s1 slot 1.
+struct OptimizerParams {
+  float* w; float* s0; float* s1; const float* grad; size_t count;
+  const double* norm_sq; float clip; float lr, momentum;
+};
+template <int OPT>
+__global__ void __launch_bounds__(256) optimizer_kernel(const OptimizerParams p) {
+  float cscale = 1.f;
+  if (p.clip > 0.f) {
+    const float norm = (float)sqrt(*p.norm_sq);
+    cscale = p.clip / fmaxf(norm, p.clip);
+  }
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < p.count; i += (size_t)gridDim.x * blockDim.x) {
+    const float g = p.grad[i] * cscale;
+    if constexpr (OPT == DCSCN_OPTIMIZER_GD) {
+      p.w[i] -= p.lr * g;
+    } else if constexpr (OPT == DCSCN_OPTIMIZER_MOMENTUM) {
+      const float a = p.momentum * p.s0[i] + g;
+      p.s0[i] = a;
+      p.w[i] -= p.lr * a;
+    } else if constexpr (OPT == DCSCN_OPTIMIZER_ADAGRAD) {
+      const float acc = p.s0[i] + g * g;
+      p.s0[i] = acc;
+      p.w[i] -= p.lr * g / sqrtf(acc);
+    } else if constexpr (OPT == DCSCN_OPTIMIZER_ADADELTA) {
+      constexpr float rho = 0.95f, eps = 1e-8f;
+      const float acc = rho * p.s0[i] + (1.f - rho) * g * g;
+      const float acc_u = p.s1[i];
+      const float u = sqrtf(acc_u + eps) / sqrtf(acc + eps) * g;
+      p.s0[i] = acc;
+      p.s1[i] = rho * acc_u + (1.f - rho) * u * u;
+      p.w[i] -= p.lr * u;
+    } else if constexpr (OPT == DCSCN_OPTIMIZER_RMSPROP) {
+      constexpr float rho = 0.9f, eps = 1e-10f;
+      const float ms = p.s0[i] + (g * g - p.s0[i]) * (1.f - rho);
+      const float mom = p.momentum * p.s1[i] + p.lr * g / sqrtf(ms + eps);
+      p.s0[i] = ms;
+      p.s1[i] = mom;
+      p.w[i] -= mom;
+    }
+  }
+}
+
 
 // ---- device-side refresh of the packed operand images after an optimizer step -------------------------------------
 // dst = operand image (hi plane block, then lo plane block, per [n_tile][tap][chunk]); map[i] = flat

@@ -161,11 +161,11 @@ _REFERENCE_FLAGS = [
     ("initializer", "he", "weight initialiser: uniform, stddev, xavier, he, identity or zero"),
     ("weight_dev", 0.01, "standard deviation for the `stddev` initialiser"),
     ("l2_decay", 0.0001, "weight of the L2 penalty on the convolution filters"),
-    ("optimizer", "adam", "this engine implements adam"),
+    ("optimizer", "adam", "gd, momentum, adadelta, adagrad, adam or rmsprop (TF1 optimizers at TF's defaults)"),
     ("beta1", 0.9, "Adam first-moment decay"),
     ("beta2", 0.999, "Adam second-moment decay"),
     ("epsilon", 1e-8, "Adam epsilon"),
-    ("momentum", 0.9, "only for the momentum / rmsprop optimisers (not carried over)"),
+    ("momentum", 0.9, "momentum of the momentum and rmsprop optimisers"),
     ("batch_num", 20, "patches per training step"),
     ("batch_image_size", 48, "edge length of a low-resolution training patch"),
     ("stride_size", 0, "patch grid stride when building batches; 0 = half a patch"),

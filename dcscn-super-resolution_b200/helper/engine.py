@@ -22,6 +22,19 @@ PRECISION_F16X1 = 1
 # DCSCN_ACTIVATOR_* (--activator)
 ACTIVATORS = {"prelu": 0, "relu": 1, "leaky_relu": 2, "sigmoid": 3, "tanh": 4, "selu": 5}
 
+# DCSCN_OPTIMIZER_* (--optimizer)
+OPTIMIZERS = {"adam": 0, "gd": 1, "momentum": 2, "adadelta": 3, "adagrad": 4, "rmsprop": 5}
+# Checkpoint suffix of each slot, in the engine's slot order, as TF's slot creator names them ("<var>/<Name>", then
+# "<var>/<Name>_1"), and the value the slot starts at.
+OPTIMIZER_SLOTS = {
+    "adam": (("/Adam", 0.0), ("/Adam_1", 0.0)),
+    "gd": (),
+    "momentum": (("/Momentum", 0.0),),
+    "adadelta": (("/Adadelta", 0.0), ("/Adadelta_1", 0.0)),
+    "adagrad": (("/Adagrad", 0.1),),
+    "rmsprop": (("/RMSProp", 1.0), ("/RMSProp_1", 0.0)),
+}
+
 
 class DcscnConfig(ctypes.Structure):
     """Mirror of `struct dcscn_config` (include/dcscn_b200.h)."""
@@ -50,6 +63,8 @@ class DcscnConfig(ctypes.Structure):
         ("device_id", ctypes.c_int32),
         ("precision", ctypes.c_int32),
         ("activator", ctypes.c_int32),
+        ("optimizer", ctypes.c_int32),
+        ("momentum", ctypes.c_float),
     ]
 
 
@@ -60,7 +75,7 @@ EXPORTED_SYMBOLS = [
     "dcscn_train_step", "dcscn_train_step_host", "dcscn_get_grad", "dcscn_get_adam_slot", "dcscn_set_adam_slot", "dcscn_get_adam_step",
     "dcscn_set_adam_step", "dcscn_last_grad_norm",
     "dcscn_patch_store_set", "dcscn_train_step_indexed", "dcscn_patch_gather", "dcscn_dropout_mask", "dcscn_grad_buffer", "dcscn_apply_gradients", "dcscn_apply_gradients_avg", "dcscn_reset_optimizer", "dcscn_graph_replays",
-    "dcscn_tile_halo",
+    "dcscn_tile_halo", "dcscn_optimizer_slot_count", "dcscn_get_optimizer_slot", "dcscn_set_optimizer_slot",
 ]
 
 _lib = None
@@ -124,6 +139,9 @@ def load_library(path=None):
     lib.dcscn_graph_replays.argtypes = [vp]
     lib.dcscn_graph_replays.restype = c64
     lib.dcscn_tile_halo.argtypes = [vp, ctypes.POINTER(ci)]
+    lib.dcscn_optimizer_slot_count.argtypes = [vp]
+    lib.dcscn_get_optimizer_slot.argtypes = [vp, ctypes.c_char_p, ci, fp, c64]
+    lib.dcscn_set_optimizer_slot.argtypes = [vp, ctypes.c_char_p, ci, fp, c64]
     _lib = lib
     return lib
 
@@ -132,7 +150,7 @@ def make_config(scale=2, layers=12, filters=196, min_filters=48, filters_decay_g
                 nin_filters=64, nin_filters2=32, cnn_size=3, reconstruct_layers=1, reconstruct_filters=32,
                 pixel_shuffler_filters=0, depthwise_separable=False, channels=1, dropout_keep=0.8,
                 l2_decay=0.0001, clipping_norm=5.0, beta1=0.9, beta2=0.999, epsilon=1e-8, device_id=0,
-                precision=PRECISION_F16X3, activator="prelu"):
+                precision=PRECISION_F16X3, activator="prelu", optimizer="adam", momentum=0.9):
     c = DcscnConfig()
     c.struct_size = ctypes.sizeof(DcscnConfig)
     c.scale, c.layers, c.filters, c.min_filters = scale, layers, filters, min_filters
@@ -144,6 +162,7 @@ def make_config(scale=2, layers=12, filters=196, min_filters=48, filters_decay_g
     c.beta1, c.beta2, c.epsilon = beta1, beta2, epsilon
     c.device_id, c.precision = device_id, precision
     c.activator = ACTIVATORS[activator]
+    c.optimizer, c.momentum = OPTIMIZERS[optimizer], momentum
     return c
 
 
@@ -427,6 +446,22 @@ class Engine:
                                                  a.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), a.size))
 
     @property
+    def optimizer_slot_count(self):
+        return int(self.lib.dcscn_optimizer_slot_count(self.handle))
+
+    def get_optimizer_slot(self, name, slot):
+        """Slot `slot` of the configured optimizer (order of OPTIMIZER_SLOTS); its initial value before any step."""
+        a = np.empty(self.param_shapes()[name], dtype=np.float32)
+        self._check(self.lib.dcscn_get_optimizer_slot(self.handle, name.encode(), slot,
+                                                      a.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), a.size))
+        return a
+
+    def set_optimizer_slot(self, name, slot, value):
+        a = np.ascontiguousarray(value, dtype=np.float32)
+        self._check(self.lib.dcscn_set_optimizer_slot(self.handle, name.encode(), slot,
+                                                      a.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), a.size))
+
+    @property
     def adam_step(self):
         """Number of optimizer updates applied so far (TF stores beta^(t+1) as beta1_power / beta2_power)."""
         t = ctypes.c_int64()
@@ -438,7 +473,8 @@ class Engine:
         self._check(self.lib.dcscn_set_adam_step(self.handle, int(t)))
 
     def reset_optimizer(self):
-        """Adam slots back to zero and update count to 0 (what re-running the initializer does in the reference)."""
+        """Optimizer slots back to their initial values and update count to 0 (what re-running the initializer does in
+        the reference)."""
         self._check(self.lib.dcscn_reset_optimizer(self.handle))
 
     @property

@@ -40,6 +40,28 @@ enum {
   DCSCN_ACTIVATOR_SELU = 5
 };
 
+/* Update rule of the train step (--optimizer, DCSCN.py:379-413): TF1's training ops at TF's defaults for every argument
+ * the reference does not pass, applied to g = the gradient after the L2 term and clip_by_global_norm, in fp32.  lr is
+ * the step's learning rate, mu = cfg.momentum.  Slots are listed in creation order: slot i is "<var>/<Name>" for i = 0
+ * and "<var>/<Name>_1" for i = 1 in the reference's checkpoints, and starts at the value given.
+ *   ADAM      slots m (0), v (0):       the update documented at dcscn_train_step (cfg.beta1 / beta2 / epsilon)
+ *   GD        no slot:                  w -= lr * g
+ *   MOMENTUM  accum (0):                a = mu * a + g;  w -= lr * a                       (no Nesterov)
+ *   ADADELTA  accum (0), accum_update (0), rho = 0.95, eps = 1e-8:
+ *             acc = rho * acc + (1 - rho) * g^2;  u = sqrt(acc_u + eps) / sqrt(acc + eps) * g;  w -= lr * u;
+ *             acc_u = rho * acc_u + (1 - rho) * u^2                                       (u uses the old acc_u)
+ *   ADAGRAD   accumulator (0.1):        acc += g^2;  w -= lr * g / sqrt(acc)               (no epsilon)
+ *   RMSPROP   rms (1.0), momentum (0), rho = 0.9, eps = 1e-10:
+ *             ms += (g^2 - ms) * (1 - rho);  mom = mu * mom + lr * g / sqrt(ms + eps);  w -= mom   (not centred) */
+enum {
+  DCSCN_OPTIMIZER_ADAM = 0,
+  DCSCN_OPTIMIZER_GD = 1,
+  DCSCN_OPTIMIZER_MOMENTUM = 2,
+  DCSCN_OPTIMIZER_ADADELTA = 3,
+  DCSCN_OPTIMIZER_ADAGRAD = 4,
+  DCSCN_OPTIMIZER_RMSPROP = 5
+};
+
 /*
  * Graph hyper-parameters: the subset of helper/args.py:16-98 flags that shape the graph built by
  * DCSCN.SuperResolution.__init__ (DCSCN.py:29-106) and build_graph (DCSCN.py:222-332).
@@ -67,6 +89,8 @@ typedef struct dcscn_config {
   int32_t device_id;              /* --gpu_device_id */
   int32_t precision;              /* DCSCN_PRECISION_* */
   int32_t activator;              /* --activator: DCSCN_ACTIVATOR_* (0 = prelu) */
+  int32_t optimizer;              /* --optimizer: DCSCN_OPTIMIZER_* (0 = adam) */
+  float momentum;                 /* --momentum (momentum and rmsprop) */
 } dcscn_config;
 
 /* SuperResolution(flags) + build_graph() + init_session (DCSCN.py:29, :222; tf_graph.py:65). */
@@ -122,7 +146,9 @@ int dcscn_forward_ensemble_partial(dcscn_handle* h, const float* x_dev, const fl
  * sess.run([self.training_optimizer, self.image_loss, self.mse], {x, x2, y, lr, dropout: keep, is_training: 1})
  * (DCSCN.py:415-425; graph: build_optimizer / add_optimizer_op, DCSCN.py:334-413): forward with inverted dropout
  * (keep = cfg.dropout_keep, masks from a counter hash of `seed`), mse loss + l2_decay * sum(l2_loss(conv_W)),
- * gradients of every variable, tf.clip_by_global_norm(cfg.clipping_norm), TF-Adam with learning rate `lr`.
+ * gradients of every variable, tf.clip_by_global_norm(cfg.clipping_norm), then the cfg.optimizer update
+ * (DCSCN_OPTIMIZER_*) with learning rate `lr`; for Adam m = b1*m + (1-b1)*g, v = b2*v + (1-b2)*g^2,
+ * w -= lr * sqrt(1-b2^t) / (1-b1^t) * m / (sqrt(v) + eps).
  * `apply_update` = 0 computes loss and gradients only (dcscn_get_grad), leaving the weights untouched.
  * x / x2 / y are DEVICE pointers (dcscn_train_step) or HOST pointers (dcscn_train_step_host); both synchronise.
  */
@@ -146,7 +172,8 @@ int dcscn_train_step_indexed(dcscn_handle* h, const int32_t* indices, int n, flo
 int dcscn_patch_gather(dcscn_handle* h, const int32_t* indices, int n, float max_value, float* x, float* x2, float* y);
 /* d loss / d variable of the LAST train step (after the L2 term, before clipping): tf.gradients(loss, trainables). */
 int dcscn_get_grad(dcscn_handle* h, const char* name, float* host_data, int64_t numel);
-/* Adam slots of a variable ("<var>/Adam" = slot 0, "<var>/Adam_1" = slot 1 in the reference's checkpoints). */
+/* Adam slots of a variable ("<var>/Adam" = slot 0, "<var>/Adam_1" = slot 1 in the reference's checkpoints).  Fail for
+ * any other cfg.optimizer. */
 int dcscn_get_adam_slot(dcscn_handle* h, const char* name, int slot, float* host_data, int64_t numel);
 /* Restoring optimizer state from a checkpoint (what tf.train.Saver.restore does for the graph sr.py / train.py build,
  * helper/tf_graph.py:263-280): the slots, and the number of applied updates t (the reference stores it as
@@ -154,14 +181,22 @@ int dcscn_get_adam_slot(dcscn_handle* h, const char* name, int slot, float* host
 int dcscn_set_adam_slot(dcscn_handle* h, const char* name, int slot, const float* host_data, int64_t numel);
 int dcscn_get_adam_step(dcscn_handle* h, int64_t* step);
 int dcscn_set_adam_step(dcscn_handle* h, int64_t step);
+/* The slots of cfg.optimizer (DCSCN_OPTIMIZER_*): how many each variable has (0 for gd, 1 for momentum and adagrad, 2 for
+ * adam, adadelta and rmsprop), and slot `slot` of variable `name` in the order the enum's comment lists.  Before the first
+ * train step, get returns the slot's initial value. */
+int dcscn_optimizer_slot_count(dcscn_handle* h);
+int dcscn_get_optimizer_slot(dcscn_handle* h, const char* name, int slot, float* host_data, int64_t numel);
+int dcscn_set_optimizer_slot(dcscn_handle* h, const char* name, int slot, const float* host_data, int64_t numel);
 /* tf.global_variables_initializer() on the optimizer's variables (helper/tf_graph.py:73-75 re-runs it for every trial of
- * train.py:100-103): both Adam slots of every variable back to zero and the update count t to 0. */
+ * train.py:100-103): every slot of every variable back to its initial value (see DCSCN_OPTIMIZER_*) and the update
+ * count t to 0. */
 int dcscn_reset_optimizer(dcscn_handle* h);
 /* Data-parallel training: after dcscn_train_step(..., apply_update = 0) on every rank, all-reduce the flat buffer
  * returned here (device pointer, `count` floats: the gradient of every trainable in dcscn_param_info order followed by
  * this rank's {image_loss, mse}) - ONE ncclAllReduce(sum) over NVLink - then call dcscn_apply_gradients_avg on every
  * rank with grad_scale = 1 / ranks: it scales the summed gradients to their mean, applies the global-norm clip of the
- * averaged gradient + Adam identically everywhere (SURVEY.md section 8e) and returns the job-wide mean loss / mse.
+ * averaged gradient + the cfg.optimizer update identically everywhere (SURVEY.md section 8e) and returns the job-wide
+ * mean loss / mse.
  * Every rank must hold the same number of patches (each normalises by its own pixel count).
  * dcscn_apply_gradients is the same with grad_scale = 1 (gradients already averaged by the caller). */
 int dcscn_grad_buffer(dcscn_handle* h, float** dev_ptr, int64_t* count);
