@@ -133,7 +133,7 @@ __global__ void __launch_bounds__(256, 2) conv_first3x3_kernel(const ConvFirstPa
 #pragma unroll
       for (int i = 0; i < 8; i += 2) {
         float t0 = acc[i] + bias[i], t1 = acc[i + 1] + bias[i + 1];
-        if (ZNEG) pz[i >> 1] = pack_h2(__float2half_rn(fmaxf(fminf(t0, 0.f), -65504.f)), __float2half_rn(fmaxf(fminf(t1, 0.f), -65504.f)));
+        if (ZNEG) pz[i >> 1] = pack_h2(__float2half_rn(zneg_value(t0)), __float2half_rn(zneg_value(t1)));
         t0 = t0 > 0.f ? t0 : alpha[i] * t0;
         t1 = t1 > 0.f ? t1 : alpha[i + 1] * t1;
         if (!ZNEG && act >= ACT_SIGMOID) {             // slope 1 on these layers: t0, t1 are still z (their training

@@ -223,6 +223,7 @@ struct dcscn_handle {
   int conv_impl = 0;
   int seg_chunks = 0;                // pipeline stages per fp32-promotion segment; 0 = automatic
   int act_grad_impl = 0;             // 0: 16-byte activation-gradient kernel, 1: channel-pair kernel (cross-check)
+  int grad_capture = 0;              // 1: the train step copies its gradient tensors out (dcscn_get_train_tensor)
   int timing = 0;
   int fuse_last = 1;                 // fold the per-pixel half of R-CNN1 into the last Up-PS epilogue
   std::vector<cudaEvent_t> ev;       // timing events (launch boundaries of the last forward)
@@ -1943,6 +1944,9 @@ int dcscn_set_option(dcscn_handle* h, const char* key, int64_t value) {
   } else if (k == "act_grad_impl") {
     if (value < 0 || value > 1) return fail("act_grad_impl must be 0 or 1");
     h->act_grad_impl = (int)value;
+  } else if (k == "grad_capture") {
+    if (value < 0 || value > 1) return fail("grad_capture must be 0 or 1");
+    h->grad_capture = (int)value;
   } else if (k == "workspace_mb") {
     if (value < 0 || value > (int64_t(1) << 40)) return fail("workspace_mb must be >= 0 MiB (0 = no limit), got %lld", (long long)value);
     h->workspace_mb = value;
@@ -2110,6 +2114,53 @@ int dcscn_get_grad(dcscn_handle* h, const char* name, float* host_data, int64_t 
   if (numel != p.numel()) return fail("dcscn_get_grad: '%s' has %lld elements, got %lld", name, (long long)p.numel(), (long long)numel);
   CUDA_TRY(cudaSetDevice(h->cfg.device_id));
   CUDA_TRY(cudaMemcpy(host_data, h->train->d_g + h->train->off[it->second], (size_t)numel * sizeof(float), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+int dcscn_get_train_tensor(dcscn_handle* h, const char* name, float* host_data, int64_t numel) {
+  if (!h || !name || !host_data) return fail("dcscn_get_train_tensor: null argument");
+  TrainState* t = h->train;
+  if (!t || t->last_px == 0) return fail("dcscn_get_train_tensor: no train step of a tensor-core graph has run yet");
+  CUDA_TRY(cudaSetDevice(h->cfg.device_id));
+  CUDA_TRY(cudaDeviceSynchronize());
+  const std::string s(name);
+  std::vector<__half> hi, lo;
+  size_t px = 0;
+  int ch = 0;
+  if (s.rfind("zneg:", 0) == 0) {   // min(z, 0) planes of the last training forward (prelu / leaky_relu only)
+    if (!needs_zneg(h)) return fail("dcscn_get_train_tensor: '%s': the activator keeps no min(z, 0) planes", name);
+    const std::string l = s.substr(5);
+    const __half* src = nullptr;
+    int pitch = 0;
+    if (l.rfind("CNN", 0) == 0) {
+      const int i = atoi(l.c_str() + 3) - 1;
+      if (i < 0 || i >= h->cfg.layers) return fail("dcscn_get_train_tensor: no tensor '%s'", name);
+      src = t->zneg_feat + h->feat_off[i]; pitch = h->feat_pitch; ch = h->filters[i];
+    } else if (l == "A1") { src = t->zneg_nin + h->b1_w; pitch = h->nin_pitch; ch = h->cfg.nin_filters;
+    } else if (l == "B2") { src = t->zneg_nin; pitch = h->nin_pitch; ch = h->cfg.nin_filters2;
+    } else if (l == "B1") { src = t->zneg_b1; pitch = h->b1_w; ch = h->cfg.nin_filters2;
+    } else return fail("dcscn_get_train_tensor: no tensor '%s'", name);
+    px = t->last_px;
+    hi.resize(px * ch);
+    CUDA_TRY(cudaMemcpy2D(hi.data(), ch * sizeof(__half), src, pitch * sizeof(__half), ch * sizeof(__half), px, cudaMemcpyDeviceToHost));
+  } else {
+    auto it = t->captured.find(s);
+    if (it == t->captured.end())
+      return fail("dcscn_get_train_tensor: no tensor '%s' (set option grad_capture = 1 before the train step)", name);
+    const TrainState::Captured& c = it->second;
+    px = c.px; ch = c.ch;
+    if (numel != (int64_t)(px * ch)) return fail("dcscn_get_train_tensor: '%s' has %lld elements, got %lld", name, (long long)(px * ch), (long long)numel);
+    if (c.f32) {
+      CUDA_TRY(cudaMemcpy(host_data, c.hi, px * sizeof(float), cudaMemcpyDeviceToHost));
+      return 0;
+    }
+    hi.resize(px * ch);
+    lo.resize(px * ch);
+    CUDA_TRY(cudaMemcpy(hi.data(), c.hi, hi.size() * sizeof(__half), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(lo.data(), c.lo, lo.size() * sizeof(__half), cudaMemcpyDeviceToHost));
+  }
+  if (numel != (int64_t)(px * ch)) return fail("dcscn_get_train_tensor: '%s' has %lld elements, got %lld", name, (long long)(px * ch), (long long)numel);
+  for (size_t i = 0; i < hi.size(); ++i) host_data[i] = __half2float(hi[i]) + (lo.empty() ? 0.f : __half2float(lo[i]));
   return 0;
 }
 

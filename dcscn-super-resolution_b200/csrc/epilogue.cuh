@@ -57,6 +57,11 @@ __device__ __forceinline__ float act_deriv_from_output(int act, float h) {
   return h < 0.f ? h + kSeluScaleAlpha : kSeluScale;
 }
 
+// min(z, 0) as the PReLU / leaky_relu backward reads it from its fp16 plane.  A z in (-2^-24, 0) would round to -0 there
+// and take slope 1 (TensorFlow takes alpha for every z < 0), so it is stored as -2^-24, the smallest fp16 subnormal:
+// the sign survives and d alpha = sum g * z moves by at most 2^-24 |g| per such element.
+__device__ __forceinline__ float zneg_value(float t) { return t < 0.f ? fminf(fmaxf(t, -65504.f), -0x1p-24f) : 0.f; }
+
 __device__ __forceinline__ uint32_t pack_h2(__half a, __half b) {
   return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
 }
@@ -113,8 +118,8 @@ __device__ __forceinline__ void epilogue_values16(const EpiParams& e, const Conv
     v[4 * q + 2] = t2 > 0.f ? t2 : a.z * t2;
     v[4 * q + 3] = t3 > 0.f ? t3 : a.w * t3;
     if (want_zneg) {
-      const __half2 z01 = __floats2half2_rn(fmaxf(fminf(t0, 0.f), -65504.f), fmaxf(fminf(t1, 0.f), -65504.f));
-      const __half2 z23 = __floats2half2_rn(fmaxf(fminf(t2, 0.f), -65504.f), fmaxf(fminf(t3, 0.f), -65504.f));
+      const __half2 z01 = __floats2half2_rn(zneg_value(t0), zneg_value(t1));
+      const __half2 z23 = __floats2half2_rn(zneg_value(t2), zneg_value(t3));
       zn[2 * q] = *reinterpret_cast<const uint32_t*>(&z01);
       zn[2 * q + 1] = *reinterpret_cast<const uint32_t*>(&z23);
     }

@@ -76,6 +76,7 @@ EXPORTED_SYMBOLS = [
     "dcscn_set_adam_step", "dcscn_last_grad_norm",
     "dcscn_patch_store_set", "dcscn_train_step_indexed", "dcscn_patch_gather", "dcscn_dropout_mask", "dcscn_grad_buffer", "dcscn_apply_gradients", "dcscn_apply_gradients_avg", "dcscn_reset_optimizer", "dcscn_graph_replays",
     "dcscn_tile_halo", "dcscn_optimizer_slot_count", "dcscn_get_optimizer_slot", "dcscn_set_optimizer_slot",
+    "dcscn_get_train_tensor",
 ]
 
 _lib = None
@@ -111,6 +112,7 @@ def load_library(path=None):
     lib.dcscn_forward_ensemble_host.argtypes = [vp, vp, vp, vp, ci, ci, ci]
     lib.dcscn_forward_ensemble_partial.argtypes = [vp, vp, vp, vp, ci, ci, ci, vp]
     lib.dcscn_get_activation.argtypes = [vp, ctypes.c_char_p, fp, c64]
+    lib.dcscn_get_train_tensor.argtypes = [vp, ctypes.c_char_p, fp, c64]
     lib.dcscn_set_option.argtypes = [vp, ctypes.c_char_p, c64]
     lib.dcscn_get_timings.argtypes = [vp, fp, ci, ctypes.POINTER(ci), ctypes.c_char_p, ci]
     u32, cf = ctypes.c_uint32, ctypes.c_float
@@ -491,6 +493,14 @@ class Engine:
         a = np.empty(shape, dtype=np.float32)
         self._check(self.lib.dcscn_get_activation(self.handle, tensor.encode(),
                                                   a.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), a.size))
+        return a
+
+    def get_train_tensor(self, name, shape):
+        """A tensor of the last train step (dcscn_get_train_tensor: "y_", "dY", "dZ:<layer>", "dH:<layer>",
+        "zneg:<layer>") as fp32 of `shape`; all but "zneg:" need set_option("grad_capture", 1) before the step."""
+        a = np.empty(shape, dtype=np.float32)
+        self._check(self.lib.dcscn_get_train_tensor(self.handle, name.encode(),
+                                                    a.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), a.size))
         return a
 
     def set_option(self, key, value):

@@ -214,6 +214,20 @@ int dcscn_dropout_mask(dcscn_handle* h, const char* tensor, uint32_t seed, int n
  * Fails after a forward that ran tiled (option "workspace_mb"): the buffers then hold its last batch of windows.
  */
 int dcscn_get_activation(dcscn_handle* h, const char* tensor, float* host_data, int64_t numel);
+/*
+ * Parity / debug: a tensor of the LAST train step of a tensor-core graph as fp32 NHWC (hi + lo of its fp16 planes),
+ * logical channels only.  After a train step dcscn_get_activation returns that step's forward, after dropout.  Needs
+ * option "grad_capture" = 1 during the step, except for the "zneg:" planes, which every prelu / leaky_relu step keeps:
+ *   "y_", "dY"        the prediction and d loss / d y_ * grad_scale, [n, s*H, s*W, 1] (fp32, exact)
+ *   "dZ:<layer>"      gradient at the layer's convolution output (before bias / activation), scaled by grad_scale:
+ *                     CNNi, A1, B1, B2 [n, H, W, cout]; Up-PS [n, H, W, r*r*C] (x2, x3) or [n, H, W, 4*C] (x4), and at x4
+ *                     Up-PS2 [n, 2H, 2W, 4*C], in the space_to_depth column order (i*r + j)*C + c
+ *   "dH:<layer>"      output of the layer's data-gradient twin = gradient at the layer's input: CNNi (i >= 2)
+ *                     [.., filters(i-1)], A1+B1 [.., concat channels], B2 [.., nin_filters2], Up-PS [.., nin_filters2 +
+ *                     nin_filters] (B2 then A1), Up-PS2 [n, 2H, 2W, C]
+ *   "zneg:<layer>"    the fp16 min(z, 0) plane the forward stored for CNNi, A1, B1, B2
+ */
+int dcscn_get_train_tensor(dcscn_handle* h, const char* name, float* host_data, int64_t numel);
 
 /* Options: "conv_impl" 0 = wgmma tensor cores (default), 1 = CUDA-core fp32 validation kernels;
  *          "seg_chunks" = pipeline stages per fp32-promotion segment (default 0 = automatic: 2, or 3 for thin layers);
@@ -225,6 +239,8 @@ int dcscn_get_activation(dcscn_handle* h, const char* tensor, float* host_data, 
  *          "l1_loss" 0 | 1 = image_loss of the train step is mean |y_ - y| instead of the MSE (--use_l1_loss,
  *          DCSCN.py:342-344; the returned mse stays the MSE);
  *          "wgrad_impl" 0 | 1 = filter gradients on wgmma tensor cores (default) or on CUDA cores (cross-check);
+ *          "grad_capture" 0 | 1 = the train step copies its activation-sized gradient tensors into buffers allocated on
+ *          first use, for dcscn_get_train_tensor (default 0: no copy, no allocation);
  *          "workspace_mb" = MiB an inference forward may allocate per batch (default 0 = no limit: the whole batch runs
  *          at once).  Covers dcscn_forward, dcscn_forward_host and the dcscn_forward_ensemble* calls.  The limit counts
  *          the activation workspace and the staging buffers of one batch of windows; an image whose workspace fits runs
