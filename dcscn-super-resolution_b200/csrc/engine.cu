@@ -14,6 +14,8 @@
 #include <map>
 #include <memory>
 #include <string>
+#include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "../../include/dcscn_b200.h"
@@ -47,6 +49,68 @@ static int fail(const char* fmt, ...) {
     if (_e != cudaSuccess)                                                                     \
       return fail("%s failed at %s:%d: %s", #expr, __FILE__, __LINE__, cudaGetErrorString(_e)); \
   } while (0)
+
+// ---------------------------------------------------------------------------------- device memory ----
+// The one owner of a cudaMalloc allocation of size() elements of T: the destructor frees it.  Pointers taken from get()
+// (kernel parameters, launch plans, tensor maps) do not own it.
+template <typename T>
+class DeviceArray {
+ public:
+  DeviceArray() = default;
+  DeviceArray(const DeviceArray&) = delete;
+  DeviceArray& operator=(const DeviceArray&) = delete;
+  DeviceArray(DeviceArray&& o) noexcept : p_(o.p_), n_(o.n_) { o.p_ = nullptr; o.n_ = 0; }
+  DeviceArray& operator=(DeviceArray&& o) noexcept {
+    if (this != &o) {
+      release();
+      std::swap(p_, o.p_);
+      std::swap(n_, o.n_);
+    }
+    return *this;
+  }
+  ~DeviceArray() { release(); }
+
+  T* get() const { return p_; }
+  size_t size() const { return n_; }
+
+  // Frees, then allocates n elements (n = 0 leaves the array empty), zero-filled when asked.
+  int alloc(size_t n, bool zero = false) {
+    release();
+    if (n == 0) return 0;
+    void* p = nullptr;
+    CUDA_TRY(cudaMalloc(&p, n * sizeof(T)));
+    p_ = static_cast<T*>(p);
+    n_ = n;
+    if (zero) CUDA_TRY(cudaMemset(p_, 0, n * sizeof(T)));
+    return 0;
+  }
+  // Grow-only staging: reallocates, without zero-filling, only when n exceeds the current size.
+  int grow(size_t n) { return n > n_ ? alloc(n) : 0; }
+  // Copies `host` in.  An allocation of the same size is reused, so the pointers cached launch plans embed stay valid
+  // across weight updates; otherwise it is replaced and *moved is set.
+  int upload(const std::vector<T>& host, bool* moved = nullptr) {
+    if (host.size() != n_) {
+      if (moved) *moved = true;
+      if (alloc(host.size())) return 1;
+    }
+    if (n_) CUDA_TRY(cudaMemcpy(p_, host.data(), n_ * sizeof(T), cudaMemcpyHostToDevice));
+    return 0;
+  }
+
+ private:
+  void release() {
+    if (p_) cudaFree(p_);
+    p_ = nullptr;
+    n_ = 0;
+  }
+  T* p_ = nullptr;
+  size_t n_ = 0;
+};
+
+struct StreamDeleter { void operator()(cudaStream_t s) const { cudaStreamDestroy(s); } };
+struct EventDeleter { void operator()(cudaEvent_t e) const { cudaEventDestroy(e); } };
+using Stream = std::unique_ptr<std::remove_pointer_t<cudaStream_t>, StreamDeleter>;
+using Event = std::unique_ptr<std::remove_pointer_t<cudaEvent_t>, EventDeleter>;
 
 static inline int pad16(int v) { return (v + 15) & ~15; }
 
@@ -82,14 +146,13 @@ struct TcLayer {
   std::vector<float> bias_host, alpha_host;  // [n_tiles*n_pad]
   int cin = 0, cout = 0;
   float wscale = 1.f;
-  __half* d_wpack = nullptr;
-  float* d_bias = nullptr;
-  float* d_alpha = nullptr;
-  float* d_wref = nullptr;      // fp32 HWIO for the validation kernel
-  int* d_in_map = nullptr;
+  DeviceArray<__half> d_wpack;
+  DeviceArray<float> d_bias;
+  DeviceArray<float> d_alpha;
+  DeviceArray<float> d_wref;    // fp32 HWIO for the validation kernel
+  DeviceArray<int> d_in_map;
   int packed_planes = 0;
-  int* d_img_map = nullptr;     // training: flat parameter index behind every hi-plane element of d_wpack (-1 = zero)
-  size_t img_map_n = 0;
+  DeviceArray<int> d_img_map;   // training: flat parameter index behind every hi-plane element of d_wpack (-1 = zero)
 };
 
 struct GatherJob {   // training: dst[i] = d_w[map[i]] where map[i] >= 0 (biases, PReLU slopes, CNN1 / R-CNN1 filters)
@@ -133,6 +196,8 @@ struct Plan {
   ~Plan() { if (gexec) cudaGraphExecDestroy(gexec); }
 };
 
+struct TrainState;                    // train_engine.inc
+
 struct dcscn_handle {
   dcscn_config cfg;
   int sm_count = 132;
@@ -153,62 +218,54 @@ struct dcscn_handle {
   std::vector<TcLayer> tcl;          // CNN2..CNNL, A1+B1, B2, Up-PS [, Up-PS2]
   std::vector<TcLayer> bwd;          // data-gradient twins (transposed, flipped filters), see build_bwd_layers
   bool train_enabled = false;
-  float *ens_x = nullptr, *ens_x2 = nullptr, *ens_y = nullptr;   // self-ensemble: transformed copies / per-flip outputs
-  size_t ens_cap = 0;
-  float *ensio_x = nullptr, *ensio_x2 = nullptr;                  // host-call staging of the ensemble entry point
-  double* ensio_y = nullptr;
-  size_t ensio_cap = 0;
+  DeviceArray<float> ens_x, ens_x2, ens_y;   // self-ensemble: transformed copies / per-flip outputs
+  DeviceArray<float> ensio_x, ensio_x2;      // host-call staging of the ensemble entry point
+  DeviceArray<double> ensio_y;
   int l1_loss = 0;                   // --use_l1_loss: image_loss = mean |y_ - y| (DCSCN.py:342-344)
   int wgrad_impl = 0;                // 0 = wgmma (wgrad_tc.cuh), 1 = CUDA cores (validation)
   bool shadow_mode = false;          // P() returns index-coded shadows (build_refresh_maps)
   bool refresh_ready = false;        // device-side weight refresh maps are valid for the current packing
   std::vector<struct GatherJob> gather_jobs;
-  struct TrainState* train = nullptr;
-  float* d_first_w = nullptr;        // CNN1 [taps][n_pad]
-  float* d_first_bias = nullptr;
-  float* d_first_alpha = nullptr;
-  float* d_last_w = nullptr;         // R-CNN1 [taps][C]
+  std::unique_ptr<TrainState> train;
+  DeviceArray<float> d_first_w;      // CNN1 [taps][n_pad]
+  DeviceArray<float> d_first_bias;
+  DeviceArray<float> d_first_alpha;
+  DeviceArray<float> d_last_w;       // R-CNN1 [taps][C]
 
   // workspace (grow-only)
   size_t cap_px = 0;                 // LR pixels the buffers can hold
-  __half *feat_hi = nullptr, *feat_lo = nullptr;
-  __half *b1_hi = nullptr, *b1_lo = nullptr;
-  __half *nin_hi = nullptr, *nin_lo = nullptr;
-  __half *mid_hi = nullptr, *mid_lo = nullptr;
-  float* hr = nullptr;
-  float* vbuf = nullptr;             // tap-planar partial products of the fused R-CNN1 [9][N][sH][sW]
-  float *io_x = nullptr, *io_x2 = nullptr, *io_y = nullptr;  // staging for forward_host
-  size_t io_cap = 0;
+  DeviceArray<__half> feat_hi, feat_lo;
+  DeviceArray<__half> b1_hi, b1_lo;
+  DeviceArray<__half> nin_hi, nin_lo;
+  DeviceArray<__half> mid_hi, mid_lo;
+  DeviceArray<float> hr;
+  DeviceArray<float> vbuf;           // tap-planar partial products of the fused R-CNN1 [9][N][sH][sW]
+  DeviceArray<float> io_x, io_x2, io_y;  // staging for forward_host
   // training patch store (dcscn_patch_store_set): uint8 patches resident in HBM + the mini-batch's index list
-  uint8_t *ps_lr = nullptr, *ps_bic = nullptr, *ps_true = nullptr;
+  DeviceArray<uint8_t> ps_lr, ps_bic, ps_true;
   int64_t ps_count = 0;
   int ps_h = 0, ps_w = 0;
-  int* ps_idx = nullptr;
-  int ps_idx_cap = 0;
+  DeviceArray<int> ps_idx;
   // Pillow-bicubic resampling tables per (input size, output size) and the float32 intermediate of the two passes
-  struct PilTable { int in = 0, out = 0, ksize = 0; double* k = nullptr; int* bounds = nullptr; };
+  struct PilTable { int in = 0, out = 0, ksize = 0; DeviceArray<double> k; DeviceArray<int> bounds; };
   std::vector<PilTable> pil_tables;
-  float* pil_tmp = nullptr;
-  size_t pil_tmp_cap = 0;
-  cudaStream_t copy_stream = nullptr;  // forward_host: x2 (only read by the last kernel) rides in beside the conv stack
-  cudaEvent_t x2_ready = nullptr;
+  DeviceArray<float> pil_tmp;
+  Stream copy_stream;                  // forward_host: x2 (only read by the last kernel) rides in beside the conv stack
+  Event x2_ready;
   bool wait_x2 = false;                // the next forward's last kernel waits for x2_ready
-  int64_t device_bytes = 0;
   // tiled inference (option "workspace_mb"): staging buffers of one batch of windows, grow-only
   int64_t workspace_mb = 0;          // 0 = whole-image forwards only
-  float *tile_x = nullptr, *tile_x2 = nullptr, *tile_y = nullptr;
-  size_t tile_cap = 0;               // LR window pixels the staging buffers hold
-  int64_t tile_bytes = 0;
+  DeviceArray<float> tile_x, tile_x2, tile_y;
   bool tiling = false;               // a tiled forward is issuing its batches (forward_impl keeps the timing events)
   bool tile_vec4 = false;            // while tiling: the four-pixel R-CNN1 kernel the whole-image forward would pick
   bool tiled_last = false;           // the last forward ran tiled: the activation buffers hold its last batch
   int tiled_batches = 0;             // batches of the last tiled forward (timing names)
 
   // depthwise-separable graphs: fp32 buffers + per-layer device filters
-  struct DsDev { float *dw = nullptr, *pw = nullptr, *bias = nullptr, *alpha = nullptr; };
+  struct DsDev { DeviceArray<float> dw, pw, bias, alpha; };
   std::vector<DsDev> ds;             // same order as `layers`
   DsDev ds_ab;                       // fused A1 | B1 1x1 layer of the tile kernels: [concat positions][A1 cols | B1 cols], scales folded
-  float *ds_feat = nullptr, *ds_b1 = nullptr, *ds_nin = nullptr, *ds_mid = nullptr, *ds_hr = nullptr;
+  DeviceArray<float> ds_feat, ds_b1, ds_nin, ds_mid, ds_hr;
   int ds_total = 0;                  // channels of the (unpadded) concat buffer
   int ds_n = 0, ds_h = 0, ds_w = 0;  // geometry of the last DS forward
   std::vector<int> ds_off;
@@ -217,7 +274,7 @@ struct dcscn_handle {
   Plan* last_plan = nullptr;
   int use_graph = 1;                 // option "graph": replay the per-(n,h,w) launch sequence of a forward as one CUDA graph
   uint64_t graph_epoch = 1;          // bumped by everything a captured launch bakes in (options, weight re-packs)
-  cudaStream_t cap_stream = nullptr; // capture happens on a private stream (the caller's may be the legacy default stream)
+  Stream cap_stream;                 // capture happens on a private stream (the caller's may be the legacy default stream)
   int64_t graph_replays = 0;
 
   int conv_impl = 0;
@@ -226,7 +283,7 @@ struct dcscn_handle {
   int grad_capture = 0;              // 1: the train step copies its gradient tensors out (dcscn_get_train_tensor)
   int timing = 0;
   int fuse_last = 1;                 // fold the per-pixel half of R-CNN1 into the last Up-PS epilogue
-  std::vector<cudaEvent_t> ev;       // timing events (launch boundaries of the last forward)
+  std::vector<Event> ev;             // timing events (launch boundaries of the last forward)
   int ev_used = 0;
   int64_t launches = 0;
   PFN_cuTensorMapEncodeTiled_v12000 encode = nullptr;
@@ -351,39 +408,6 @@ static const std::vector<float>& P(const dcscn_handle* h, const std::string& nam
 }
 
 // ------------------------------------------------------------------------------ weight packing ----
-// Device copies of host vectors.  Re-uploading the same number of bytes reuses the allocation, so cached launch
-// plans (which embed these pointers) stay valid across weight updates; `g_upload_realloc` records when that failed.
-static std::map<void*, size_t> g_upload_bytes;
-static bool g_upload_realloc = false;
-
-static void dev_free(void* p) {
-  if (!p) return;
-  g_upload_bytes.erase(p);
-  cudaFree(p);
-}
-
-template <typename T>
-static int upload(T** dptr, const std::vector<T>& host, dcscn_handle* h) {
-  (void)h;
-  const size_t bytes = host.size() * sizeof(T);
-  if (*dptr) {
-    auto it = g_upload_bytes.find((void*)*dptr);
-    if (it != g_upload_bytes.end() && it->second == bytes && bytes > 0) {
-      CUDA_TRY(cudaMemcpy(*dptr, host.data(), bytes, cudaMemcpyHostToDevice));
-      return 0;
-    }
-    dev_free(*dptr);
-    *dptr = nullptr;
-    g_upload_realloc = true;
-  }
-  if (host.empty()) return 0;
-  CUDA_TRY(cudaMalloc((void**)dptr, bytes));
-  g_upload_bytes[(void*)*dptr] = bytes;
-  g_upload_realloc = true;
-  CUDA_TRY(cudaMemcpy(*dptr, host.data(), bytes, cudaMemcpyHostToDevice));
-  return 0;
-}
-
 // Appends the TF layer `scope` as columns [col0, col0+cout) of a fused tensor-core layer.
 static void fuse_columns(const dcscn_handle* h, TcLayer& t, const std::string& scope, int col0, int n_total_pad) {
   const LayerDef* l = find_layer(h, scope);
@@ -437,7 +461,8 @@ static void tile_image(const TcLayer& t, std::vector<float>& img) {
       }
 }
 
-static int pack_tc_layer(dcscn_handle* h, TcLayer& t) {
+// Sets *moved when a device array of the layer was reallocated.
+static int pack_tc_layer(dcscn_handle* h, TcLayer& t, bool* moved) {
   const int NPL = planes(h);
   float maxw = 0.f;
   for (float v : t.w_host) maxw = std::max(maxw, std::fabs(v));
@@ -455,11 +480,9 @@ static int pack_tc_layer(dcscn_handle* h, TcLayer& t) {
     pack[blk * NPL * tile_elems + pos] = hi;
     if (NPL == 2) pack[blk * NPL * tile_elems + tile_elems + pos] = __float2half_rn(v - __half2float(hi));
   }
-  if (upload(&t.d_wpack, pack, h)) return 1;
-  if (upload(&t.d_bias, t.bias_host, h)) return 1;
-  if (upload(&t.d_alpha, t.alpha_host, h)) return 1;
-  if (upload(&t.d_wref, t.w_host, h)) return 1;
-  if (upload(&t.d_in_map, t.in_map, h)) return 1;
+  if (t.d_wpack.upload(pack, moved) || t.d_bias.upload(t.bias_host, moved) || t.d_alpha.upload(t.alpha_host, moved) ||
+      t.d_wref.upload(t.w_host, moved) || t.d_in_map.upload(t.in_map, moved))
+    return 1;
   t.packed_planes = NPL;
   return 0;
 }
@@ -500,32 +523,11 @@ static TcLayer make_tc(const std::string& name, int ksz, int cin, int cout_cols,
   return t;
 }
 
-static void free_tc(TcLayer& t) {
-  dev_free(t.d_wpack);
-  dev_free(t.d_bias);
-  dev_free(t.d_alpha);
-  dev_free(t.d_wref);
-  dev_free(t.d_in_map);
-  dev_free(t.d_img_map);
-  t.d_img_map = nullptr;
-  t.d_wpack = nullptr;
-  t.d_bias = t.d_alpha = t.d_wref = nullptr;
-  t.d_in_map = nullptr;
-}
-
-static void adopt_tc(TcLayer& t, const TcLayer& old) {  // keep the device allocations of the previous packing
-  t.d_wpack = old.d_wpack; t.d_bias = old.d_bias; t.d_alpha = old.d_alpha;
-  t.d_wref = old.d_wref; t.d_in_map = old.d_in_map; t.d_img_map = old.d_img_map;
-}
-
 // (Re)builds every device-side weight image from the host fp32 parameters.
 static int finalize_params_ds(dcscn_handle* h) {
-  for (auto& d : h->ds) {
-    cudaFree(d.dw); cudaFree(d.pw); cudaFree(d.bias); cudaFree(d.alpha);
-  }
-  cudaFree(h->ds_ab.pw); cudaFree(h->ds_ab.bias); cudaFree(h->ds_ab.alpha);
   h->ds_ab = dcscn_handle::DsDev();
-  h->ds.assign(h->layers.size(), dcscn_handle::DsDev());
+  h->ds.clear();
+  h->ds.resize(h->layers.size());
   // concat buffer: every CNNi slot starts on a multiple of 4 channels (16-byte loads / stores); the pad channels are never
   // written (the buffer is zero-filled once) and meet zero rows in the A1 / B1 filters
   h->ds_off.clear();
@@ -563,16 +565,16 @@ static int finalize_params_ds(dcscn_handle* h) {
       layer_slopes(h, l, ab_alpha.data() + col0);
       continue;
     }
-    if (upload(&h->ds[i].dw, dwv, h) || upload(&h->ds[i].pw, pwv, h)) return 1;
-    if (l.bias && upload(&h->ds[i].bias, P(h, l.scope + "/conv_B"), h)) return 1;
+    if (h->ds[i].dw.upload(dwv) || h->ds[i].pw.upload(pwv)) return 1;
+    if (l.bias && h->ds[i].bias.upload(P(h, l.scope + "/conv_B"))) return 1;
     if (l.act) {
       std::vector<float> a(l.cout);
       layer_slopes(h, l, a.data());
-      if (slopes && upload(&h->ds[i].alpha, a, h)) return 1;
+      if (slopes && h->ds[i].alpha.upload(a)) return 1;
     }
   }
-  if (upload(&h->ds_ab.pw, ab_pw, h) || upload(&h->ds_ab.bias, ab_bias, h)) return 1;
-  if (slopes && upload(&h->ds_ab.alpha, ab_alpha, h)) return 1;
+  if (h->ds_ab.pw.upload(ab_pw) || h->ds_ab.bias.upload(ab_bias)) return 1;
+  if (slopes && h->ds_ab.alpha.upload(ab_alpha)) return 1;
   h->params_dirty = false;
   return 0;
 }
@@ -658,32 +660,30 @@ static int finalize_params(dcscn_handle* h) {
   h->tcl.clear();
   h->bwd.clear();
   h->refresh_ready = false;
-  g_upload_realloc = false;
+  bool moved = false;
   {
     std::vector<float> w, b, a;
     first_layer_vectors(h, w, b, a);
-    if (upload(&h->d_first_w, w, h) || upload(&h->d_first_bias, b, h) || upload(&h->d_first_alpha, a, h)) return 1;
+    if (h->d_first_w.upload(w, &moved) || h->d_first_bias.upload(b, &moved) || h->d_first_alpha.upload(a, &moved)) return 1;
   }
   if (construct_tc_layers(h)) return 1;
-  for (size_t i = 0; i < h->tcl.size(); ++i) {
-    if (i < old_tcl.size()) adopt_tc(h->tcl[i], old_tcl[i]);
-    if (pack_tc_layer(h, h->tcl[i])) return 1;
-  }
-  for (size_t i = h->tcl.size(); i < old_tcl.size(); ++i) free_tc(old_tcl[i]);
-  for (size_t i = 0; i < h->bwd.size(); ++i) {
-    if (i < old_bwd.size()) adopt_tc(h->bwd[i], old_bwd[i]);
-    if (pack_tc_layer(h, h->bwd[i])) return 1;
-  }
-  for (size_t i = h->bwd.size(); i < old_bwd.size(); ++i) free_tc(old_bwd[i]);
+  // each layer keeps the device allocations of its previous packing; those of layers that no longer exist are freed with
+  // old_tcl / old_bwd
+  auto repack = [&](std::vector<TcLayer>& cur, std::vector<TcLayer>& old) {
+    for (size_t i = 0; i < cur.size(); ++i) {
+      TcLayer& t = cur[i];
+      if (i < old.size()) {
+        t.d_wpack = std::move(old[i].d_wpack); t.d_bias = std::move(old[i].d_bias); t.d_alpha = std::move(old[i].d_alpha);
+        t.d_wref = std::move(old[i].d_wref); t.d_in_map = std::move(old[i].d_in_map); t.d_img_map = std::move(old[i].d_img_map);
+      }
+      if (pack_tc_layer(h, t, &moved)) return 1;
+    }
+    return 0;
+  };
+  if (repack(h->tcl, old_tcl) || repack(h->bwd, old_bwd)) return 1;
   // R-CNN1 (CUDA cores): [taps][C]
-  {
-    const LayerDef* l = find_layer(h, "R-CNN1");
-    const auto& W = P(h, "R-CNN1/conv_W");  // [k,k,C,1]
-    std::vector<float> w(W.begin(), W.end());
-    (void)l;
-    if (upload(&h->d_last_w, w, h)) return 1;
-  }
-  if (g_upload_realloc) {  // some device pointer moved: cached plans embed stale pointers
+  if (h->d_last_w.upload(P(h, "R-CNN1/conv_W"), &moved)) return 1;
+  if (moved) {  // some device pointer moved: cached plans embed stale pointers
     h->plans.clear();
     h->last_plan = nullptr;
   }
@@ -701,19 +701,6 @@ static int rdot_parts(int n_pad, int cout) {
 }
 
 // ----------------------------------------------------------------------------------- workspace ----
-template <typename T>
-static int dev_alloc(dcscn_handle* h, T** p, size_t count, bool zero) {
-  if (*p) {
-    cudaFree(*p);
-    *p = nullptr;
-  }
-  if (count == 0) return 0;
-  CUDA_TRY(cudaMalloc((void**)p, count * sizeof(T)));
-  if (zero) CUDA_TRY(cudaMemset(*p, 0, count * sizeof(T)));
-  h->device_bytes += (int64_t)(count * sizeof(T));
-  return 0;
-}
-
 // Elements per LR pixel of every buffer ensure_workspace allocates: the one statement of their sizes, shared by the
 // allocation and by the tile planner's workspace budget (valid once the parameters are finalised).
 struct WorkspaceShape {
@@ -755,33 +742,32 @@ static int ensure_workspace(dcscn_handle* h, size_t lr_px) {
   const dcscn_config& c = h->cfg;
   const WorkspaceShape ws = workspace_shape(h);
   if (c.depthwise_separable) {
-    h->device_bytes = 0;
-    if (dev_alloc(h, &h->ds_feat, lr_px * ws.feat, true)) return 1;   // pad channels must stay zero
-    if (dev_alloc(h, &h->ds_b1, lr_px * ws.b1, false)) return 1;
-    if (dev_alloc(h, &h->ds_nin, lr_px * ws.nin, false)) return 1;
-    if (c.scale == 4 && dev_alloc(h, &h->ds_mid, lr_px * ws.mid, false)) return 1;
-    if (dev_alloc(h, &h->ds_hr, lr_px * ws.hr, false)) return 1;
+    if (h->ds_feat.alloc(lr_px * ws.feat, true)) return 1;   // pad channels must stay zero
+    if (h->ds_b1.alloc(lr_px * ws.b1) || h->ds_nin.alloc(lr_px * ws.nin)) return 1;
+    if (c.scale == 4 && h->ds_mid.alloc(lr_px * ws.mid)) return 1;
+    if (h->ds_hr.alloc(lr_px * ws.hr)) return 1;
     h->cap_px = lr_px;
     return 0;
   }
   h->plans.clear();
   h->last_plan = nullptr;
-  h->device_bytes = 0;
   const bool two = ws.planes == 2;
-  if (dev_alloc(h, &h->feat_hi, lr_px * ws.feat, true)) return 1;
-  if (dev_alloc(h, &h->feat_lo, two ? lr_px * ws.feat : 0, true)) return 1;
-  if (dev_alloc(h, &h->b1_hi, lr_px * ws.b1, true)) return 1;
-  if (dev_alloc(h, &h->b1_lo, two ? lr_px * ws.b1 : 0, true)) return 1;
-  if (dev_alloc(h, &h->nin_hi, lr_px * ws.nin, true)) return 1;
-  if (dev_alloc(h, &h->nin_lo, two ? lr_px * ws.nin : 0, true)) return 1;
+  if (h->feat_hi.alloc(lr_px * ws.feat, true) || h->feat_lo.alloc(two ? lr_px * ws.feat : 0, true)) return 1;
+  if (h->b1_hi.alloc(lr_px * ws.b1, true) || h->b1_lo.alloc(two ? lr_px * ws.b1 : 0, true)) return 1;
+  if (h->nin_hi.alloc(lr_px * ws.nin, true) || h->nin_lo.alloc(two ? lr_px * ws.nin : 0, true)) return 1;
   if (c.scale == 4) {
-    if (dev_alloc(h, &h->mid_hi, lr_px * ws.mid, true)) return 1;
-    if (dev_alloc(h, &h->mid_lo, two ? lr_px * ws.mid : 0, true)) return 1;
+    if (h->mid_hi.alloc(lr_px * ws.mid, true) || h->mid_lo.alloc(two ? lr_px * ws.mid : 0, true)) return 1;
   }
-  if (dev_alloc(h, &h->hr, lr_px * ws.hr, true)) return 1;
-  if (dev_alloc(h, &h->vbuf, lr_px * ws.vbuf, true)) return 1;
+  if (h->hr.alloc(lr_px * ws.hr, true) || h->vbuf.alloc(lr_px * ws.vbuf, true)) return 1;
   h->cap_px = lr_px;
   return 0;
+}
+
+// Device bytes of the activation workspace and the tiled-inference staging buffers (dcscn_device_bytes).
+static int64_t workspace_bytes(const dcscn_handle* h) {
+  auto bytes = [](const auto&... a) { return (int64_t)(0 + ... + (a.size() * sizeof(*a.get()))); };
+  return bytes(h->feat_hi, h->feat_lo, h->b1_hi, h->b1_lo, h->nin_hi, h->nin_lo, h->mid_hi, h->mid_lo, h->hr, h->vbuf,
+               h->ds_feat, h->ds_b1, h->ds_nin, h->ds_mid, h->ds_hr, h->tile_x, h->tile_x2, h->tile_y);
 }
 
 // --------------------------------------------------------------------------------------- plans ----
@@ -860,10 +846,10 @@ static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, const __ha
   // weight tiles per promotion segment; 1 = promote every 16-channel K slice.  The automatic lengths keep the dominant
   // chain as short as the earlier two-pass scheme had it (2 tiles for wide layers, 3 for thin ones).
   L.p.seg_chunks = h->seg_chunks > 0 ? h->seg_chunks : (t.n_pad > 64 ? 2 : 3);
-  L.p.wpack = t.d_wpack;
+  L.p.wpack = t.d_wpack.get();
   L.p.epi = epi;
-  L.p.epi.bias = t.d_bias;
-  L.p.epi.alpha = t.d_alpha;
+  L.p.epi.bias = t.d_bias.get();
+  L.p.epi.alpha = t.d_alpha.get();
   L.p.epi.out_scale = 1.0f / t.wscale;   // refreshed at every launch (launch_tc): a re-pack may pick another scale
   if (!h->tcl.empty() && &t >= h->tcl.data() && &t < h->tcl.data() + h->tcl.size()) {
     L.layer_index = (int)(&t - h->tcl.data());
@@ -907,8 +893,8 @@ static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, const __ha
   L.ref.src_hi = src_hi;
   L.ref.src_lo = planes(h) == 2 ? src_lo : nullptr;
   L.ref.src_pitch = src_pitch;
-  L.ref.in_map = t.d_in_map;
-  L.ref.w = t.d_wref;
+  L.ref.in_map = t.d_in_map.get();
+  L.ref.w = t.d_wref.get();
   L.ref.n_total_pad = t.n_tiles * t.n_pad;
   L.ref.epi = L.p.epi;
   L.ref.epi.out_scale = 1.0f;
@@ -943,32 +929,32 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
   pl->first.g = ConvGeom{n, H, W, 1, 1, 1, 1};
   pl->first.ksz = find_layer(h, "CNN1")->k;
   pl->first.n_pad = h->feat_w[0];
-  pl->first.w = h->d_first_w;
-  pl->first.epi = epi_planes(h->feat_hi, lo(h->feat_lo, 0), h->feat_pitch, 0, h->feat_w[0]);
-  pl->first.epi.bias = h->d_first_bias;
-  pl->first.epi.alpha = h->d_first_alpha;
+  pl->first.w = h->d_first_w.get();
+  pl->first.epi = epi_planes(h->feat_hi.get(), lo(h->feat_lo.get(), 0), h->feat_pitch, 0, h->feat_w[0]);
+  pl->first.epi.bias = h->d_first_bias.get();
+  pl->first.epi.alpha = h->d_first_alpha.get();
   pl->first.epi.act = c.activator;
   pl->first.epi.n_valid = h->filters[0];
 
   size_t ti = 0;
   for (int i = 1; i < c.layers; ++i, ++ti) {
-    EpiParams e = epi_planes(h->feat_hi + h->feat_off[i], lo(h->feat_lo, h->feat_off[i]), h->feat_pitch, 0, h->feat_w[i]);
+    EpiParams e = epi_planes(h->feat_hi.get() + h->feat_off[i], lo(h->feat_lo.get(), h->feat_off[i]), h->feat_pitch, 0, h->feat_w[i]);
     e.act = c.activator;
-    if (add_tc_launch(h, pl.get(), h->tcl[ti], h->feat_hi + h->feat_off[i - 1], lo(h->feat_lo, h->feat_off[i - 1]),
+    if (add_tc_launch(h, pl.get(), h->tcl[ti], h->feat_hi.get() + h->feat_off[i - 1], lo(h->feat_lo.get(), h->feat_off[i - 1]),
                       h->feat_pitch, n, H, W, e))
       return nullptr;
   }
   {  // A1+B1: columns [0,a1_w) -> nin[:, b1_w:], columns [a1_w, a1_w+b1_w) -> b1
-    EpiParams e = epi_planes(h->nin_hi + h->b1_w, lo(h->nin_lo, h->b1_w), h->nin_pitch, 0, h->a1_w);
+    EpiParams e = epi_planes(h->nin_hi.get() + h->b1_w, lo(h->nin_lo.get(), h->b1_w), h->nin_pitch, 0, h->a1_w);
     e.num_seg = 2;
-    e.seg[1] = {h->a1_w, h->a1_w + h->b1_w, h->b1_hi, two ? h->b1_lo : nullptr, h->b1_w};
+    e.seg[1] = {h->a1_w, h->a1_w + h->b1_w, h->b1_hi.get(), two ? h->b1_lo.get() : nullptr, h->b1_w};
     e.act = c.activator;
-    if (add_tc_launch(h, pl.get(), h->tcl[ti++], h->feat_hi, lo(h->feat_lo, 0), h->feat_pitch, n, H, W, e)) return nullptr;
+    if (add_tc_launch(h, pl.get(), h->tcl[ti++], h->feat_hi.get(), lo(h->feat_lo.get(), 0), h->feat_pitch, n, H, W, e)) return nullptr;
   }
   {  // B2 -> nin[:, 0:b1_w]
-    EpiParams e = epi_planes(h->nin_hi, lo(h->nin_lo, 0), h->nin_pitch, 0, h->b1_w);
+    EpiParams e = epi_planes(h->nin_hi.get(), lo(h->nin_lo.get(), 0), h->nin_pitch, 0, h->b1_w);
     e.act = c.activator;
-    if (add_tc_launch(h, pl.get(), h->tcl[ti++], h->b1_hi, two ? h->b1_lo : nullptr, h->b1_w, n, H, W, e)) return nullptr;
+    if (add_tc_launch(h, pl.get(), h->tcl[ti++], h->b1_hi.get(), two ? h->b1_lo.get() : nullptr, h->b1_w, n, H, W, e)) return nullptr;
   }
   int HR_H = H, HR_W = W;
   {  // Up-PS
@@ -980,15 +966,15 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
       e.d2s_r = 2;
       e.d2s_cout = c.nin_filters + c.nin_filters2;
       e.num_seg = 1;
-      e.seg[0] = {0, 0, h->mid_hi, two ? h->mid_lo : nullptr, h->mid_pitch};
+      e.seg[0] = {0, 0, h->mid_hi.get(), two ? h->mid_lo.get() : nullptr, h->mid_pitch};
     } else {
       e.mode = EPI_D2S_F32;
       e.d2s_r = c.scale;
       e.d2s_cout = h->ps_out;
-      e.dst_f32 = h->hr;
+      e.dst_f32 = h->hr.get();
       e.d2s_pitch = h->ps_out;
     }
-    if (add_tc_launch(h, pl.get(), h->tcl[ti++], h->nin_hi, two ? h->nin_lo : nullptr, h->nin_pitch, n, H, W, e)) return nullptr;
+    if (add_tc_launch(h, pl.get(), h->tcl[ti++], h->nin_hi.get(), two ? h->nin_lo.get() : nullptr, h->nin_pitch, n, H, W, e)) return nullptr;
     HR_H = H * (c.scale == 4 ? 2 : c.scale);
     HR_W = W * (c.scale == 4 ? 2 : c.scale);
   }
@@ -999,9 +985,9 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
     e.mode = EPI_D2S_F32;
     e.d2s_r = 2;
     e.d2s_cout = h->ps_out;
-    e.dst_f32 = h->hr;
+    e.dst_f32 = h->hr.get();
     e.d2s_pitch = h->ps_out;
-    if (add_tc_launch(h, pl.get(), h->tcl[ti++], h->mid_hi, two ? h->mid_lo : nullptr, h->mid_pitch, n, HR_H, HR_W, e))
+    if (add_tc_launch(h, pl.get(), h->tcl[ti++], h->mid_hi.get(), two ? h->mid_lo.get() : nullptr, h->mid_pitch, n, HR_H, HR_W, e))
       return nullptr;
     HR_H *= 2;
     HR_W *= 2;
@@ -1018,8 +1004,8 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
     if (pl->fused_last) {
       L.p.epi.rdot_parts = ((per * 16) % cout == 0) ? 1 : parts;
       L.p.epi.mode = EPI_D2S_RDOT;
-      L.p.epi.rdot_w = h->d_last_w;
-      L.p.epi.rdot_out = h->vbuf;
+      L.p.epi.rdot_w = h->d_last_w.get();
+      L.p.epi.rdot_out = h->vbuf.get();
       L.p.epi.rdot_taps = klast * klast;
     }
     const int gparts = pl->fused_last ? L.p.epi.rdot_parts : 1;
@@ -1029,7 +1015,7 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
     pl->gather.H = HR_H;
     pl->gather.W = HR_W;
     pl->gather.ksz = klast;
-    pl->gather.v = h->vbuf;
+    pl->gather.v = h->vbuf.get();
   }
   memset(&pl->last, 0, sizeof(pl->last));
   pl->last.n_img = n;
@@ -1038,8 +1024,8 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
   pl->last.ksz = find_layer(h, "R-CNN1")->k;
   pl->last.C = h->ps_out;
   pl->last.pitch = h->ps_out;
-  pl->last.src = h->hr;
-  pl->last.w = h->d_last_w;
+  pl->last.src = h->hr.get();
+  pl->last.w = h->d_last_w.get();
   pl->last.bias = 0.f;
   if (h->plans.size() >= 64) h->plans.erase(h->plans.begin());
   h->plans.push_back(std::move(pl));
@@ -1101,9 +1087,9 @@ static int mark(dcscn_handle* h, cudaStream_t st) {
   if (h->ev_used >= (int)h->ev.size()) {
     cudaEvent_t e;
     CUDA_TRY(cudaEventCreate(&e));
-    h->ev.push_back(e);
+    h->ev.emplace_back(e);
   }
-  CUDA_TRY(cudaEventRecord(h->ev[h->ev_used++], st));
+  CUDA_TRY(cudaEventRecord(h->ev[h->ev_used++].get(), st));
   return 0;
 }
 
@@ -1161,7 +1147,7 @@ static DsTileParams ds_tile_params(const LayerDef& l, const dcscn_handle::DsDev&
   DsTileParams p;
   memset(&p, 0, sizeof(p));
   p.n_img = n; p.H = H; p.W = W; p.cin = l.cin; p.cout = l.cout;
-  p.src = src; p.src_pitch = src_pitch; p.dw = d.dw; p.pw = d.pw; p.bias = d.bias; p.alpha = d.alpha;
+  p.src = src; p.src_pitch = src_pitch; p.dw = d.dw.get(); p.pw = d.pw.get(); p.bias = d.bias.get(); p.alpha = d.alpha.get();
   p.dst = dst; p.dst_pitch = dst_pitch; p.dst_off = dst_off;
   return p;
 }
@@ -1187,53 +1173,53 @@ static int forward_ds_tile(dcscn_handle* h, const float* x, const float* x2, flo
   }
   size_t li = 0;
   for (int i = 0; i < L; ++i, ++li) {
-    const float* src = i == 0 ? x : h->ds_feat + h->ds_off[i - 1];
-    DsTileParams p = ds_tile_params(h->layers[li], h->ds[li], src, i == 0 ? c.channels : T, h->ds_feat, T, h->ds_off[i], n, H, W);
+    const float* src = i == 0 ? x : h->ds_feat.get() + h->ds_off[i - 1];
+    DsTileParams p = ds_tile_params(h->layers[li], h->ds[li], src, i == 0 ? c.channels : T, h->ds_feat.get(), T, h->ds_off[i], n, H, W);
     if (launch_ds_tile(h, p, h->layers[li].k, st)) return 1;
-    if (ds_activate(h, h->ds_feat, (long long)n * H * W, T, h->ds_off[i], h->filters[i], st)) return 1;
+    if (ds_activate(h, h->ds_feat.get(), (long long)n * H * W, T, h->ds_off[i], h->filters[i], st)) return 1;
   }
   {  // A1 | B1: both are 1x1 over the whole concat buffer -> ONE pass; the per-channel depthwise scales are folded into the
      // pointwise rows.  Columns [0, na) = A1 -> [B2 | A1] buffer at channel nb; columns [na, na+nb) = B1 -> B1 buffer.
     if (h->layers[li].k != 1 || h->layers[li + 1].k != 1) return fail("depthwise-separable A1 / B1 must be 1x1");
     LayerDef ab = h->layers[li];
     ab.k = 1; ab.cin = T; ab.cout = cps;
-    DsTileParams p = ds_tile_params(ab, h->ds_ab, h->ds_feat, T, h->ds_nin, cps, nb, n, H, W);
+    DsTileParams p = ds_tile_params(ab, h->ds_ab, h->ds_feat.get(), T, h->ds_nin.get(), cps, nb, n, H, W);
     p.dw = nullptr;
     p.split = na;
-    p.dst2 = h->ds_b1; p.dst2_pitch = nb; p.dst2_off = 0;
+    p.dst2 = h->ds_b1.get(); p.dst2_pitch = nb; p.dst2_off = 0;
     if (cps > 32) return fail("depthwise-separable graph: nin_filters + nin_filters2 = %d > 32 is not supported by the fused A1|B1 kernel", cps);
     if (launch_ds_tile(h, p, 1, st)) return 1;
-    if (ds_activate(h, h->ds_nin, (long long)n * H * W, cps, nb, na, st) || ds_activate(h, h->ds_b1, (long long)n * H * W, nb, 0, nb, st))
+    if (ds_activate(h, h->ds_nin.get(), (long long)n * H * W, cps, nb, na, st) || ds_activate(h, h->ds_b1.get(), (long long)n * H * W, nb, 0, nb, st))
       return 1;
     li += 2;
   }
   {  // B2
-    DsTileParams p = ds_tile_params(h->layers[li], h->ds[li], h->ds_b1, nb, h->ds_nin, cps, 0, n, H, W);
+    DsTileParams p = ds_tile_params(h->layers[li], h->ds[li], h->ds_b1.get(), nb, h->ds_nin.get(), cps, 0, n, H, W);
     if (launch_ds_tile(h, p, h->layers[li].k, st)) return 1;
-    if (ds_activate(h, h->ds_nin, (long long)n * H * W, cps, 0, nb, st)) return 1;
+    if (ds_activate(h, h->ds_nin.get(), (long long)n * H * W, cps, 0, nb, st)) return 1;
     ++li;
   }
   int HH = H, WW = W;
   if (c.scale == 4) {
-    DsTileParams p = ds_tile_params(h->layers[li], h->ds[li], h->ds_nin, cps, h->ds_mid, cps, 0, n, H, W);
+    DsTileParams p = ds_tile_params(h->layers[li], h->ds[li], h->ds_nin.get(), cps, h->ds_mid.get(), cps, 0, n, H, W);
     p.d2s_r = 2; p.d2s_cout = cps;
     if (launch_ds_tile(h, p, h->layers[li].k, st)) return 1;
     ++li;
     HH = 2 * H; WW = 2 * W;
-    DsTileParams q = ds_tile_params(h->layers[li], h->ds[li], h->ds_mid, cps, h->ds_hr, h->ps_out, 0, n, HH, WW);
+    DsTileParams q = ds_tile_params(h->layers[li], h->ds[li], h->ds_mid.get(), cps, h->ds_hr.get(), h->ps_out, 0, n, HH, WW);
     q.d2s_r = 2; q.d2s_cout = h->ps_out;
     if (launch_ds_tile(h, q, h->layers[li].k, st)) return 1;
     ++li;
     HH *= 2; WW *= 2;
   } else {
-    DsTileParams p = ds_tile_params(h->layers[li], h->ds[li], h->ds_nin, cps, h->ds_hr, h->ps_out, 0, n, H, W);
+    DsTileParams p = ds_tile_params(h->layers[li], h->ds[li], h->ds_nin.get(), cps, h->ds_hr.get(), h->ps_out, 0, n, H, W);
     p.d2s_r = c.scale; p.d2s_cout = h->ps_out;
     if (launch_ds_tile(h, p, h->layers[li].k, st)) return 1;
     ++li;
     HH = c.scale * H; WW = c.scale * W;
   }
   if (h->wait_x2) {
-    CUDA_TRY(cudaStreamWaitEvent(st, h->x2_ready, 0));
+    CUDA_TRY(cudaStreamWaitEvent(st, h->x2_ready.get(), 0));
     h->wait_x2 = false;
   }
   // R-CNN1 (no bias / activation) + x2
@@ -1248,14 +1234,14 @@ static int forward_ds_tile(dcscn_handle* h, const float* x, const float* x2, flo
                       ((reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(x2)) & 15) == 0 &&
                       (!h->tiling || h->tile_vec4);
     const int grid = (int)std::min<long long>(((vec4 ? total / 4 : total) + 255) / 256, (long long)h->sm_count * 16);
-    if (vec4) ds_single4_kernel<<<grid, 256, 0, st>>>(h->ds_hr, x2, y, n, HH, WW, d.dw, d.pw, d.bias, d.alpha);
-    else if (lr.k == 3) ds_single_kernel<3><<<grid, 256, 0, st>>>(h->ds_hr, x2, y, n, HH, WW, d.dw, d.pw, d.bias, d.alpha);
-    else ds_single_kernel<1><<<grid, 256, 0, st>>>(h->ds_hr, x2, y, n, HH, WW, d.dw, d.pw, d.bias, d.alpha);
+    if (vec4) ds_single4_kernel<<<grid, 256, 0, st>>>(h->ds_hr.get(), x2, y, n, HH, WW, d.dw.get(), d.pw.get(), d.bias.get(), d.alpha.get());
+    else if (lr.k == 3) ds_single_kernel<3><<<grid, 256, 0, st>>>(h->ds_hr.get(), x2, y, n, HH, WW, d.dw.get(), d.pw.get(), d.bias.get(), d.alpha.get());
+    else ds_single_kernel<1><<<grid, 256, 0, st>>>(h->ds_hr.get(), x2, y, n, HH, WW, d.dw.get(), d.pw.get(), d.bias.get(), d.alpha.get());
     CUDA_TRY(cudaGetLastError());
     h->launches++;
     return mark(h, st);
   }
-  DsTileParams p = ds_tile_params(lr, d, h->ds_hr, h->ps_out, y, 1, 0, n, HH, WW);
+  DsTileParams p = ds_tile_params(lr, d, h->ds_hr.get(), h->ps_out, y, 1, 0, n, HH, WW);
   p.add = x2;
   return launch_ds_tile(h, p, lr.k, st);
 }
@@ -1316,13 +1302,17 @@ static int forward_impl(dcscn_handle* h, const float* x, const float* x2, float*
     h->launches += pl->g_launches;
     h->graph_replays++;
   } else if (graphable && pl->eager_runs >= 1 && pl->last_x == x) {
-    if (!h->cap_stream) CUDA_TRY(cudaStreamCreateWithFlags(&h->cap_stream, cudaStreamNonBlocking));
+    if (!h->cap_stream) {
+      cudaStream_t s;
+      CUDA_TRY(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+      h->cap_stream.reset(s);
+    }
     if (pl->gexec) { cudaGraphExecDestroy(pl->gexec); pl->gexec = nullptr; }
     const int64_t before = h->launches;
-    CUDA_TRY(cudaStreamBeginCapture(h->cap_stream, cudaStreamCaptureModeThreadLocal));
-    const int rc = issue_front(h, pl, x, n, H, W, fused, h->cap_stream);
+    CUDA_TRY(cudaStreamBeginCapture(h->cap_stream.get(), cudaStreamCaptureModeThreadLocal));
+    const int rc = issue_front(h, pl, x, n, H, W, fused, h->cap_stream.get());
     cudaGraph_t g = nullptr;
-    const cudaError_t ce = cudaStreamEndCapture(h->cap_stream, &g);
+    const cudaError_t ce = cudaStreamEndCapture(h->cap_stream.get(), &g);
     h->launches = before;
     if (rc) { if (g) cudaGraphDestroy(g); return 1; }
     if (ce != cudaSuccess || g == nullptr) return fail("forward: stream capture failed: %s", cudaGetErrorString(ce));
@@ -1341,7 +1331,7 @@ static int forward_impl(dcscn_handle* h, const float* x, const float* x2, float*
   pl->last_x = x;
   pl->ran_fused = fused;
   if (h->wait_x2) {  // forward_host: x2 was copied on the side stream
-    CUDA_TRY(cudaStreamWaitEvent(st, h->x2_ready, 0));
+    CUDA_TRY(cudaStreamWaitEvent(st, h->x2_ready.get(), 0));
     h->wait_x2 = false;
   }
   if (fused) {  // R-CNN1 second half: 9-tap gather of the tap-planar partial products + x2
@@ -1443,17 +1433,7 @@ static int forward_tiled(dcscn_handle* h, const float* x, const float* x2, float
                          const TilePlan& tp, cudaStream_t st) {
   const int s = h->cfg.scale;
   const size_t lr_px = (size_t)tp.batch * tp.th * tp.tw, hr_px = lr_px * s * s;
-  if (lr_px > h->tile_cap) {
-    cudaFree(h->tile_x); cudaFree(h->tile_x2); cudaFree(h->tile_y);
-    h->tile_x = h->tile_x2 = h->tile_y = nullptr;
-    h->tile_cap = 0;
-    h->tile_bytes = 0;
-    CUDA_TRY(cudaMalloc((void**)&h->tile_x, lr_px * sizeof(float)));
-    CUDA_TRY(cudaMalloc((void**)&h->tile_x2, hr_px * sizeof(float)));
-    CUDA_TRY(cudaMalloc((void**)&h->tile_y, hr_px * sizeof(float)));
-    h->tile_cap = lr_px;
-    h->tile_bytes = (int64_t)((lr_px + 2 * hr_px) * sizeof(float));
-  }
+  if (h->tile_x.grow(lr_px) || h->tile_x2.grow(hr_px) || h->tile_y.grow(hr_px)) return 1;
   struct Scope {
     dcscn_handle* h;
     ~Scope() { h->tiling = false; }
@@ -1462,7 +1442,7 @@ static int forward_tiled(dcscn_handle* h, const float* x, const float* x2, float
   h->ev_used = 0;
   if (mark(h, st)) return 1;
   if (h->wait_x2) {  // forward_host: x2 was copied on the side stream, and the first gather reads it
-    CUDA_TRY(cudaStreamWaitEvent(st, h->x2_ready, 0));
+    CUDA_TRY(cudaStreamWaitEvent(st, h->x2_ready.get(), 0));
     h->wait_x2 = false;
   }
   const long long windows = (long long)n * tp.my * tp.mx;
@@ -1472,14 +1452,14 @@ static int forward_tiled(dcscn_handle* h, const float* x, const float* x2, float
     const TileGeom g{n, H, W, s, tp.th, tp.tw, tile_halo(h), tp.my, tp.mx, first, count};
     const long long elems = (long long)count * tp.th * tp.tw * (1 + s * s);
     tile_gather_kernel<<<(int)std::min<long long>((elems + 255) / 256, (long long)h->sm_count * 8), 256, 0, st>>>(
-        g, x, x2, h->tile_x, h->tile_x2);
+        g, x, x2, h->tile_x.get(), h->tile_x2.get());
     CUDA_TRY(cudaGetLastError());
     h->launches++;
     if (mark(h, st)) return 1;
-    if (forward_impl(h, h->tile_x, h->tile_x2, h->tile_y, count, tp.th, tp.tw, st)) return 1;
+    if (forward_impl(h, h->tile_x.get(), h->tile_x2.get(), h->tile_y.get(), count, tp.th, tp.tw, st)) return 1;
     const long long hr_elems = (long long)count * tp.th * tp.tw * s * s;
     tile_stitch_kernel<<<(int)std::min<long long>((hr_elems + 255) / 256, (long long)h->sm_count * 8), 256, 0, st>>>(
-        g, h->tile_y, y);
+        g, h->tile_y.get(), y);
     CUDA_TRY(cudaGetLastError());
     h->launches++;
     if (mark(h, st)) return 1;
@@ -1523,7 +1503,7 @@ static double pil_bicubic_filter(double x) {   // Pillow Resample.c bicubic_filt
 static int pil_axis(dcscn_handle* h, int in_size, int out_size, PilAxis* ax) {
   for (const auto& t : h->pil_tables)
     if (t.in == in_size && t.out == out_size) {
-      *ax = PilAxis{t.k, t.bounds, t.ksize};
+      *ax = PilAxis{t.k.get(), t.bounds.get(), t.ksize};
       return 0;
     }
   double scale = (double)in_size / (double)out_size, filterscale = scale;
@@ -1554,17 +1534,10 @@ static int pil_axis(dcscn_handle* h, int in_size, int out_size, PilAxis* ax) {
   }
   dcscn_handle::PilTable t;
   t.in = in_size; t.out = out_size; t.ksize = ksize;
-  CUDA_TRY(cudaMalloc((void**)&t.k, kk.size() * sizeof(double)));
-  CUDA_TRY(cudaMalloc((void**)&t.bounds, bounds.size() * sizeof(int)));
-  CUDA_TRY(cudaMemcpy(t.k, kk.data(), kk.size() * sizeof(double), cudaMemcpyHostToDevice));
-  CUDA_TRY(cudaMemcpy(t.bounds, bounds.data(), bounds.size() * sizeof(int), cudaMemcpyHostToDevice));
-  if (h->pil_tables.size() >= 64) {
-    cudaFree(h->pil_tables.front().k);
-    cudaFree(h->pil_tables.front().bounds);
-    h->pil_tables.erase(h->pil_tables.begin());
-  }
-  h->pil_tables.push_back(t);
-  *ax = PilAxis{t.k, t.bounds, t.ksize};
+  if (t.k.upload(kk) || t.bounds.upload(bounds)) return 1;
+  *ax = PilAxis{t.k.get(), t.bounds.get(), t.ksize};
+  if (h->pil_tables.size() >= 64) h->pil_tables.erase(h->pil_tables.begin());
+  h->pil_tables.push_back(std::move(t));
   return 0;
 }
 
@@ -1574,18 +1547,12 @@ static int pil_resize_impl(dcscn_handle* h, const float* src, float* dst, int n,
   PilAxis ax, ay;
   if (pil_axis(h, W, OW, &ax) || pil_axis(h, H, OH, &ay)) return 1;
   const size_t need = (size_t)n * H * OW;
-  if (need > h->pil_tmp_cap) {
-    cudaFree(h->pil_tmp);
-    h->pil_tmp = nullptr;
-    h->pil_tmp_cap = 0;
-    CUDA_TRY(cudaMalloc((void**)&h->pil_tmp, need * sizeof(float)));
-    h->pil_tmp_cap = need;
-  }
+  if (h->pil_tmp.grow(need)) return 1;
   const long long t1 = (long long)need, t2 = (long long)n * OH * OW;
   pil_resample_h_kernel<<<(int)std::min<long long>((t1 + 255) / 256, (long long)h->sm_count * 16), 256, 0, st>>>(
-      src, h->pil_tmp, (long long)n * H, W, OW, ax);
+      src, h->pil_tmp.get(), (long long)n * H, W, OW, ax);
   pil_resample_v_kernel<<<(int)std::min<long long>((t2 + 255) / 256, (long long)h->sm_count * 16), 256, 0, st>>>(
-      h->pil_tmp, dst, n, H, OH, OW, ay);
+      h->pil_tmp.get(), dst, n, H, OH, OW, ay);
   CUDA_TRY(cudaGetLastError());
   h->launches += 2;
   return 0;
@@ -1631,38 +1598,6 @@ int dcscn_destroy(dcscn_handle* h) {
   if (!h) return 0;
   cudaSetDevice(h->cfg.device_id);
   cudaDeviceSynchronize();
-  for (TcLayer& t : h->tcl) free_tc(t);
-  for (TcLayer& t : h->bwd) free_tc(t);
-  train_free(h);
-  cudaFree(h->ens_x); cudaFree(h->ens_x2); cudaFree(h->ens_y); cudaFree(h->ensio_x); cudaFree(h->ensio_x2); cudaFree(h->ensio_y);
-  cudaFree(h->d_first_w);
-  cudaFree(h->d_first_bias);
-  cudaFree(h->d_first_alpha);
-  cudaFree(h->d_last_w);
-  cudaFree(h->feat_hi);
-  cudaFree(h->feat_lo);
-  cudaFree(h->b1_hi);
-  cudaFree(h->b1_lo);
-  cudaFree(h->nin_hi);
-  cudaFree(h->nin_lo);
-  cudaFree(h->mid_hi);
-  cudaFree(h->mid_lo);
-  cudaFree(h->hr);
-  cudaFree(h->vbuf);
-  cudaFree(h->ds_feat); cudaFree(h->ds_b1); cudaFree(h->ds_nin); cudaFree(h->ds_mid); cudaFree(h->ds_hr);
-  for (auto& d : h->ds) { cudaFree(d.dw); cudaFree(d.pw); cudaFree(d.bias); cudaFree(d.alpha); }
-  cudaFree(h->ds_ab.pw); cudaFree(h->ds_ab.bias); cudaFree(h->ds_ab.alpha);
-  cudaFree(h->io_x);
-  cudaFree(h->io_x2);
-  cudaFree(h->io_y);
-  cudaFree(h->tile_x); cudaFree(h->tile_x2); cudaFree(h->tile_y);
-  for (auto& pt : h->pil_tables) { cudaFree(pt.k); cudaFree(pt.bounds); }
-  cudaFree(h->pil_tmp);
-  cudaFree(h->ps_lr); cudaFree(h->ps_bic); cudaFree(h->ps_true); cudaFree(h->ps_idx);
-  h->plans.clear();
-  if (h->cap_stream) cudaStreamDestroy(h->cap_stream);
-  if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
-  if (h->x2_ready) cudaEventDestroy(h->x2_ready);
   delete h;
   return 0;
 }
@@ -1721,40 +1656,35 @@ int dcscn_forward_host(dcscn_handle* h, const float* x, const float* x2, float* 
   CUDA_TRY(cudaSetDevice(h->cfg.device_id));
   const size_t lr = (size_t)n * height * width;
   const size_t hr = lr * h->cfg.scale * h->cfg.scale;
-  if (hr > h->io_cap) {
-    cudaFree(h->io_x);
-    cudaFree(h->io_x2);
-    cudaFree(h->io_y);
-    h->io_x = h->io_x2 = h->io_y = nullptr;
-    CUDA_TRY(cudaMalloc((void**)&h->io_x, lr * sizeof(float)));
-    CUDA_TRY(cudaMalloc((void**)&h->io_x2, hr * sizeof(float)));
-    CUDA_TRY(cudaMalloc((void**)&h->io_y, hr * sizeof(float)));
-    h->io_cap = hr;
-  }
+  if (h->io_x.grow(lr) || h->io_x2.grow(hr) || h->io_y.grow(hr)) return 1;
   cudaStream_t st = 0;
   if (!h->copy_stream) {
-    CUDA_TRY(cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
-    CUDA_TRY(cudaEventCreateWithFlags(&h->x2_ready, cudaEventDisableTiming));
+    cudaStream_t s;
+    cudaEvent_t e;
+    CUDA_TRY(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+    h->copy_stream.reset(s);
+    CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    h->x2_ready.reset(e);
   }
   // x feeds the first kernel; x2 (4x / 9x / 16x the bytes) is only read by the very last one, so it is copied on a second
   // stream while the conv stack runs and the last kernel waits for it
-  CUDA_TRY(cudaMemcpyAsync(h->io_x, x, lr * sizeof(float), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(h->io_x.get(), x, lr * sizeof(float), cudaMemcpyHostToDevice, st));
   if (x2) {
-    CUDA_TRY(cudaMemcpyAsync(h->io_x2, x2, hr * sizeof(float), cudaMemcpyHostToDevice, h->copy_stream));
-    CUDA_TRY(cudaEventRecord(h->x2_ready, h->copy_stream));
+    CUDA_TRY(cudaMemcpyAsync(h->io_x2.get(), x2, hr * sizeof(float), cudaMemcpyHostToDevice, h->copy_stream.get()));
+    CUDA_TRY(cudaEventRecord(h->x2_ready.get(), h->copy_stream.get()));
     h->wait_x2 = true;
   } else {
     // x2 = Pillow-bicubic up-scale of x, formed in HBM (what util.resize_image_by_pil does on the host, bit for bit)
     const int s = h->cfg.scale;
-    if (pil_resize_impl(h, h->io_x, h->io_x2, n, height, width, s * height, s * width, st)) return 1;
+    if (pil_resize_impl(h, h->io_x.get(), h->io_x2.get(), n, height, width, s * height, s * width, st)) return 1;
   }
-  const int rc = forward_any(h, h->io_x, h->io_x2, h->io_y, n, height, width, st);
+  const int rc = forward_any(h, h->io_x.get(), h->io_x2.get(), h->io_y.get(), n, height, width, st);
   h->wait_x2 = false;
   if (rc) {
-    cudaStreamSynchronize(h->copy_stream);
+    cudaStreamSynchronize(h->copy_stream.get());
     return 1;
   }
-  CUDA_TRY(cudaMemcpyAsync(y, h->io_y, hr * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(y, h->io_y.get(), hr * sizeof(float), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
   return 0;
 }
@@ -1769,15 +1699,7 @@ static int ensemble_impl(dcscn_handle* h, const float* x, const float* x2, doubl
   CUDA_TRY(cudaSetDevice(h->cfg.device_id));
   const int s = h->cfg.scale;
   const size_t lr = (size_t)height * width, hr = lr * s * s;
-  if (hr > h->ens_cap) {
-    cudaFree(h->ens_x); cudaFree(h->ens_x2); cudaFree(h->ens_y);
-    h->ens_x = h->ens_x2 = h->ens_y = nullptr;
-    h->ens_cap = 0;
-    CUDA_TRY(cudaMalloc((void**)&h->ens_x, 4 * lr * sizeof(float)));
-    CUDA_TRY(cudaMalloc((void**)&h->ens_x2, 4 * hr * sizeof(float)));
-    CUDA_TRY(cudaMalloc((void**)&h->ens_y, 8 * hr * sizeof(float)));
-    h->ens_cap = hr;
-  }
+  if (h->ens_x.grow(4 * lr) || h->ens_x2.grow(4 * hr) || h->ens_y.grow(8 * hr)) return 1;
   const int grid_lr = (int)std::min<size_t>((4 * lr + 255) / 256, (size_t)h->sm_count * 8);
   const int grid_hr = (int)std::min<size_t>((4 * hr + 255) / 256, (size_t)h->sm_count * 8);
   for (int grp = 0; grp < 2; ++grp) {
@@ -1786,15 +1708,15 @@ static int ensemble_impl(dcscn_handle* h, const float* x, const float* x2, doubl
     for (int t = 4 * grp; t < 4 * grp + 4; ++t)
       if ((mask >> t) & 1) sel.t[sel.count++] = t;
     if (sel.count == 0) continue;
-    ensemble_flip_kernel<<<grid_lr, 256, 0, st>>>(x, h->ens_x, height, width, sel);
-    ensemble_flip_kernel<<<grid_hr, 256, 0, st>>>(x2, h->ens_x2, s * height, s * width, sel);
+    ensemble_flip_kernel<<<grid_lr, 256, 0, st>>>(x, h->ens_x.get(), height, width, sel);
+    ensemble_flip_kernel<<<grid_hr, 256, 0, st>>>(x2, h->ens_x2.get(), s * height, s * width, sel);
     CUDA_TRY(cudaGetLastError());
     h->launches += 2;
     const int fh = grp == 0 ? height : width, fw = grp == 0 ? width : height;
-    if (forward_any(h, h->ens_x, h->ens_x2, h->ens_y + (size_t)grp * 4 * hr, sel.count, fh, fw, st)) return 1;
+    if (forward_any(h, h->ens_x.get(), h->ens_x2.get(), h->ens_y.get() + (size_t)grp * 4 * hr, sel.count, fh, fw, st)) return 1;
   }
   ensemble_reduce_kernel<<<(int)std::min<size_t>((hr + 255) / 256, (size_t)h->sm_count * 8), 256, 0, st>>>(
-      h->ens_y, h->ens_y + 4 * hr, y, s * height, s * width, mask, divisor);
+      h->ens_y.get(), h->ens_y.get() + 4 * hr, y, s * height, s * width, mask, divisor);
   CUDA_TRY(cudaGetLastError());
   h->launches++;
   return 0;
@@ -1818,26 +1740,17 @@ int dcscn_forward_ensemble_host(dcscn_handle* h, const float* x, const float* x2
   CUDA_TRY(cudaSetDevice(h->cfg.device_id));
   const size_t lr = (size_t)height * width;
   const size_t hr = lr * h->cfg.scale * h->cfg.scale;
-  if (hr > h->ensio_cap) {
-    cudaFree(h->ensio_x); cudaFree(h->ensio_x2); cudaFree(h->ensio_y);
-    h->ensio_x = h->ensio_x2 = nullptr;
-    h->ensio_y = nullptr;
-    h->ensio_cap = 0;
-    CUDA_TRY(cudaMalloc((void**)&h->ensio_x, lr * sizeof(float)));
-    CUDA_TRY(cudaMalloc((void**)&h->ensio_x2, hr * sizeof(float)));
-    CUDA_TRY(cudaMalloc((void**)&h->ensio_y, hr * sizeof(double)));
-    h->ensio_cap = hr;
-  }
+  if (h->ensio_x.grow(lr) || h->ensio_x2.grow(hr) || h->ensio_y.grow(hr)) return 1;
   cudaStream_t st = 0;
-  CUDA_TRY(cudaMemcpyAsync(h->ensio_x, x, lr * sizeof(float), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(h->ensio_x.get(), x, lr * sizeof(float), cudaMemcpyHostToDevice, st));
   if (x2) {
-    CUDA_TRY(cudaMemcpyAsync(h->ensio_x2, x2, hr * sizeof(float), cudaMemcpyHostToDevice, st));
-  } else if (pil_resize_impl(h, h->ensio_x, h->ensio_x2, 1, height, width, h->cfg.scale * height, h->cfg.scale * width, st)) {
+    CUDA_TRY(cudaMemcpyAsync(h->ensio_x2.get(), x2, hr * sizeof(float), cudaMemcpyHostToDevice, st));
+  } else if (pil_resize_impl(h, h->ensio_x.get(), h->ensio_x2.get(), 1, height, width, h->cfg.scale * height, h->cfg.scale * width, st)) {
     return 1;
   }
   if (flips < 1 || flips > 8) return fail("forward_ensemble: flips must be 1..8 (got %d)", flips);
-  if (ensemble_impl(h, h->ensio_x, h->ensio_x2, h->ensio_y, height, width, (1 << flips) - 1, (double)flips, st)) return 1;
-  CUDA_TRY(cudaMemcpyAsync(y, h->ensio_y, hr * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (ensemble_impl(h, h->ensio_x.get(), h->ensio_x2.get(), h->ensio_y.get(), height, width, (1 << flips) - 1, (double)flips, st)) return 1;
+  CUDA_TRY(cudaMemcpyAsync(y, h->ensio_y.get(), hr * sizeof(double), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
   return 0;
 }
@@ -1860,13 +1773,13 @@ int dcscn_get_activation(dcscn_handle* h, const char* tensor, float* host_data, 
     if (t.rfind("CNN", 0) == 0) {
       int i = atoi(t.c_str() + 3) - 1;
       if (i < 0 || i >= c.layers) return fail("dcscn_get_activation: no tensor '%s'", tensor);
-      src = h->ds_feat; pitch = h->ds_total; off = h->ds_off[i]; ch = h->filters[i];
-    } else if (t == "A1") { src = h->ds_nin; pitch = cps; off = c.nin_filters2; ch = c.nin_filters;
-    } else if (t == "B2") { src = h->ds_nin; pitch = cps; off = 0; ch = c.nin_filters2;
-    } else if (t == "B1") { src = h->ds_b1; pitch = c.nin_filters2; off = 0; ch = c.nin_filters2;
-    } else if (t == "Up-PS" && c.scale == 4) { src = h->ds_mid; pitch = cps; off = 0; ch = cps; px *= 4;
+      src = h->ds_feat.get(); pitch = h->ds_total; off = h->ds_off[i]; ch = h->filters[i];
+    } else if (t == "A1") { src = h->ds_nin.get(); pitch = cps; off = c.nin_filters2; ch = c.nin_filters;
+    } else if (t == "B2") { src = h->ds_nin.get(); pitch = cps; off = 0; ch = c.nin_filters2;
+    } else if (t == "B1") { src = h->ds_b1.get(); pitch = c.nin_filters2; off = 0; ch = c.nin_filters2;
+    } else if (t == "Up-PS" && c.scale == 4) { src = h->ds_mid.get(); pitch = cps; off = 0; ch = cps; px *= 4;
     } else if ((t == "Up-PS" && c.scale != 4) || (t == "Up-PS2" && c.scale == 4)) {
-      src = h->ds_hr; pitch = h->ps_out; off = 0; ch = h->ps_out; px *= (size_t)c.scale * c.scale;
+      src = h->ds_hr.get(); pitch = h->ps_out; off = 0; ch = h->ps_out; px *= (size_t)c.scale * c.scale;
     } else return fail("dcscn_get_activation: no tensor '%s'", tensor);
     if (numel != (int64_t)(px * ch)) return fail("dcscn_get_activation: '%s' has %lld elements, got %lld", tensor, (long long)(px * ch), (long long)numel);
     std::vector<float> full(px * pitch);
@@ -1888,19 +1801,19 @@ int dcscn_get_activation(dcscn_handle* h, const char* tensor, float* host_data, 
   if (t.rfind("CNN", 0) == 0) {
     int i = atoi(t.c_str() + 3) - 1;
     if (i < 0 || i >= c.layers) return fail("dcscn_get_activation: no tensor '%s'", tensor);
-    hi = h->feat_hi; lo = h->feat_lo; pitch = h->feat_pitch; off = h->feat_off[i]; ch = h->filters[i];
+    hi = h->feat_hi.get(); lo = h->feat_lo.get(); pitch = h->feat_pitch; off = h->feat_off[i]; ch = h->filters[i];
   } else if (t == "A1") {
-    hi = h->nin_hi; lo = h->nin_lo; pitch = h->nin_pitch; off = h->b1_w; ch = c.nin_filters;
+    hi = h->nin_hi.get(); lo = h->nin_lo.get(); pitch = h->nin_pitch; off = h->b1_w; ch = c.nin_filters;
   } else if (t == "B2") {
-    hi = h->nin_hi; lo = h->nin_lo; pitch = h->nin_pitch; off = 0; ch = c.nin_filters2;
+    hi = h->nin_hi.get(); lo = h->nin_lo.get(); pitch = h->nin_pitch; off = 0; ch = c.nin_filters2;
   } else if (t == "B1") {
-    hi = h->b1_hi; lo = h->b1_lo; pitch = h->b1_w; off = 0; ch = c.nin_filters2;
+    hi = h->b1_hi.get(); lo = h->b1_lo.get(); pitch = h->b1_w; off = 0; ch = c.nin_filters2;
   } else if (t == "Up-PS" && c.scale == 4) {
-    hi = h->mid_hi; lo = h->mid_lo; pitch = h->mid_pitch; off = 0; ch = c.nin_filters + c.nin_filters2; px *= 4;
+    hi = h->mid_hi.get(); lo = h->mid_lo.get(); pitch = h->mid_pitch; off = 0; ch = c.nin_filters + c.nin_filters2; px *= 4;
   } else if (((t == "Up-PS" && c.scale != 4) || (t == "Up-PS2" && c.scale == 4)) && pl->ran_fused) {
     return fail("dcscn_get_activation: '%s' is not materialised when the R-CNN1 fusion is on (set option fuse_last=0)", tensor);
   } else if ((t == "Up-PS" && c.scale != 4) || (t == "Up-PS2" && c.scale == 4)) {
-    f32 = h->hr; pitch = h->ps_out; ch = h->ps_out; px *= (size_t)c.scale * c.scale;
+    f32 = h->hr.get(); pitch = h->ps_out; ch = h->ps_out; px *= (size_t)c.scale * c.scale;
   } else {
     return fail("dcscn_get_activation: no tensor '%s'", tensor);
   }
@@ -1909,12 +1822,10 @@ int dcscn_get_activation(dcscn_handle* h, const char* tensor, float* host_data, 
   if (f32) {
     CUDA_TRY(cudaMemcpy(full.data(), f32, full.size() * sizeof(float), cudaMemcpyDeviceToHost));
   } else {
-    float* tmp = nullptr;
-    CUDA_TRY(cudaMalloc((void**)&tmp, full.size() * sizeof(float)));
-    planes_to_f32_kernel<<<1024, 256>>>(hi, planes(h) == 2 ? lo : nullptr, tmp, full.size());
-    cudaError_t e = cudaMemcpy(full.data(), tmp, full.size() * sizeof(float), cudaMemcpyDeviceToHost);
-    cudaFree(tmp);
-    if (e != cudaSuccess) return fail("dcscn_get_activation: copy failed: %s", cudaGetErrorString(e));
+    DeviceArray<float> tmp;
+    if (tmp.alloc(full.size())) return 1;
+    planes_to_f32_kernel<<<1024, 256>>>(hi, planes(h) == 2 ? lo : nullptr, tmp.get(), full.size());
+    CUDA_TRY(cudaMemcpy(full.data(), tmp.get(), full.size() * sizeof(float), cudaMemcpyDeviceToHost));
   }
   for (size_t p = 0; p < px; ++p)
     for (int k = 0; k < ch; ++k) host_data[p * ch + k] = full[p * pitch + off + k];
@@ -1966,9 +1877,9 @@ int dcscn_get_timings(dcscn_handle* h, float* ms, int capacity, int* count, char
   if (!h || !count) return fail("dcscn_get_timings: null argument");
   *count = 0;
   if (h->ev_used < 2) return 0;
-  CUDA_TRY(cudaEventSynchronize(h->ev[h->ev_used - 1]));
+  CUDA_TRY(cudaEventSynchronize(h->ev[h->ev_used - 1].get()));
   const int n = h->ev_used - 1;
-  for (int i = 0; i < n && i < capacity; ++i) CUDA_TRY(cudaEventElapsedTime(&ms[i], h->ev[i], h->ev[i + 1]));
+  for (int i = 0; i < n && i < capacity; ++i) CUDA_TRY(cudaEventElapsedTime(&ms[i], h->ev[i].get(), h->ev[i + 1].get()));
   *count = n;
   if (names && names_len > 0) {
     std::string s = "CNN1";
@@ -2006,19 +1917,12 @@ int dcscn_train_step_host(dcscn_handle* h, const float* x, const float* x2, cons
   CUDA_TRY(cudaSetDevice(h->cfg.device_id));
   const size_t lr_px = (size_t)n * height * width;
   const size_t hr_px = lr_px * h->cfg.scale * h->cfg.scale;
-  if (hr_px > h->io_cap) {
-    cudaFree(h->io_x); cudaFree(h->io_x2); cudaFree(h->io_y);
-    h->io_x = h->io_x2 = h->io_y = nullptr;
-    CUDA_TRY(cudaMalloc((void**)&h->io_x, lr_px * sizeof(float)));
-    CUDA_TRY(cudaMalloc((void**)&h->io_x2, hr_px * sizeof(float)));
-    CUDA_TRY(cudaMalloc((void**)&h->io_y, hr_px * sizeof(float)));
-    h->io_cap = hr_px;
-  }
+  if (h->io_x.grow(lr_px) || h->io_x2.grow(hr_px) || h->io_y.grow(hr_px)) return 1;
   cudaStream_t st = 0;
-  CUDA_TRY(cudaMemcpyAsync(h->io_x, x, lr_px * sizeof(float), cudaMemcpyHostToDevice, st));
-  CUDA_TRY(cudaMemcpyAsync(h->io_x2, x2, hr_px * sizeof(float), cudaMemcpyHostToDevice, st));
-  CUDA_TRY(cudaMemcpyAsync(h->io_y, y, hr_px * sizeof(float), cudaMemcpyHostToDevice, st));
-  return train_step_impl(h, h->io_x, h->io_x2, h->io_y, n, height, width, lr, seed, apply_update, out_loss, out_mse, st);
+  CUDA_TRY(cudaMemcpyAsync(h->io_x.get(), x, lr_px * sizeof(float), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(h->io_x2.get(), x2, hr_px * sizeof(float), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(h->io_y.get(), y, hr_px * sizeof(float), cudaMemcpyHostToDevice, st));
+  return train_step_impl(h, h->io_x.get(), h->io_x2.get(), h->io_y.get(), n, height, width, lr, seed, apply_update, out_loss, out_mse, st);
 }
 
 int dcscn_patch_store_set(dcscn_handle* h, const uint8_t* lr, const uint8_t* bicubic, const uint8_t* truth, int64_t count,
@@ -2026,19 +1930,13 @@ int dcscn_patch_store_set(dcscn_handle* h, const uint8_t* lr, const uint8_t* bic
   if (!h || !lr || !bicubic || !truth) return fail("dcscn_patch_store_set: null argument");
   if (count <= 0 || count > 0x7FFFFFFF || patch_height <= 0 || patch_width <= 0) return fail("dcscn_patch_store_set: bad size");
   CUDA_TRY(cudaSetDevice(h->cfg.device_id));
-  for (auto& pt : h->pil_tables) { cudaFree(pt.k); cudaFree(pt.bounds); }
-  cudaFree(h->pil_tmp);
-  cudaFree(h->ps_lr); cudaFree(h->ps_bic); cudaFree(h->ps_true);
-  h->ps_lr = h->ps_bic = h->ps_true = nullptr;
   h->ps_count = 0;
   const size_t s2 = (size_t)h->cfg.scale * h->cfg.scale;
   const size_t lr_b = (size_t)count * patch_height * patch_width, hr_b = lr_b * s2;
-  CUDA_TRY(cudaMalloc((void**)&h->ps_lr, lr_b));
-  CUDA_TRY(cudaMalloc((void**)&h->ps_bic, hr_b));
-  CUDA_TRY(cudaMalloc((void**)&h->ps_true, hr_b));
-  CUDA_TRY(cudaMemcpy(h->ps_lr, lr, lr_b, cudaMemcpyHostToDevice));
-  CUDA_TRY(cudaMemcpy(h->ps_bic, bicubic, hr_b, cudaMemcpyHostToDevice));
-  CUDA_TRY(cudaMemcpy(h->ps_true, truth, hr_b, cudaMemcpyHostToDevice));
+  if (h->ps_lr.alloc(lr_b) || h->ps_bic.alloc(hr_b) || h->ps_true.alloc(hr_b)) return 1;
+  CUDA_TRY(cudaMemcpy(h->ps_lr.get(), lr, lr_b, cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(h->ps_bic.get(), bicubic, hr_b, cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(h->ps_true.get(), truth, hr_b, cudaMemcpyHostToDevice));
   h->ps_count = count;
   h->ps_h = patch_height;
   h->ps_w = patch_width;
@@ -2055,28 +1953,14 @@ static int patch_gather(dcscn_handle* h, const int32_t* indices, int n, float ma
   }
   const int s = h->cfg.scale;
   const size_t lr_px = (size_t)n * h->ps_h * h->ps_w, hr_px = lr_px * s * s;
-  if (hr_px > h->io_cap) {
-    cudaFree(h->io_x); cudaFree(h->io_x2); cudaFree(h->io_y);
-    h->io_x = h->io_x2 = h->io_y = nullptr;
-    h->io_cap = 0;
-    CUDA_TRY(cudaMalloc((void**)&h->io_x, lr_px * sizeof(float)));
-    CUDA_TRY(cudaMalloc((void**)&h->io_x2, hr_px * sizeof(float)));
-    CUDA_TRY(cudaMalloc((void**)&h->io_y, hr_px * sizeof(float)));
-    h->io_cap = hr_px;
-  }
-  if (n > h->ps_idx_cap) {
-    cudaFree(h->ps_idx);
-    h->ps_idx = nullptr;
-    CUDA_TRY(cudaMalloc((void**)&h->ps_idx, (size_t)n * sizeof(int)));
-    h->ps_idx_cap = n;
-  }
-  CUDA_TRY(cudaMemcpyAsync(h->ps_idx, indices, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
+  if (h->io_x.grow(lr_px) || h->io_x2.grow(hr_px) || h->io_y.grow(hr_px) || h->ps_idx.grow(n)) return 1;
+  CUDA_TRY(cudaMemcpyAsync(h->ps_idx.get(), indices, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
   const double scale = (double)max_value / 255.0;
   const int grid_lr = (int)std::min<size_t>((lr_px + 255) / 256, (size_t)h->sm_count * 8);
   const int grid_hr = (int)std::min<size_t>((hr_px + 255) / 256, (size_t)h->sm_count * 8);
-  patch_gather_kernel<<<grid_lr, 256, 0, st>>>(h->ps_lr, h->ps_idx, h->io_x, n, h->ps_h, h->ps_w, scale);
-  patch_gather_kernel<<<grid_hr, 256, 0, st>>>(h->ps_bic, h->ps_idx, h->io_x2, n, s * h->ps_h, s * h->ps_w, scale);
-  patch_gather_kernel<<<grid_hr, 256, 0, st>>>(h->ps_true, h->ps_idx, h->io_y, n, s * h->ps_h, s * h->ps_w, scale);
+  patch_gather_kernel<<<grid_lr, 256, 0, st>>>(h->ps_lr.get(), h->ps_idx.get(), h->io_x.get(), n, h->ps_h, h->ps_w, scale);
+  patch_gather_kernel<<<grid_hr, 256, 0, st>>>(h->ps_bic.get(), h->ps_idx.get(), h->io_x2.get(), n, s * h->ps_h, s * h->ps_w, scale);
+  patch_gather_kernel<<<grid_hr, 256, 0, st>>>(h->ps_true.get(), h->ps_idx.get(), h->io_y.get(), n, s * h->ps_h, s * h->ps_w, scale);
   CUDA_TRY(cudaGetLastError());
   h->launches += 3;
   return 0;
@@ -2088,7 +1972,7 @@ int dcscn_train_step_indexed(dcscn_handle* h, const int32_t* indices, int n, flo
   CUDA_TRY(cudaSetDevice(h->cfg.device_id));
   cudaStream_t st = 0;
   if (patch_gather(h, indices, n, max_value, st)) return 1;
-  return train_step_impl(h, h->io_x, h->io_x2, h->io_y, n, h->ps_h, h->ps_w, lr, seed, apply_update, out_loss, out_mse, st);
+  return train_step_impl(h, h->io_x.get(), h->io_x2.get(), h->io_y.get(), n, h->ps_h, h->ps_w, lr, seed, apply_update, out_loss, out_mse, st);
 }
 
 int dcscn_patch_gather(dcscn_handle* h, const int32_t* indices, int n, float max_value, float* x, float* x2, float* y) {
@@ -2098,9 +1982,9 @@ int dcscn_patch_gather(dcscn_handle* h, const int32_t* indices, int n, float max
   if (patch_gather(h, indices, n, max_value, st)) return 1;
   const int s = h->cfg.scale;
   const size_t lr_px = (size_t)n * h->ps_h * h->ps_w, hr_px = lr_px * s * s;
-  CUDA_TRY(cudaMemcpyAsync(x, h->io_x, lr_px * sizeof(float), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(x2, h->io_x2, hr_px * sizeof(float), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(y, h->io_y, hr_px * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(x, h->io_x.get(), lr_px * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(x2, h->io_x2.get(), hr_px * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(y, h->io_y.get(), hr_px * sizeof(float), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
   return 0;
 }
@@ -2113,13 +1997,13 @@ int dcscn_get_grad(dcscn_handle* h, const char* name, float* host_data, int64_t 
   const ParamDef& p = h->params[it->second];
   if (numel != p.numel()) return fail("dcscn_get_grad: '%s' has %lld elements, got %lld", name, (long long)p.numel(), (long long)numel);
   CUDA_TRY(cudaSetDevice(h->cfg.device_id));
-  CUDA_TRY(cudaMemcpy(host_data, h->train->d_g + h->train->off[it->second], (size_t)numel * sizeof(float), cudaMemcpyDeviceToHost));
+  CUDA_TRY(cudaMemcpy(host_data, h->train->d_g.get() + h->train->off[it->second], (size_t)numel * sizeof(float), cudaMemcpyDeviceToHost));
   return 0;
 }
 
 int dcscn_get_train_tensor(dcscn_handle* h, const char* name, float* host_data, int64_t numel) {
   if (!h || !name || !host_data) return fail("dcscn_get_train_tensor: null argument");
-  TrainState* t = h->train;
+  TrainState* t = h->train.get();
   if (!t || t->last_px == 0) return fail("dcscn_get_train_tensor: no train step of a tensor-core graph has run yet");
   CUDA_TRY(cudaSetDevice(h->cfg.device_id));
   CUDA_TRY(cudaDeviceSynchronize());
@@ -2135,10 +2019,10 @@ int dcscn_get_train_tensor(dcscn_handle* h, const char* name, float* host_data, 
     if (l.rfind("CNN", 0) == 0) {
       const int i = atoi(l.c_str() + 3) - 1;
       if (i < 0 || i >= h->cfg.layers) return fail("dcscn_get_train_tensor: no tensor '%s'", name);
-      src = t->zneg_feat + h->feat_off[i]; pitch = h->feat_pitch; ch = h->filters[i];
-    } else if (l == "A1") { src = t->zneg_nin + h->b1_w; pitch = h->nin_pitch; ch = h->cfg.nin_filters;
-    } else if (l == "B2") { src = t->zneg_nin; pitch = h->nin_pitch; ch = h->cfg.nin_filters2;
-    } else if (l == "B1") { src = t->zneg_b1; pitch = h->b1_w; ch = h->cfg.nin_filters2;
+      src = t->zneg_feat.get() + h->feat_off[i]; pitch = h->feat_pitch; ch = h->filters[i];
+    } else if (l == "A1") { src = t->zneg_nin.get() + h->b1_w; pitch = h->nin_pitch; ch = h->cfg.nin_filters;
+    } else if (l == "B2") { src = t->zneg_nin.get(); pitch = h->nin_pitch; ch = h->cfg.nin_filters2;
+    } else if (l == "B1") { src = t->zneg_b1.get(); pitch = h->b1_w; ch = h->cfg.nin_filters2;
     } else return fail("dcscn_get_train_tensor: no tensor '%s'", name);
     px = t->last_px;
     hi.resize(px * ch);
@@ -2151,13 +2035,13 @@ int dcscn_get_train_tensor(dcscn_handle* h, const char* name, float* host_data, 
     px = c.px; ch = c.ch;
     if (numel != (int64_t)(px * ch)) return fail("dcscn_get_train_tensor: '%s' has %lld elements, got %lld", name, (long long)(px * ch), (long long)numel);
     if (c.f32) {
-      CUDA_TRY(cudaMemcpy(host_data, c.hi, px * sizeof(float), cudaMemcpyDeviceToHost));
+      CUDA_TRY(cudaMemcpy(host_data, c.hi.get(), px * sizeof(float), cudaMemcpyDeviceToHost));
       return 0;
     }
     hi.resize(px * ch);
     lo.resize(px * ch);
-    CUDA_TRY(cudaMemcpy(hi.data(), c.hi, hi.size() * sizeof(__half), cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemcpy(lo.data(), c.lo, lo.size() * sizeof(__half), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(hi.data(), c.hi.get(), hi.size() * sizeof(__half), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(lo.data(), c.lo.get(), lo.size() * sizeof(__half), cudaMemcpyDeviceToHost));
   }
   if (numel != (int64_t)(px * ch)) return fail("dcscn_get_train_tensor: '%s' has %lld elements, got %lld", name, (long long)(px * ch), (long long)numel);
   for (size_t i = 0; i < hi.size(); ++i) host_data[i] = __half2float(hi[i]) + (lo.empty() ? 0.f : __half2float(lo[i]));
@@ -2173,7 +2057,7 @@ int dcscn_get_adam_slot(dcscn_handle* h, const char* name, int slot, float* host
   const ParamDef& p = h->params[it->second];
   if (numel != p.numel() || (slot != 0 && slot != 1)) return fail("dcscn_get_adam_slot: bad size or slot");
   CUDA_TRY(cudaSetDevice(h->cfg.device_id));
-  const float* src = (slot == 0 ? h->train->d_m : h->train->d_v) + h->train->off[it->second];
+  const float* src = (slot == 0 ? h->train->d_m.get() : h->train->d_v.get()) + h->train->off[it->second];
   CUDA_TRY(cudaMemcpy(host_data, src, (size_t)numel * sizeof(float), cudaMemcpyDeviceToHost));
   return 0;
 }
@@ -2187,7 +2071,7 @@ int dcscn_set_adam_slot(dcscn_handle* h, const char* name, int slot, const float
   if (it == h->param_index.end()) return fail("dcscn_set_adam_slot: unknown variable '%s'", name);
   const ParamDef& p = h->params[it->second];
   if (numel != p.numel() || (slot != 0 && slot != 1)) return fail("dcscn_set_adam_slot: bad size or slot");
-  float* dst = (slot == 0 ? h->train->d_m : h->train->d_v) + h->train->off[it->second];
+  float* dst = (slot == 0 ? h->train->d_m.get() : h->train->d_v.get()) + h->train->off[it->second];
   CUDA_TRY(cudaMemcpy(dst, host_data, (size_t)numel * sizeof(float), cudaMemcpyHostToDevice));
   return 0;
 }
@@ -2217,7 +2101,7 @@ static int optimizer_slot_view(dcscn_handle* h, const char* fn, const char* name
   if (slot < 0 || slot >= optimizer_slot_count(h->cfg.optimizer))
     return fail("%s: optimizer %d has no slot %d", fn, h->cfg.optimizer, slot);
   *off = h->train ? h->train->off[it->second] : 0;
-  *buf = !h->train ? nullptr : slot == 0 ? h->train->d_m : h->train->d_v;
+  *buf = !h->train ? nullptr : slot == 0 ? h->train->d_m.get() : h->train->d_v.get();
   return 0;
 }
 
@@ -2258,7 +2142,7 @@ int dcscn_reset_optimizer(dcscn_handle* h) {
 int dcscn_grad_buffer(dcscn_handle* h, float** dev_ptr, int64_t* count) {
   if (!h || !dev_ptr || !count) return fail("dcscn_grad_buffer: null argument");
   if (!h->train || h->train->total == 0) return fail("dcscn_grad_buffer: no train step has run yet");
-  *dev_ptr = h->train->d_g;
+  *dev_ptr = h->train->d_g.get();
   *count = (int64_t)h->train->total + 2;   // gradients of every trainable, then {image_loss, mse} of the last step
   return 0;
 }
@@ -2305,7 +2189,7 @@ int dcscn_dropout_mask(dcscn_handle* h, const char* tensor, uint32_t seed, int n
 }
 
 int64_t dcscn_launch_count(dcscn_handle* h) { return h ? h->launches : 0; }
-int64_t dcscn_device_bytes(dcscn_handle* h) { return h ? h->device_bytes + h->tile_bytes : 0; }
+int64_t dcscn_device_bytes(dcscn_handle* h) { return h ? workspace_bytes(h) : 0; }
 
 int dcscn_tile_halo(dcscn_handle* h, int* lr_pixels) {
   if (!h || !lr_pixels) return fail("dcscn_tile_halo: null argument");

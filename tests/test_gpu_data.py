@@ -23,6 +23,15 @@ def build_set(scale, size):
     return ds
 
 
+def host_batch(ds, idx, max_value=255.0):
+    """(x, x2, y) as the host loader feeds patches `idx`, fp32."""
+    host = []
+    for k in idx:
+        ds.batch_index, ds.index = [int(k)], 0          # make the host loader serve exactly patch k
+        host.append(ds.load_batch_image(max_value))
+    return tuple(np.stack([h[j] for h in host]).astype(np.float32) for j in range(3))
+
+
 @pytest.mark.parametrize("max_value", [255.0, 1.0])
 def test_gather_equals_the_host_loader(max_value):
     import dcscn_oracle as O
@@ -34,13 +43,7 @@ def test_gather_equals_the_host_loader(max_value):
     rs = np.random.RandomState(0)
     idx = rs.randint(0, ds.count, size=13)
     x, x2, y = eng.gather_patches(idx, max_value=max_value)
-    host = []
-    for k in idx:
-        ds.batch_index, ds.index = [int(k)], 0          # make the host loader serve exactly patch k
-        host.append(ds.load_batch_image(max_value))
-    hx = np.stack([h[0] for h in host]).astype(np.float32)
-    hx2 = np.stack([h[1] for h in host]).astype(np.float32)
-    hy = np.stack([h[2] for h in host]).astype(np.float32)
+    hx, hx2, hy = host_batch(ds, idx, max_value)
     np.testing.assert_array_equal(x, hx)
     np.testing.assert_array_equal(x2, hx2)
     np.testing.assert_array_equal(y, hy)
@@ -98,6 +101,32 @@ def test_device_bicubic_is_pillow_bit_for_bit(shape, scale):
         ref = util.resize_image_by_pil(a[i].reshape(h, w, 1).astype(np.float64), scale)[:, :, 0]
         assert ref.shape == (oh, ow)
         np.testing.assert_array_equal(got[i], ref)
+    eng.close()
+
+
+def test_set_patch_store_keeps_the_bicubic_tables():
+    """Setting the patch store replaces the three patch arrays only: the Pillow tables and the bicubic scratch that an
+    earlier device resize cached stay valid, so the same resize after it is still Pillow bit for bit, and each store
+    serves its own patches as the host loader does."""
+    import torch
+    from helper import engine as E, utilty as util
+    eng = E.Engine(E.make_config(**KW))
+    rs = np.random.RandomState(7)
+    n, h, w = 2, 37, 53
+    a = (rs.rand(n, h, w) * 255).astype(np.float32)
+    ref = np.stack([util.resize_image_by_pil(a[i].reshape(h, w, 1).astype(np.float64), 2)[:, :, 0] for i in range(n)])
+
+    def check_resize():
+        np.testing.assert_array_equal(eng.bicubic_resize(torch.from_numpy(a).cuda(), 2 * h, 2 * w).cpu().numpy(), ref)
+
+    check_resize()
+    for size in (24, 16):          # the second store replaces the first
+        ds = build_set(2, size)
+        eng.set_patch_store(ds.input_images, ds.input_interpolated_images, ds.true_images)
+        check_resize()
+        idx = rs.randint(0, ds.count, size=9)
+        for got, want in zip(eng.gather_patches(idx), host_batch(ds, idx)):
+            np.testing.assert_array_equal(got, want)
     eng.close()
 
 
