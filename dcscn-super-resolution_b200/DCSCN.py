@@ -441,6 +441,7 @@ class SuperResolution:
         self.train = loader.DynamicDataSets(self.scale, batch_image_size, channels=self.channels,
                                             resampling_method=self.resampling_method)
         self.train.set_data_dir(data_dir)
+        self._images_on_device = False    # uploaded to HBM by init_epoch_index once the engine exists
 
     def load_datasets(self, data_dir, batch_dir, batch_image_size, stride_size=0):
         """DCSCN.py:155-173"""
@@ -477,6 +478,14 @@ class SuperResolution:
                                             self.train.true_images)
                 self._patches_on_device = True
             self.batch_indices = np.zeros(self.local_batch, dtype=np.int64)
+        # random-crop data sets (the default): the decoded images move to HBM once and a mini-batch becomes a list of crop
+        # descriptors (image, top, left, mirror) drawn on the host (helper/engine.py: set_image_store / train_step_crops)
+        self.batch_crops = None
+        if isinstance(self.train, loader.DynamicDataSets) and self.engine is not None and self.train.count > 0:
+            if not getattr(self, "_images_on_device", False):
+                self.engine.set_image_store(self.train.decoded_images())
+                self._images_on_device = True
+            self.batch_crops = np.zeros((self.local_batch, 4), dtype=np.int32)
         self.training_psnr_sum = 0
         self.training_loss_sum = 0
         self.training_step = 0
@@ -487,6 +496,10 @@ class SuperResolution:
         if getattr(self, "batch_indices", None) is not None:            # patches already live in HBM: draw the indices only
             for i in range(len(self.batch_indices)):
                 self.batch_indices[i] = self.train.get_next_image_no()
+            return
+        if getattr(self, "batch_crops", None) is not None:              # images already live in HBM: draw the crops only
+            for i in range(len(self.batch_crops)):
+                self.batch_crops[i] = self.train.draw_crop()
             return
         for i in range(len(self.batch_input)):
             self.batch_input[i], self.batch_input_bicubic[i], self.batch_true[i] = self.train.load_batch_image(
@@ -505,6 +518,14 @@ class SuperResolution:
             else:
                 image_loss, mse = self.engine.train_step_indexed(self.batch_indices, lr=self.lr, seed=self.step,
                                                                  max_value=self.max_value)
+        elif getattr(self, "batch_crops", None) is not None:
+            if world > 1:
+                image_loss, mse = self.engine.train_step_data_parallel(None, None, None, lr=self.lr, seed=self.step * world + rank,
+                                                                       crops=self.batch_crops, patch_size=self.train.batch_image_size,
+                                                                       max_value=self.max_value)
+            else:
+                image_loss, mse = self.engine.train_step_crops(self.batch_crops, self.train.batch_image_size, lr=self.lr,
+                                                               seed=self.step, max_value=self.max_value)
         else:
             x = np.ascontiguousarray(np.stack(self.batch_input), dtype=np.float32)
             x2 = np.ascontiguousarray(np.stack(self.batch_input_bicubic), dtype=np.float32)

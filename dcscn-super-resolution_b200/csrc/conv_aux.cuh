@@ -471,6 +471,117 @@ __global__ void __launch_bounds__(256) patch_gather_kernel(const uint8_t* __rest
   }
 }
 
+// ------------------------------------------------------------- random-crop training data ----------------------
+// What loader.DynamicDataSets.load_batch_image does per patch on the host (reference helper/loader.py:310-355): crop an
+// e x e square out of a decoded image, RGB -> Y in float64, mirror left-right, Pillow-bicubic down by 1/scale and back up.
+// The decoded uint8 images live in HBM (dcscn_image_store_set); a mini-batch is a list of crop descriptors.
+struct ImageEntry {
+  long long offset;    // first byte of the image in the pixel store
+  int height, width, channels;   // channels: 3 (RGB, interleaved) or 1 (mode 'L')
+};
+
+struct CropJob {
+  int image, top, left, mirror;
+  int mode8;           // 1: a mode-'L' image, resampled by Pillow's 8-bit path; 0: an RGB image, resampled as mode 'F'
+  int slot;            // position of the crop inside its resampler group (mode-'F' crops, then mode-'L' crops)
+};
+
+// util._Y_ROW
+#define DCSCN_Y_R (65.738 / 256.0)
+#define DCSCN_Y_G (129.057 / 256.0)
+#define DCSCN_Y_B (25.064 / 256.0)
+
+// One thread per HR crop pixel (i, r, c): the source pixel is (top + r, left + (mirror ? e - 1 - c : c)).  An RGB pixel
+// becomes util.convert_rgb_to_y's float64 Y, which numpy's dot (BLAS ddot) forms as fma(b, c2, fma(g, c1, r * c0)) + 16;
+// the truth is fp32(Y * scale) (the float64 product of _rescaled, loader.py:323-327) and the mode-'F' resampler input is
+// fp32(Y) (Image.fromarray of a float64 array).  A mode-'L' pixel is fed to the 8-bit resampler as is and its truth is
+// fp32(double(u8) * scale).  scale = max_value / 255, exactly 1 at 255 (no multiply in the reference).
+__global__ void __launch_bounds__(256) crop_gather_kernel(const uint8_t* __restrict__ pixels, const ImageEntry* __restrict__ table,
+                                                          const CropJob* __restrict__ jobs, int n, int e, double scale,
+                                                          float* __restrict__ truth, float* __restrict__ f_in,
+                                                          uint8_t* __restrict__ l_in) {
+  const long long per = (long long)e * e, total = per * n;
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
+    const int i = (int)(idx / per);
+    const int r = (int)(idx - (long long)i * per);
+    const int y = r / e, x = r - y * e;
+    const CropJob j = jobs[i];
+    const ImageEntry im = table[j.image];
+    const int col = j.left + (j.mirror ? e - 1 - x : x);
+    const uint8_t* p = pixels + im.offset + ((long long)(j.top + y) * im.width + col) * im.channels;
+    const long long dst = (long long)j.slot * per + r;
+    if (im.channels == 3) {
+      const double v = __dadd_rn(__fma_rn((double)__ldg(p + 2), DCSCN_Y_B,
+                                          __fma_rn((double)__ldg(p + 1), DCSCN_Y_G, __dmul_rn((double)__ldg(p), DCSCN_Y_R))),
+                                 16.0);
+      truth[idx] = (float)__dmul_rn(v, scale);
+      f_in[dst] = (float)v;
+    } else {
+      const uint8_t v = __ldg(p);
+      truth[idx] = (float)__dmul_rn((double)v, scale);
+      l_in[dst] = v;
+    }
+  }
+}
+
+// Pillow's ImagingResampleHorizontal_8bpc / ImagingResampleVertical_8bpc (src/libImaging/Resample.c) for mode 'L': the
+// double weights of the mode-'F' tables become 22-bit fixed point, (int)(w * 2^22 + 0.5) or (int)(w * 2^22 - 0.5) for
+// w < 0 (normalize_coeffs_8bpc); the int32 sum starts at 2^21 and the sample is clamp(sum >> 22, 0, 255).
+__device__ __forceinline__ int pil_coeff8(double w) {
+  const double s = __dmul_rn(w, 4194304.0);
+  return w < 0.0 ? __double2int_rz(__dadd_rn(s, -0.5)) : __double2int_rz(__dadd_rn(s, 0.5));
+}
+
+__device__ __forceinline__ uint8_t pil_clip8(int ss) {
+  const int v = ss >> 22;
+  return (uint8_t)(v < 0 ? 0 : (v > 255 ? 255 : v));
+}
+
+__global__ void __launch_bounds__(256) pil_resample8_h_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst,
+                                                              long long rows, int W, int OW, const PilAxis ax) {
+  const long long total = rows * OW;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long row = i / OW;
+    const int xx = (int)(i - row * OW);
+    const int x0 = __ldg(ax.bounds + 2 * xx), cnt = __ldg(ax.bounds + 2 * xx + 1);
+    const double* k = ax.k + (size_t)xx * ax.ksize;
+    const uint8_t* p = src + row * W + x0;
+    int ss = 1 << 21;
+    for (int x = 0; x < cnt; ++x) ss += (int)__ldg(p + x) * pil_coeff8(__ldg(k + x));
+    dst[i] = pil_clip8(ss);
+  }
+}
+
+__global__ void __launch_bounds__(256) pil_resample8_v_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, int n,
+                                                              int H, int OH, int OW, const PilAxis ax) {
+  const long long per = (long long)OH * OW, total = per * n;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int img = (int)(i / per);
+    const int r = (int)(i - (long long)img * per);
+    const int yy = r / OW, xx = r - yy * OW;
+    const int y0 = __ldg(ax.bounds + 2 * yy), cnt = __ldg(ax.bounds + 2 * yy + 1);
+    const double* k = ax.k + (size_t)yy * ax.ksize;
+    const uint8_t* p = src + ((size_t)img * H + y0) * OW + xx;
+    int ss = 1 << 21;
+    for (int y = 0; y < cnt; ++y) ss += (int)__ldg(p + (size_t)y * OW) * pil_coeff8(__ldg(k + y));
+    dst[i] = pil_clip8(ss);
+  }
+}
+
+// out [n, H, W] (batch order) from the resampled crops of the two groups: a mode-'F' sample v becomes fp32 v * fp32(scale)
+// (numpy multiplies an fp32 array by a Python float in fp32), a mode-'L' sample fp32(double(u8) * scale).
+__global__ void __launch_bounds__(256) crop_place_kernel(const CropJob* __restrict__ jobs, const float* __restrict__ f_src,
+                                                         const uint8_t* __restrict__ l_src, float* __restrict__ out, int n,
+                                                         int H, int W, double scale) {
+  const long long per = (long long)H * W, total = per * n;
+  const float fscale = (float)scale;
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
+    const int i = (int)(idx / per);
+    const long long src = (long long)jobs[i].slot * per + (idx - (long long)i * per);
+    out[idx] = jobs[i].mode8 ? (float)__dmul_rn((double)__ldg(l_src + src), scale) : __fmul_rn(__ldg(f_src + src), fscale);
+  }
+}
+
 // ------------------------------------------------------------- self-ensemble (DCSCN.py:547-586) --------------
 // The 8 transforms of helper/utilty.py:595-617 (`flip`) as index maps on an [H][W] image:
 //   0 identity, 1 flipud, 2 fliplr, 3 flipud(fliplr), 4 rot90(+1), 5 rot90(-1), 6 flipud(rot90(+1)) = transpose,

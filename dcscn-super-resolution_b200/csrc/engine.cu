@@ -246,6 +246,14 @@ struct dcscn_handle {
   int64_t ps_count = 0;
   int ps_h = 0, ps_w = 0;
   DeviceArray<int> ps_idx;
+  // random-crop image store (dcscn_image_store_set): the decoded uint8 images and their table (a host copy checks crops),
+  // the mini-batch's crop jobs and the resampler staging of the mode-'F' (float) and mode-'L' (uint8) groups
+  DeviceArray<uint8_t> is_pixels;
+  DeviceArray<ImageEntry> is_table;
+  std::vector<ImageEntry> is_host;
+  DeviceArray<CropJob> crop_jobs;
+  DeviceArray<float> crop_f;
+  DeviceArray<uint8_t> crop_u8;
   // Pillow-bicubic resampling tables per (input size, output size) and the float32 intermediate of the two passes
   struct PilTable { int in = 0, out = 0, ksize = 0; DeviceArray<double> k; DeviceArray<int> bounds; };
   std::vector<PilTable> pil_tables;
@@ -1982,6 +1990,117 @@ int dcscn_patch_gather(dcscn_handle* h, const int32_t* indices, int n, float max
   if (patch_gather(h, indices, n, max_value, st)) return 1;
   const int s = h->cfg.scale;
   const size_t lr_px = (size_t)n * h->ps_h * h->ps_w, hr_px = lr_px * s * s;
+  CUDA_TRY(cudaMemcpyAsync(x, h->io_x.get(), lr_px * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(x2, h->io_x2.get(), hr_px * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(y, h->io_y.get(), hr_px * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  return 0;
+}
+
+int dcscn_image_store_set(dcscn_handle* h, const uint8_t* pixels, int64_t bytes, const int64_t* offsets, const int32_t* heights,
+                          const int32_t* widths, const int32_t* channels, int count) {
+  if (!h || !pixels || !offsets || !heights || !widths || !channels) return fail("dcscn_image_store_set: null argument");
+  if (count <= 0 || bytes <= 0) return fail("dcscn_image_store_set: empty store");
+  std::vector<ImageEntry> table((size_t)count);
+  for (int i = 0; i < count; ++i) {
+    if (heights[i] <= 0 || widths[i] <= 0 || (channels[i] != 1 && channels[i] != 3))
+      return fail("dcscn_image_store_set: image %d is %d x %d x %d (1 or 3 channels expected)", i, heights[i], widths[i], channels[i]);
+    const int64_t size = (int64_t)heights[i] * widths[i] * channels[i];
+    if (offsets[i] < 0 || offsets[i] > bytes - size)
+      return fail("dcscn_image_store_set: image %d (%lld bytes at offset %lld) lies outside the %lld-byte store", i,
+                  (long long)size, (long long)offsets[i], (long long)bytes);
+    table[i] = ImageEntry{(long long)offsets[i], heights[i], widths[i], channels[i]};
+  }
+  CUDA_TRY(cudaSetDevice(h->cfg.device_id));
+  h->is_host.clear();
+  if (h->is_pixels.alloc((size_t)bytes) || h->is_table.upload(table)) return 1;
+  CUDA_TRY(cudaMemcpy(h->is_pixels.get(), pixels, (size_t)bytes, cudaMemcpyHostToDevice));
+  h->is_host = std::move(table);
+  return 0;
+}
+
+// Builds the fp32 mini-batch tensors of the crops into io_x / io_x2 / io_y (shared with the host-buffer calls): crop
+// gather, the mode-'F' group through pil_resize_impl (e -> p -> e), the mode-'L' group through the 8-bit resampler, place.
+static int crop_gather(dcscn_handle* h, const int32_t* crops, int n, int patch_size, float max_value, cudaStream_t st) {
+  if (h->is_host.empty()) return fail("train_step_crops: no image store (call dcscn_image_store_set first)");
+  if (n <= 0) return fail("train_step_crops: empty mini-batch");
+  const int s = h->cfg.scale;
+  if (patch_size <= 0 || patch_size > 4096) return fail("train_step_crops: bad patch size %d", patch_size);
+  const int e = s * patch_size;
+  // util.resize_image_by_pil(truth, 1 / scale) makes int(e * (1 / scale)) pixels
+  if ((int)(e * (1.0 / s)) != patch_size) return fail("train_step_crops: a %d-pixel crop does not shrink to %d at scale %d", e, patch_size, s);
+  std::vector<CropJob> jobs((size_t)n);
+  int n8 = 0;
+  for (int i = 0; i < n; ++i) {
+    const int32_t* c = crops + 4 * (size_t)i;
+    if (c[0] < 0 || c[0] >= (int)h->is_host.size())
+      return fail("train_step_crops: crop %d names image %d (%d images)", i, c[0], (int)h->is_host.size());
+    const ImageEntry& im = h->is_host[c[0]];
+    if (c[1] < 0 || c[1] > im.height - e || c[2] < 0 || c[2] > im.width - e)
+      return fail("train_step_crops: crop %d at (%d, %d) of %d x %d does not fit image %d (%d x %d)", i, c[1], c[2], e, e, c[0],
+                  im.height, im.width);
+    if (c[3] != 0 && c[3] != 1) return fail("train_step_crops: crop %d has mirror %d (0 or 1)", i, c[3]);
+    jobs[i] = CropJob{c[0], c[1], c[2], c[3], im.channels == 1, 0};
+    n8 += im.channels == 1;
+  }
+  const int nf = n - n8;
+  for (int i = 0, kf = 0, k8 = 0; i < n; ++i) jobs[i].slot = jobs[i].mode8 ? k8++ : kf++;
+  const size_t hr = (size_t)e * e, lr = (size_t)patch_size * patch_size, mid = (size_t)e * patch_size;
+  // crop_f: input, down-scaled, up-scaled of the mode-'F' group; crop_u8: input, h-pass, down-scaled, h-pass, up-scaled
+  if (h->io_x.grow(lr * n) || h->io_x2.grow(hr * n) || h->io_y.grow(hr * n) || h->crop_jobs.grow(n) ||
+      h->crop_f.grow((2 * hr + lr) * nf) || h->crop_u8.grow((2 * hr + 2 * mid + lr) * n8))
+    return 1;
+  CUDA_TRY(cudaMemcpyAsync(h->crop_jobs.get(), jobs.data(), (size_t)n * sizeof(CropJob), cudaMemcpyHostToDevice, st));
+  const double scale = (double)max_value / 255.0;
+  float* f_in = h->crop_f.get();
+  float* f_small = f_in + hr * nf;
+  float* f_big = f_small + lr * nf;
+  uint8_t* l_in = h->crop_u8.get();
+  uint8_t* l_tmp1 = l_in + hr * n8;
+  uint8_t* l_small = l_tmp1 + mid * n8;
+  uint8_t* l_tmp2 = l_small + lr * n8;
+  uint8_t* l_big = l_tmp2 + mid * n8;
+  auto grid = [&](size_t total) { return (int)std::min<size_t>((total + 255) / 256, (size_t)h->sm_count * 16); };
+  crop_gather_kernel<<<grid(hr * n), 256, 0, st>>>(h->is_pixels.get(), h->is_table.get(), h->crop_jobs.get(), n, e, scale,
+                                                   h->io_y.get(), f_in, l_in);
+  CUDA_TRY(cudaGetLastError());
+  h->launches += 1;
+  if (nf > 0 && (pil_resize_impl(h, f_in, f_small, nf, e, e, patch_size, patch_size, st) ||
+                 pil_resize_impl(h, f_small, f_big, nf, patch_size, patch_size, e, e, st)))
+    return 1;
+  if (n8 > 0) {
+    PilAxis down, up;
+    if (pil_axis(h, e, patch_size, &down) || pil_axis(h, patch_size, e, &up)) return 1;
+    pil_resample8_h_kernel<<<grid(mid * n8), 256, 0, st>>>(l_in, l_tmp1, (long long)n8 * e, e, patch_size, down);
+    pil_resample8_v_kernel<<<grid(lr * n8), 256, 0, st>>>(l_tmp1, l_small, n8, e, patch_size, patch_size, down);
+    pil_resample8_h_kernel<<<grid(mid * n8), 256, 0, st>>>(l_small, l_tmp2, (long long)n8 * patch_size, patch_size, e, up);
+    pil_resample8_v_kernel<<<grid(hr * n8), 256, 0, st>>>(l_tmp2, l_big, n8, patch_size, e, e, up);
+    CUDA_TRY(cudaGetLastError());
+    h->launches += 4;
+  }
+  crop_place_kernel<<<grid(lr * n), 256, 0, st>>>(h->crop_jobs.get(), f_small, l_small, h->io_x.get(), n, patch_size, patch_size, scale);
+  crop_place_kernel<<<grid(hr * n), 256, 0, st>>>(h->crop_jobs.get(), f_big, l_big, h->io_x2.get(), n, e, e, scale);
+  CUDA_TRY(cudaGetLastError());
+  h->launches += 2;
+  return 0;
+}
+
+int dcscn_train_step_crops(dcscn_handle* h, const int32_t* crops, int n, int patch_size, float max_value, float lr, uint32_t seed,
+                           int apply_update, float* out_loss, float* out_mse) {
+  if (!h || !crops) return fail("dcscn_train_step_crops: null argument");
+  CUDA_TRY(cudaSetDevice(h->cfg.device_id));
+  cudaStream_t st = 0;
+  if (crop_gather(h, crops, n, patch_size, max_value, st)) return 1;
+  return train_step_impl(h, h->io_x.get(), h->io_x2.get(), h->io_y.get(), n, patch_size, patch_size, lr, seed, apply_update,
+                         out_loss, out_mse, st);
+}
+
+int dcscn_crop_gather(dcscn_handle* h, const int32_t* crops, int n, int patch_size, float max_value, float* x, float* x2, float* y) {
+  if (!h || !crops || !x || !x2 || !y) return fail("dcscn_crop_gather: null argument");
+  CUDA_TRY(cudaSetDevice(h->cfg.device_id));
+  cudaStream_t st = 0;
+  if (crop_gather(h, crops, n, patch_size, max_value, st)) return 1;
+  const size_t lr_px = (size_t)n * patch_size * patch_size, hr_px = lr_px * h->cfg.scale * h->cfg.scale;
   CUDA_TRY(cudaMemcpyAsync(x, h->io_x.get(), lr_px * sizeof(float), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaMemcpyAsync(x2, h->io_x2.get(), hr_px * sizeof(float), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaMemcpyAsync(y, h->io_y.get(), hr_px * sizeof(float), cudaMemcpyDeviceToHost, st));

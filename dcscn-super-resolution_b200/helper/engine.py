@@ -76,7 +76,7 @@ EXPORTED_SYMBOLS = [
     "dcscn_set_adam_step", "dcscn_last_grad_norm",
     "dcscn_patch_store_set", "dcscn_train_step_indexed", "dcscn_patch_gather", "dcscn_dropout_mask", "dcscn_grad_buffer", "dcscn_apply_gradients", "dcscn_apply_gradients_avg", "dcscn_reset_optimizer", "dcscn_graph_replays",
     "dcscn_tile_halo", "dcscn_optimizer_slot_count", "dcscn_get_optimizer_slot", "dcscn_set_optimizer_slot",
-    "dcscn_get_train_tensor",
+    "dcscn_get_train_tensor", "dcscn_image_store_set", "dcscn_train_step_crops", "dcscn_crop_gather",
 ]
 
 _lib = None
@@ -134,6 +134,10 @@ def load_library(path=None):
     lib.dcscn_train_step_indexed.argtypes = [vp, i32p, ci, cf, cf, u32, ci, fp, fp]
     lib.dcscn_patch_gather.argtypes = [vp, i32p, ci, cf, vp, vp, vp]
     lib.dcscn_apply_gradients_avg.argtypes = [vp, cf, cf, fp, fp, vp]
+    c64p = ctypes.POINTER(c64)
+    lib.dcscn_image_store_set.argtypes = [vp, vp, c64, c64p, i32p, i32p, i32p, ci]
+    lib.dcscn_train_step_crops.argtypes = [vp, i32p, ci, ci, cf, cf, u32, ci, fp, fp]
+    lib.dcscn_crop_gather.argtypes = [vp, i32p, ci, ci, cf, vp, vp, vp]
     lib.dcscn_launch_count.argtypes = [vp]
     lib.dcscn_launch_count.restype = c64
     lib.dcscn_device_bytes.argtypes = [vp]
@@ -364,6 +368,51 @@ class Engine:
                                                 x.ctypes.data, x2.ctypes.data, y.ctypes.data))
         return x, x2, y
 
+    # ---- random-crop training data: decoded images resident in HBM ----
+    def set_image_store(self, images):
+        """Decoded uint8 images [h, w, 3] (RGB) or [h, w(, 1)] (mode 'L'), as util.load_image returns them -> device
+        memory, once per data set.  A crop (image, top, left, mirror) of train_step_crops / gather_crops names image i of
+        this list."""
+        arrays = [np.ascontiguousarray(np.atleast_3d(a), dtype=np.uint8) for a in images]
+        shapes = np.array([a.shape for a in arrays], dtype=np.int64).reshape(-1, 3)
+        sizes = np.array([a.size for a in arrays], dtype=np.int64)
+        offsets = np.ascontiguousarray(np.concatenate([[0], np.cumsum(sizes)[:-1]]), dtype=np.int64)
+        pixels = np.concatenate([a.reshape(-1) for a in arrays]) if arrays else np.zeros(0, np.uint8)
+        heights, widths, channels = (np.ascontiguousarray(shapes[:, k], dtype=np.int32) for k in range(3))
+        i32 = ctypes.POINTER(ctypes.c_int32)
+        self._check(self.lib.dcscn_image_store_set(self.handle, pixels.ctypes.data, int(pixels.size),
+                                                   offsets.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)),
+                                                   heights.ctypes.data_as(i32), widths.ctypes.data_as(i32),
+                                                   channels.ctypes.data_as(i32), len(arrays)))
+
+    @staticmethod
+    def _crop_array(crops):
+        c = np.ascontiguousarray(np.asarray(crops, dtype=np.int64).reshape(-1, 4))
+        if c.size and (c.min() < -2 ** 31 or c.max() >= 2 ** 31):
+            raise EngineError("crop descriptor out of the int32 range")
+        return np.ascontiguousarray(c.astype(np.int32))
+
+    def train_step_crops(self, crops, patch_size, lr, seed, max_value=255.0, apply_update=True):
+        """One optimisation step on the crops (image, top, left, mirror) of the device image store, each
+        scale * patch_size pixels square; returns (image_loss, mse)."""
+        c = self._crop_array(crops)
+        loss, mse = ctypes.c_float(), ctypes.c_float()
+        self._check(self.lib.dcscn_train_step_crops(self.handle, c.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), len(c),
+                                                    int(patch_size), float(max_value), float(lr), int(seed) & 0xFFFFFFFF,
+                                                    int(bool(apply_update)), ctypes.byref(loss), ctypes.byref(mse)))
+        return float(loss.value), float(mse.value)
+
+    def gather_crops(self, crops, patch_size, max_value=255.0):
+        """The fp32 mini-batch tensors (x, x2, y) the crop step feeds the network, copied back to the host."""
+        c = self._crop_array(crops)
+        n, p, e = len(c), int(patch_size), int(patch_size) * int(self.config.scale)
+        x = np.empty((n, p, p, 1), np.float32)
+        x2 = np.empty((n, e, e, 1), np.float32)
+        y = np.empty((n, e, e, 1), np.float32)
+        self._check(self.lib.dcscn_crop_gather(self.handle, c.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), n, p,
+                                               float(max_value), x.ctypes.data, x2.ctypes.data, y.ctypes.data))
+        return x, x2, y
+
     def train_step_host(self, x, x2, y, lr, seed, apply_update=True):
         """One optimisation step on host fp32 arrays x [n,h,w,1], x2 / y [n,sh,sw,1]; returns (image_loss, mse)."""
         xa, x2a, ya = _host_array(x), _host_array(x2), _host_array(y)
@@ -413,13 +462,15 @@ class Engine:
                                                        ctypes.byref(mse), ctypes.c_void_p(st)))
         return float(loss.value), float(mse.value)
 
-    def train_step_data_parallel(self, x, x2, y, lr, seed, indices=None, max_value=255.0):
+    def train_step_data_parallel(self, x, x2, y, lr, seed, indices=None, max_value=255.0, crops=None, patch_size=None):
         """One optimisation step with the mini-batch sharded over the ranks of the current torch.distributed job (equal
         shards): local gradients -> ONE flat all-reduce carrying [gradients | loss | mse] -> identical mean, clip and
         Adam on every rank.  Returns the job-wide (image_loss, mse).  With `indices` the rank's shard is taken from the
-        device patch store (x, x2, y ignored)."""
+        device patch store, with `crops` (and `patch_size`) from the device image store (x, x2, y ignored)."""
         import torch.distributed as dist
-        if indices is not None:
+        if crops is not None:
+            loss, mse = self.train_step_crops(crops, patch_size, lr, seed, max_value=max_value, apply_update=False)
+        elif indices is not None:
             loss, mse = self.train_step_indexed(indices, lr, seed, max_value=max_value, apply_update=False)
         else:
             fn = self.train_step if hasattr(x, "is_cuda") and x.is_cuda else self.train_step_host

@@ -11,6 +11,7 @@ import logging
 import random
 
 import numpy as np
+from PIL import Image
 
 from helper import utilty as util
 
@@ -131,12 +132,14 @@ class BatchDataSets(_ShuffledOrder):
 
 
 class DynamicDataSets(_ShuffledOrder):
-    """A random HR crop per request, mirrored left-right half of the time (loader.py:278-355)."""
+    """A random HR crop per request, mirrored left-right half of the time (loader.py:278-355).  A crop is drawn as a
+    descriptor (image, top, left, mirror) by `draw_crop`; `load_batch_image` cuts and resamples it on the host, the engine
+    does the same from its image store (SuperResolution.init_epoch_index / train_batch)."""
 
     def __init__(self, scale, batch_image_size, channels=1, resampling_method="bicubic"):
         self.scale, self.channels, self.resampling_method = scale, channels, resampling_method
         self.batch_image_size = batch_image_size
-        self.filenames, self.batch_index, self.index, self.count = [], None, 0, 0
+        self.filenames, self.sizes, self.batch_index, self.index, self.count = [], [], None, 0, 0
 
     def set_data_dir(self, data_dir):
         self.filenames = util.get_files_in_directory(data_dir)
@@ -144,28 +147,39 @@ class DynamicDataSets(_ShuffledOrder):
         if self.count <= 0:
             logging.error("Data Directory is empty.")
             exit(-1)
+        self.sizes = []
+        for filename in self.filenames:            # PIL reads the header only; pixels are decoded on demand
+            with Image.open(filename) as im:
+                self.sizes.append((im.height, im.width))
 
     def init_batch_index(self, shuffle=True):
         super().init_batch_index(True)
 
-    def load_random_patch(self, filename):
-        """loader.py:332-355: None when the image is smaller than one HR patch."""
-        image = util.load_image(filename, print_console=False)
+    def draw_crop(self):
+        """(image number, top, left, mirror) of the next patch, drawing from `random` exactly as the reference's
+        load_batch_image / load_random_patch do (loader.py:310-355); images smaller than one HR patch are skipped."""
         edge = self.batch_image_size * self.scale
-        rows, cols = image.shape[:2]
-        if rows < edge or cols < edge:
-            print("Error: %s should have more than %d x %d size." % (filename, edge, edge))
-            return None
-        top = random.randrange(rows - edge) if rows > edge else 0
-        left = random.randrange(cols - edge) if cols > edge else 0
-        return build_input_image(image[top:top + edge, left:left + edge, :], channels=self.channels, convert_ycbcr=True)
+        while True:
+            number = self.get_next_image_no()
+            rows, cols = self.sizes[number]
+            if rows < edge or cols < edge:
+                print("Error: %s should have more than %d x %d size." % (self.filenames[number], edge, edge))
+                continue
+            top = random.randrange(rows - edge) if rows > edge else 0
+            left = random.randrange(cols - edge) if cols > edge else 0
+            return number, top, left, int(random.randrange(2) == 0)
+
+    def decoded_images(self):
+        """Every image of the set decoded once (util.load_image), in image-number order: the engine's image store."""
+        return [util.load_image(filename, print_console=False) for filename in self.filenames]
 
     def load_batch_image(self, max_value):
         """loader.py:310-330"""
-        truth = None
-        while truth is None:
-            truth = self.load_random_patch(self.filenames[self.get_next_image_no()])
-        if random.randrange(2) == 0:
+        number, top, left, mirror = self.draw_crop()
+        edge = self.batch_image_size * self.scale
+        image = util.load_image(self.filenames[number], print_console=False)
+        truth = build_input_image(image[top:top + edge, left:left + edge, :], channels=self.channels, convert_ycbcr=True)
+        if mirror:
             truth = np.fliplr(truth)
         small = util.resize_image_by_pil(truth, 1 / self.scale)
         return _rescaled((small, util.resize_image_by_pil(small, self.scale), truth), max_value)

@@ -76,3 +76,34 @@ def resize_float(image, out_width, out_height):
             acc = acc + tmp[y0 + y, :].astype(np.float64) * ky[yy, y]
         out[yy, :] = acc.astype(np.float32)
     return out
+
+
+def _coeffs_8bpc(kk):
+    """Pillow's normalize_coeffs_8bpc: the double weights as 22-bit fixed point, rounded half away from zero."""
+    scaled = kk * (1 << 22)
+    return np.where(kk < 0, np.trunc(scaled - 0.5), np.trunc(scaled + 0.5)).astype(np.int64)
+
+
+def _clip8(ss):
+    return np.clip(ss >> 22, 0, 255).astype(np.uint8)
+
+
+def resize_uint8(image, out_width, out_height):
+    """Pillow's `Image.fromarray(image).resize([out_width, out_height], Image.BICUBIC)` for a 2-D uint8 array (mode 'L',
+    ImagingResampleHorizontal_8bpc / ImagingResampleVertical_8bpc): the same tables as `resize_float` in 22-bit fixed
+    point, an int32 sum that starts at 2^21, clamp(sum >> 22, 0, 255), and a uint8 image between the two passes.  The
+    device kernels `pil_resample8_h/v_kernel` (csrc/conv_aux.cuh) apply it to the mode-'L' crops of a mini-batch."""
+    img = np.asarray(image, dtype=np.uint8).astype(np.int64)
+    h, w = img.shape
+    kx, bx = precompute_coeffs(w, out_width)
+    ky, by = precompute_coeffs(h, out_height)
+    kx, ky = _coeffs_8bpc(kx), _coeffs_8bpc(ky)
+    tmp = np.empty((h, out_width), dtype=np.int64)
+    for xx in range(out_width):
+        x0, n = bx[xx]
+        tmp[:, xx] = _clip8((1 << 21) + img[:, x0:x0 + n] @ kx[xx, :n])
+    out = np.empty((out_height, out_width), dtype=np.uint8)
+    for yy in range(out_height):
+        y0, n = by[yy]
+        out[yy, :] = _clip8((1 << 21) + ky[yy, :n] @ tmp[y0:y0 + n, :])
+    return out

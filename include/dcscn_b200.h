@@ -170,6 +170,25 @@ int dcscn_patch_store_set(dcscn_handle* h, const uint8_t* lr, const uint8_t* bic
 int dcscn_train_step_indexed(dcscn_handle* h, const int32_t* indices, int n, float max_value, float lr, uint32_t seed,
                              int apply_update, float* out_loss, float* out_mse);
 int dcscn_patch_gather(dcscn_handle* h, const int32_t* indices, int n, float max_value, float* x, float* x2, float* y);
+/*
+ * Random-crop training data on the device (reference: helper/loader.py:278-355 DynamicDataSets, the data set of train.py
+ * without --build_batch, which decodes, crops, converts and resizes every patch of every step in Python).
+ * dcscn_image_store_set copies the decoded uint8 images (what util.load_image returns: RGB, 3 interleaved channels, or
+ * mode 'L', 1 channel; image i is heights[i] x widths[i] x channels[i] bytes at offsets[i] of `pixels`) into HBM once;
+ * it replaces the previous image store and nothing else.  dcscn_train_step_crops is dcscn_train_step on the mini-batch of
+ * `n` crop descriptors crops[4 * i ..] = (image, top, left, mirror) (loader.py:332-355 load_random_patch + the mirror of
+ * loader.py:318-319): an e x e crop, e = scale * patch_size, at row `top` and column `left`, mirrored left-right when
+ * mirror = 1.  Per crop the device forms what load_batch_image returns, bit for bit: the truth y = Y (float64 RGB -> Y,
+ * util.convert_rgb_to_y) or the 'L' sample, x = Pillow bicubic of y down by 1 / scale (mode 'F' for Y, Pillow's 8-bit
+ * path for 'L'), x2 = x up by scale, each multiplied by max_value / 255 under numpy's dtype rules (loader.py:323-327).
+ * Every descriptor is checked before any launch: image in range, 0 <= top <= height - e, 0 <= left <= width - e,
+ * mirror 0 or 1.  dcscn_crop_gather returns the same fp32 tensors x [n, ps, ps], x2 / y [n, e, e] to the host.
+ */
+int dcscn_image_store_set(dcscn_handle* h, const uint8_t* pixels, int64_t bytes, const int64_t* offsets, const int32_t* heights,
+                          const int32_t* widths, const int32_t* channels, int count);
+int dcscn_train_step_crops(dcscn_handle* h, const int32_t* crops, int n, int patch_size, float max_value, float lr, uint32_t seed,
+                           int apply_update, float* out_loss, float* out_mse);
+int dcscn_crop_gather(dcscn_handle* h, const int32_t* crops, int n, int patch_size, float max_value, float* x, float* x2, float* y);
 /* d loss / d variable of the LAST train step (after the L2 term, before clipping): tf.gradients(loss, trainables). */
 int dcscn_get_grad(dcscn_handle* h, const char* name, float* host_data, int64_t numel);
 /* Adam slots of a variable ("<var>/Adam" = slot 0, "<var>/Adam_1" = slot 1 in the reference's checkpoints).  Fail for
