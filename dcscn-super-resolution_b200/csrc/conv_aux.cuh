@@ -397,6 +397,70 @@ __global__ void __launch_bounds__(128) conv_ref_kernel(const ConvRefParams p) {
   }
 }
 
+// ------------------------------------------------- depthwise step of wide depthwise-separable graphs -----------
+// The depthwise half of tf.nn.separable_conv2d (helper/tf_graph.py:155-216) for graphs too wide for ds_tile_kernel:
+// u[c] = sum over the k x k taps of x[c] dw[tap][c] (SAME zero padding, no bias), read from and written to fp16 hi/lo
+// planes, so that the pointwise half, bias and activation run as a 1x1 layer of conv_tc_kernel over u.  fp32 FMAs in
+// tap order, one thread per pixel and 8 channel positions (16-byte loads and stores).
+struct DwParams {
+  int n_img, H, W;           // resolution of the layer's input (= output)
+  int ksz;                   // 3 or 5; 0 = the layer has no depthwise step
+  int cpad;                  // channel positions of the source region (a multiple of 16), also u's pitch
+  const __half* src_hi;      // source planes, offset to the region's first position
+  const __half* src_lo;      // null in f16x1
+  int src_pitch;
+  const float* dw;           // [k*k][cpad] fp32, zero at positions no channel maps to
+  __half* u_hi;              // [px][cpad]
+  __half* u_lo;              // null in f16x1
+};
+
+template <int K>
+__global__ void __launch_bounds__(256) depthwise_planes_kernel(const DwParams p) {
+  constexpr int half = K / 2;
+  const int groups = p.cpad >> 3;
+  const long long total = (long long)p.n_img * p.H * p.W * groups;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int c0 = (int)(i % groups) * 8;
+    const long long pix = i / groups;
+    const int x = (int)(pix % p.W);
+    const int y = (int)((pix / p.W) % p.H);
+    const long long img0 = pix - (long long)y * p.W - x;   // first pixel of this image
+    float acc[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[j] = 0.f;
+#pragma unroll
+    for (int ty = 0; ty < K; ++ty) {
+      const int yy = y + ty - half;
+      if (yy < 0 || yy >= p.H) continue;
+#pragma unroll
+      for (int tx = 0; tx < K; ++tx) {
+        const int xx = x + tx - half;
+        if (xx < 0 || xx >= p.W) continue;
+        const size_t off = (size_t)(img0 + (long long)yy * p.W + xx) * p.src_pitch + c0;
+        const uint4 hq = __ldg(reinterpret_cast<const uint4*>(p.src_hi + off));
+        const uint4 lq = p.src_lo != nullptr ? __ldg(reinterpret_cast<const uint4*>(p.src_lo + off)) : make_uint4(0, 0, 0, 0);
+        const __half2* h2 = reinterpret_cast<const __half2*>(&hq);
+        const __half2* l2 = reinterpret_cast<const __half2*>(&lq);
+        const float4* w4 = reinterpret_cast<const float4*>(p.dw + (size_t)(ty * K + tx) * p.cpad + c0);
+        const float4 wa = __ldg(w4), wb = __ldg(w4 + 1);
+        const float w[8] = {wa.x, wa.y, wa.z, wa.w, wb.x, wb.y, wb.z, wb.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float2 hv = __half22float2(h2[j]), lv = __half22float2(l2[j]);
+          acc[2 * j] = fmaf(hv.x + lv.x, w[2 * j], acc[2 * j]);
+          acc[2 * j + 1] = fmaf(hv.y + lv.y, w[2 * j + 1], acc[2 * j + 1]);
+        }
+      }
+    }
+    uint32_t ph[4], pl[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) split_f16x2(acc[2 * j], acc[2 * j + 1], ph[j], pl[j]);
+    const size_t o = (size_t)pix * p.cpad + c0;
+    *reinterpret_cast<uint4*>(p.u_hi + o) = make_uint4(ph[0], ph[1], ph[2], ph[3]);
+    if (p.u_lo != nullptr) *reinterpret_cast<uint4*>(p.u_lo + o) = make_uint4(pl[0], pl[1], pl[2], pl[3]);
+  }
+}
+
 // ---------------------------------------------------------------- helpers ----------------------------------
 __global__ void planes_to_f32_kernel(const __half* hi, const __half* lo, float* out, size_t n) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {

@@ -153,6 +153,10 @@ struct TcLayer {
   DeviceArray<int> d_in_map;
   int packed_planes = 0;
   DeviceArray<int> d_img_map;   // training: flat parameter index behind every hi-plane element of d_wpack (-1 = zero)
+  // wide depthwise-separable graphs: the k x k depthwise step that runs in front of this 1x1 pointwise layer
+  int dw_ksz = 0;               // 0 = none
+  std::vector<float> dw_host;   // [taps][cin_pad] by source position, zero where no channel maps
+  DeviceArray<float> d_dw;
 };
 
 struct GatherJob {   // training: dst[i] = d_w[map[i]] where map[i] >= 0 (biases, PReLU slopes, CNN1 / R-CNN1 filters)
@@ -176,6 +180,8 @@ struct Plan {
   int n = 0, h = 0, w = 0;
   ConvFirstParams first;
   std::vector<TcLaunch> tc;      // in execution order
+  std::vector<DwParams> dw;      // depthwise step in front of tc[i] (ksz 0: none; wide depthwise-separable graphs)
+  int dw_count = 0;              // depthwise launches per forward
   ConvLastParams last;
   bool fused_last = false;       // Up-PS epilogue computes the per-pixel half of R-CNN1 (EPI_D2S_RDOT)
   int fused_index = -1;          // index into tc of the launch that carries the fused epilogue
@@ -238,6 +244,7 @@ struct dcscn_handle {
   DeviceArray<__half> b1_hi, b1_lo;
   DeviceArray<__half> nin_hi, nin_lo;
   DeviceArray<__half> mid_hi, mid_lo;
+  DeviceArray<__half> u_hi, u_lo;    // wide depthwise-separable graphs: a layer's depthwise output, read by its pointwise
   DeviceArray<float> hr;
   DeviceArray<float> vbuf;           // tap-planar partial products of the fused R-CNN1 [9][N][sH][sW]
   DeviceArray<float> io_x, io_x2, io_y;  // staging for forward_host
@@ -269,7 +276,12 @@ struct dcscn_handle {
   bool tiled_last = false;           // the last forward ran tiled: the activation buffers hold its last batch
   int tiled_batches = 0;             // batches of the last tiled forward (timing names)
 
-  // depthwise-separable graphs: fp32 buffers + per-layer device filters
+  // Depthwise-separable graphs run one of two ways, chosen from the graph's shape alone (ds_tile_fits):
+  //   * ds_wide = false: every layer on the fp32 CUDA-core kernels of conv_ds_tile.cuh, in the ds_* buffers below;
+  //   * ds_wide = true: the tensor-core graph's buffers, plans and kernels, each k x k separable layer as
+  //     depthwise_planes_kernel followed by a 1x1 conv_tc_kernel layer (see construct_tc_layers).
+  bool ds_wide = false;
+  // depthwise-separable graphs on the CUDA-core kernels: fp32 buffers + per-layer device filters
   struct DsDev { DeviceArray<float> dw, pw, bias, alpha; };
   std::vector<DsDev> ds;             // same order as `layers`
   DsDev ds_ab;                       // fused A1 | B1 1x1 layer of the tile kernels: [concat positions][A1 cols | B1 cols], scales folded
@@ -298,6 +310,9 @@ struct dcscn_handle {
 };
 
 static int planes(const dcscn_handle* h) { return h->cfg.precision == DCSCN_PRECISION_F16X1 ? 1 : 2; }
+
+// A depthwise-separable graph whose layers all run on the fp32 CUDA-core kernels (forward_ds_tile).
+static bool uses_ds_tile(const dcscn_handle* h) { return h->cfg.depthwise_separable && !h->ds_wide; }
 
 // Filter-count schedule of the feature-extraction stack (DCSCN.py:240-244).
 static std::vector<int> feature_filters(const dcscn_config& c) {
@@ -345,6 +360,37 @@ static void layer_slopes(const dcscn_handle* h, const LayerDef& l, float* dst) {
     const std::vector<float>& A = P(h, prelu_name(l.scope));
     std::copy(A.begin(), A.begin() + l.cout, dst);
   }
+}
+
+// Shared memory launch_ds_tile gives ds_tile_kernel for a layer (the template's column count sizes the carve-up).
+static size_t ds_tile_launch_smem(int ksz, int cin, int cout) {
+  const int cols = cout < 32 ? ((cout + 3) & ~3) : 32;
+  const int tcols = cols <= 4 ? 4 : cols <= 8 ? 8 : cols <= 16 ? 16 : cols <= 24 ? 24 : 32;
+  const size_t in_px = ksz == 3 ? (size_t)(kDtT + 2) * kDtS : (size_t)kDtThreads;
+  const size_t cache = ds_tile_caches_depthwise(ksz, cin, cout) ? (size_t)kDtThreads * kDtCP : 0;   // private depthwise rows
+  return (in_px * kDtCP + (size_t)cin * tcols + (size_t)ksz * ksz * cin + cache) * sizeof(float);
+}
+static bool ds_tile_accepts(int ksz, int cin, int cout) {
+  return (ksz == 1 || ksz == 3) && !(cout > 32 && cin > kDtCC) && ds_tile_launch_smem(ksz, cin, cout) <= 200 * 1024;
+}
+
+// Whether forward_ds_tile runs every layer of the depthwise-separable graph: the one statement of the choice between
+// the fp32 CUDA-core kernels and the wide path (dcscn_handle::ds_wide).
+static bool ds_tile_fits(const dcscn_handle* h) {
+  const dcscn_config& c = h->cfg;
+  int T = 0;   // concat channels with 4-aligned slots (finalize_params_ds)
+  for (int f : h->filters) T += (f + 3) & ~3;
+  const int cps = c.nin_filters + c.nin_filters2;
+  if (cps > 32 || !ds_tile_accepts(1, T, cps)) return false;   // the fused A1 | B1 launch
+  for (const LayerDef& l : h->layers) {
+    if (l.scope == "A1" || l.scope == "B1") continue;
+    if (l.cin == 1 && l.cout == 1) {                              // R-CNN1 on ds_single(4)_kernel
+      if (l.k != 1 && l.k != 3) return false;
+    } else if (!ds_tile_accepts(l.k, l.cin, l.cout)) {
+      return false;
+    }
+  }
+  return true;
 }
 
 static int build_graph(dcscn_handle* h) {
@@ -402,6 +448,7 @@ static int build_graph(dcscn_handle* h) {
   h->a1_w = pad16(c.nin_filters);
   h->nin_pitch = h->b1_w + h->a1_w;  // [B2 | A1]  (Concat2 order, DCSCN.py:281)
   h->mid_pitch = pad16(cin);
+  h->ds_wide = c.depthwise_separable && !ds_tile_fits(h);
   return 0;
 }
 
@@ -416,11 +463,50 @@ static const std::vector<float>& P(const dcscn_handle* h, const std::string& nam
 }
 
 // ------------------------------------------------------------------------------ weight packing ----
-// Appends the TF layer `scope` as columns [col0, col0+cout) of a fused tensor-core layer.
+// Whether a layer of a wide depthwise-separable graph runs as depthwise_planes_kernel + a 1x1 pointwise layer.  The
+// other layers fold their depthwise filter into a dense one (layer_filter): 1x1 layers (a per-channel scale), CNN1
+// (one input channel) and R-CNN1 (one output channel).
+// Once a handle trains, every layer is composed instead: the dense train step differentiates the composed k x k filters.
+static bool ds_split(const dcscn_handle* h, const LayerDef& l) {
+  return h->ds_wide && !h->train_enabled && l.k > 1 && l.cin > 1 && l.cout > 1;
+}
+
+// The HWIO filter the packed form of layer `l` computes with: conv_W; on the wide depthwise-separable path the pointwise
+// filter alone for a split layer, else W[t][ci][co] = dw[t][ci] pw[ci][co] in `tmp` (exact in real arithmetic: one
+// side of the product has a single channel or a single tap).
+static const std::vector<float>& layer_filter(const dcscn_handle* h, const LayerDef& l, std::vector<float>& tmp) {
+  // shadow mode (build_refresh_maps): a composed filter lives in the layer's conv_W slot of TrainState::d_wc
+  if (!h->ds_wide || h->shadow_mode) return P(h, l.scope + "/conv_W");
+  const std::vector<float>& pw = P(h, l.scope + "/pointwise_W");
+  if (ds_split(h, l)) return pw;
+  const std::vector<float>& dw = P(h, l.scope + "/depthwise_W");
+  const int taps = l.k * l.k;
+  tmp.assign((size_t)taps * l.cin * l.cout, 0.f);
+  for (int tp = 0; tp < taps; ++tp)
+    for (int ci = 0; ci < l.cin; ++ci)
+      for (int co = 0; co < l.cout; ++co)
+        tmp[((size_t)tp * l.cin + ci) * l.cout + co] = dw[(size_t)tp * l.cin + ci] * pw[(size_t)ci * l.cout + co];
+  return tmp;
+}
+
+// Filter size of the tensor-core layer that computes `l`.
+static int tc_ksz(const dcscn_handle* h, const LayerDef& l) { return ds_split(h, l) ? 1 : l.k; }
+
+// Appends the TF layer `scope` as columns [col0, col0+cout) of a fused tensor-core layer (t.in_map set).  A split layer
+// of a wide depthwise-separable graph also gets its depthwise filter, by source position.
 static void fuse_columns(const dcscn_handle* h, TcLayer& t, const std::string& scope, int col0, int n_total_pad) {
   const LayerDef* l = find_layer(h, scope);
-  const std::vector<float>& W = P(h, scope + "/conv_W");
-  const int taps = l->k * l->k;
+  std::vector<float> tmp;
+  const std::vector<float>& W = layer_filter(h, *l, tmp);
+  const int taps = t.ksz * t.ksz;
+  if (ds_split(h, *l)) {
+    const std::vector<float>& D = P(h, scope + "/depthwise_W");
+    const int dtaps = l->k * l->k;
+    t.dw_ksz = l->k;
+    t.dw_host.assign((size_t)dtaps * t.cin_pad, 0.f);
+    for (int tp = 0; tp < dtaps; ++tp)
+      for (int ci = 0; ci < l->cin; ++ci) t.dw_host[(size_t)tp * t.cin_pad + t.in_map[ci]] = D[(size_t)tp * l->cin + ci];
+  }
   for (int tp = 0; tp < taps; ++tp)
     for (int ci = 0; ci < l->cin; ++ci)
       for (int co = 0; co < l->cout; ++co)
@@ -489,7 +575,7 @@ static int pack_tc_layer(dcscn_handle* h, TcLayer& t, bool* moved) {
     if (NPL == 2) pack[blk * NPL * tile_elems + tile_elems + pos] = __float2half_rn(v - __half2float(hi));
   }
   if (t.d_wpack.upload(pack, moved) || t.d_bias.upload(t.bias_host, moved) || t.d_alpha.upload(t.alpha_host, moved) ||
-      t.d_wref.upload(t.w_host, moved) || t.d_in_map.upload(t.in_map, moved))
+      t.d_wref.upload(t.w_host, moved) || t.d_in_map.upload(t.in_map, moved) || t.d_dw.upload(t.dw_host, moved))
     return 1;
   t.packed_planes = NPL;
   return 0;
@@ -597,7 +683,8 @@ static void first_layer_vectors(const dcscn_handle* h, std::vector<float>& w, st
   w.assign((size_t)taps * np, 0.f);
   b.assign(np, 0.f);
   a.assign(np, 1.f);
-  const auto& W = P(h, "CNN1/conv_W");
+  std::vector<float> tmp;
+  const std::vector<float>& W = layer_filter(h, *l, tmp);
   for (int tp = 0; tp < taps; ++tp)
     for (int co = 0; co < l->cout; ++co) w[(size_t)tp * np + co] = W[(size_t)tp * l->cout + co];
   const auto& B = P(h, "CNN1/conv_B");
@@ -613,7 +700,7 @@ static int construct_tc_layers(dcscn_handle* h) {
   for (int i = 1; i < L; ++i) {
     const std::string scope = "CNN" + std::to_string(i + 1);
     const LayerDef* l = find_layer(h, scope);
-    TcLayer t = make_tc(scope, l->k, l->cin, l->cout, h->feat_w[i - 1]);
+    TcLayer t = make_tc(scope, tc_ksz(h, *l), l->cin, l->cout, h->feat_w[i - 1]);
     for (int ci = 0; ci < l->cin; ++ci) t.in_map.push_back(ci);
     fuse_columns(h, t, scope, 0, 0);
     h->tcl.push_back(std::move(t));
@@ -632,7 +719,7 @@ static int construct_tc_layers(dcscn_handle* h) {
   // B2
   {
     const LayerDef* l = find_layer(h, "B2");
-    TcLayer t = make_tc("B2", l->k, l->cin, l->cout, h->b1_w);
+    TcLayer t = make_tc("B2", tc_ksz(h, *l), l->cin, l->cout, h->b1_w);
     for (int ci = 0; ci < l->cin; ++ci) t.in_map.push_back(ci);
     fuse_columns(h, t, "B2", 0, 0);
     h->tcl.push_back(std::move(t));
@@ -642,27 +729,28 @@ static int construct_tc_layers(dcscn_handle* h) {
     const LayerDef* l = find_layer(h, "Up-PS/Up-PS_CNN");
     // the LAST depth_to_space layer carries the fused R-CNN1 epilogue (3x3 R-CNN1 only)
     const int fuse_unit = find_layer(h, "R-CNN1")->k == 3 ? h->ps_out : 0;
-    TcLayer t = make_tc("Up-PS", l->k, l->cin, l->cout, h->nin_pitch, c.scale == 4 ? 0 : fuse_unit);
+    TcLayer t = make_tc("Up-PS", tc_ksz(h, *l), l->cin, l->cout, h->nin_pitch, c.scale == 4 ? 0 : fuse_unit);
     for (int ci = 0; ci < c.nin_filters2; ++ci) t.in_map.push_back(ci);
     for (int ci = 0; ci < c.nin_filters; ++ci) t.in_map.push_back(h->b1_w + ci);
     fuse_columns(h, t, "Up-PS/Up-PS_CNN", 0, 0);
     h->tcl.push_back(std::move(t));
     if (c.scale == 4) {
       const LayerDef* l2 = find_layer(h, "Up-PS2/Up-PS2_CNN");
-      TcLayer t2 = make_tc("Up-PS2", l2->k, l2->cin, l2->cout, h->mid_pitch, fuse_unit);
+      TcLayer t2 = make_tc("Up-PS2", tc_ksz(h, *l2), l2->cin, l2->cout, h->mid_pitch, fuse_unit);
       for (int ci = 0; ci < l2->cin; ++ci) t2.in_map.push_back(ci);
       fuse_columns(h, t2, "Up-PS2/Up-PS2_CNN", 0, 0);
       h->tcl.push_back(std::move(t2));
     }
   }
-  if (h->train_enabled && build_bwd_layers(h)) return 1;
+  // forward_ds_tile graphs train on the fp32 step of train_ds.inc, which needs no dgrad twins
+  if (h->train_enabled && !uses_ds_tile(h) && build_bwd_layers(h)) return 1;
   return 0;
 }
 
 static int finalize_params(dcscn_handle* h) {
   const dcscn_config& c = h->cfg;
   if (sync_host_params(h)) return 1;
-  if (c.depthwise_separable) return finalize_params_ds(h);
+  if (uses_ds_tile(h)) return finalize_params_ds(h);
   std::vector<TcLayer> old_tcl = std::move(h->tcl);
   std::vector<TcLayer> old_bwd = std::move(h->bwd);
   h->tcl.clear();
@@ -683,6 +771,7 @@ static int finalize_params(dcscn_handle* h) {
       if (i < old.size()) {
         t.d_wpack = std::move(old[i].d_wpack); t.d_bias = std::move(old[i].d_bias); t.d_alpha = std::move(old[i].d_alpha);
         t.d_wref = std::move(old[i].d_wref); t.d_in_map = std::move(old[i].d_in_map); t.d_img_map = std::move(old[i].d_img_map);
+        t.d_dw = std::move(old[i].d_dw);
       }
       if (pack_tc_layer(h, t, &moved)) return 1;
     }
@@ -690,7 +779,10 @@ static int finalize_params(dcscn_handle* h) {
   };
   if (repack(h->tcl, old_tcl) || repack(h->bwd, old_bwd)) return 1;
   // R-CNN1 (CUDA cores): [taps][C]
-  if (h->d_last_w.upload(P(h, "R-CNN1/conv_W"), &moved)) return 1;
+  {
+    std::vector<float> tmp;
+    if (h->d_last_w.upload(layer_filter(h, *find_layer(h, "R-CNN1"), tmp), &moved)) return 1;
+  }
   if (moved) {  // some device pointer moved: cached plans embed stale pointers
     h->plans.clear();
     h->last_plan = nullptr;
@@ -712,11 +804,12 @@ static int rdot_parts(int n_pad, int cout) {
 // Elements per LR pixel of every buffer ensure_workspace allocates: the one statement of their sizes, shared by the
 // allocation and by the tile planner's workspace budget (valid once the parameters are finalised).
 struct WorkspaceShape {
-  size_t feat, b1, nin, mid;   // fp16 elements per plane (tensor-core graphs) or fp32 (depthwise-separable graphs)
+  size_t feat, b1, nin, mid;   // fp16 elements per plane (tensor-core graphs) or fp32 (forward_ds_tile)
+  size_t u;                    // fp16 elements per plane: the widest depthwise output of a wide depthwise-separable graph
   size_t hr, vbuf;             // fp32
   int planes;                  // fp16 planes (tensor-core graphs)
   size_t bytes_per_px(bool ds) const {
-    return ds ? 4 * (feat + b1 + nin + mid + hr) : 2 * (size_t)planes * (feat + b1 + nin + mid) + 4 * (hr + vbuf);
+    return ds ? 4 * (feat + b1 + nin + mid + hr) : 2 * (size_t)planes * (feat + b1 + nin + mid + u) + 4 * (hr + vbuf);
   }
 };
 
@@ -724,7 +817,8 @@ static WorkspaceShape workspace_shape(const dcscn_handle* h) {
   const dcscn_config& c = h->cfg;
   const size_t s2 = (size_t)c.scale * c.scale;
   WorkspaceShape w;
-  if (c.depthwise_separable) {
+  w.u = 0;
+  if (uses_ds_tile(h)) {
     const int cps = c.nin_filters + c.nin_filters2;
     w.feat = h->ds_total;
     w.b1 = c.nin_filters2;
@@ -742,6 +836,15 @@ static WorkspaceShape workspace_shape(const dcscn_handle* h) {
   w.hr = s2 * h->ps_out;
   w.vbuf = s2 * 9 * (size_t)rdot_parts(h->tcl.empty() ? 16 : h->tcl.back().n_pad, h->ps_out);
   w.planes = planes(h);
+  if (h->ds_wide) {   // u of a split layer has its source region's pitch; Up-PS2 runs at 2x the LR resolution
+    for (const LayerDef& l : h->layers) {
+      if (!ds_split(h, l)) continue;
+      const std::string& sc = l.scope;
+      const size_t per_px = sc == "B2" ? w.b1 : sc == "Up-PS/Up-PS_CNN" ? w.nin : sc == "Up-PS2/Up-PS2_CNN" ? w.mid
+                                                                          : (size_t)pad16(l.cin);
+      w.u = std::max(w.u, per_px);
+    }
+  }
   return w;
 }
 
@@ -749,7 +852,7 @@ static int ensure_workspace(dcscn_handle* h, size_t lr_px) {
   if (lr_px <= h->cap_px) return 0;
   const dcscn_config& c = h->cfg;
   const WorkspaceShape ws = workspace_shape(h);
-  if (c.depthwise_separable) {
+  if (uses_ds_tile(h)) {
     if (h->ds_feat.alloc(lr_px * ws.feat, true)) return 1;   // pad channels must stay zero
     if (h->ds_b1.alloc(lr_px * ws.b1) || h->ds_nin.alloc(lr_px * ws.nin)) return 1;
     if (c.scale == 4 && h->ds_mid.alloc(lr_px * ws.mid)) return 1;
@@ -766,6 +869,7 @@ static int ensure_workspace(dcscn_handle* h, size_t lr_px) {
   if (c.scale == 4) {
     if (h->mid_hi.alloc(lr_px * ws.mid, true) || h->mid_lo.alloc(two ? lr_px * ws.mid : 0, true)) return 1;
   }
+  if (h->u_hi.alloc(lr_px * ws.u, true) || h->u_lo.alloc(two ? lr_px * ws.u : 0, true)) return 1;
   if (h->hr.alloc(lr_px * ws.hr, true) || h->vbuf.alloc(lr_px * ws.vbuf, true)) return 1;
   h->cap_px = lr_px;
   return 0;
@@ -774,7 +878,7 @@ static int ensure_workspace(dcscn_handle* h, size_t lr_px) {
 // Device bytes of the activation workspace and the tiled-inference staging buffers (dcscn_device_bytes).
 static int64_t workspace_bytes(const dcscn_handle* h) {
   auto bytes = [](const auto&... a) { return (int64_t)(0 + ... + (a.size() * sizeof(*a.get()))); };
-  return bytes(h->feat_hi, h->feat_lo, h->b1_hi, h->b1_lo, h->nin_hi, h->nin_lo, h->mid_hi, h->mid_lo, h->hr, h->vbuf,
+  return bytes(h->feat_hi, h->feat_lo, h->b1_hi, h->b1_lo, h->nin_hi, h->nin_lo, h->mid_hi, h->mid_lo, h->u_hi, h->u_lo, h->hr, h->vbuf,
                h->ds_feat, h->ds_b1, h->ds_nin, h->ds_mid, h->ds_hr, h->tile_x, h->tile_x2, h->tile_y);
 }
 
@@ -910,6 +1014,23 @@ static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, const __ha
   return 0;
 }
 
+// A forward layer: its depthwise step when it has one (the 1x1 pointwise then reads u instead of the source), then
+// its tensor-core launch.  pl->dw stays parallel to pl->tc.
+static int add_layer_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, const __half* src_hi, const __half* src_lo,
+                            int src_pitch, int n, int H, int W, const EpiParams& epi) {
+  DwParams d;
+  memset(&d, 0, sizeof(d));
+  if (t.dw_ksz) {
+    d = DwParams{n, H, W, t.dw_ksz, t.cin_pad, src_hi, src_lo, src_pitch, t.d_dw.get(), h->u_hi.get(), planes(h) == 2 ? h->u_lo.get() : nullptr};
+    src_hi = d.u_hi;
+    src_lo = d.u_lo;
+    src_pitch = t.cin_pad;
+    pl->dw_count++;
+  }
+  pl->dw.push_back(d);
+  return add_tc_launch(h, pl, t, src_hi, src_lo, src_pitch, n, H, W, epi);
+}
+
 static EpiParams epi_planes(__half* hi, __half* lo, int pitch, int col_begin, int col_end) {
   EpiParams e;
   memset(&e, 0, sizeof(e));
@@ -948,7 +1069,7 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
   for (int i = 1; i < c.layers; ++i, ++ti) {
     EpiParams e = epi_planes(h->feat_hi.get() + h->feat_off[i], lo(h->feat_lo.get(), h->feat_off[i]), h->feat_pitch, 0, h->feat_w[i]);
     e.act = c.activator;
-    if (add_tc_launch(h, pl.get(), h->tcl[ti], h->feat_hi.get() + h->feat_off[i - 1], lo(h->feat_lo.get(), h->feat_off[i - 1]),
+    if (add_layer_launch(h, pl.get(), h->tcl[ti], h->feat_hi.get() + h->feat_off[i - 1], lo(h->feat_lo.get(), h->feat_off[i - 1]),
                       h->feat_pitch, n, H, W, e))
       return nullptr;
   }
@@ -957,12 +1078,12 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
     e.num_seg = 2;
     e.seg[1] = {h->a1_w, h->a1_w + h->b1_w, h->b1_hi.get(), two ? h->b1_lo.get() : nullptr, h->b1_w};
     e.act = c.activator;
-    if (add_tc_launch(h, pl.get(), h->tcl[ti++], h->feat_hi.get(), lo(h->feat_lo.get(), 0), h->feat_pitch, n, H, W, e)) return nullptr;
+    if (add_layer_launch(h, pl.get(), h->tcl[ti++], h->feat_hi.get(), lo(h->feat_lo.get(), 0), h->feat_pitch, n, H, W, e)) return nullptr;
   }
   {  // B2 -> nin[:, 0:b1_w]
     EpiParams e = epi_planes(h->nin_hi.get(), lo(h->nin_lo.get(), 0), h->nin_pitch, 0, h->b1_w);
     e.act = c.activator;
-    if (add_tc_launch(h, pl.get(), h->tcl[ti++], h->b1_hi.get(), two ? h->b1_lo.get() : nullptr, h->b1_w, n, H, W, e)) return nullptr;
+    if (add_layer_launch(h, pl.get(), h->tcl[ti++], h->b1_hi.get(), two ? h->b1_lo.get() : nullptr, h->b1_w, n, H, W, e)) return nullptr;
   }
   int HR_H = H, HR_W = W;
   {  // Up-PS
@@ -982,7 +1103,7 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
       e.dst_f32 = h->hr.get();
       e.d2s_pitch = h->ps_out;
     }
-    if (add_tc_launch(h, pl.get(), h->tcl[ti++], h->nin_hi.get(), two ? h->nin_lo.get() : nullptr, h->nin_pitch, n, H, W, e)) return nullptr;
+    if (add_layer_launch(h, pl.get(), h->tcl[ti++], h->nin_hi.get(), two ? h->nin_lo.get() : nullptr, h->nin_pitch, n, H, W, e)) return nullptr;
     HR_H = H * (c.scale == 4 ? 2 : c.scale);
     HR_W = W * (c.scale == 4 ? 2 : c.scale);
   }
@@ -995,7 +1116,7 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
     e.d2s_cout = h->ps_out;
     e.dst_f32 = h->hr.get();
     e.d2s_pitch = h->ps_out;
-    if (add_tc_launch(h, pl.get(), h->tcl[ti++], h->mid_hi.get(), two ? h->mid_lo.get() : nullptr, h->mid_pitch, n, HR_H, HR_W, e))
+    if (add_layer_launch(h, pl.get(), h->tcl[ti++], h->mid_hi.get(), two ? h->mid_lo.get() : nullptr, h->mid_pitch, n, HR_H, HR_W, e))
       return nullptr;
     HR_H *= 2;
     HR_W *= 2;
@@ -1129,12 +1250,7 @@ static int launch_ds_tile_k(dcscn_handle* h, const DsTileParams& p, unsigned gri
 static int launch_ds_tile(dcscn_handle* h, DsTileParams p, int ksz, cudaStream_t st) {
   if (ksz != 1 && ksz != 3) return fail("depthwise-separable layer: kernel size %d is not supported (1 or 3)", ksz);
   if (p.cout > 32 && p.cin > kDtCC) return fail("depthwise-separable layer %d -> %d: more than 32 output columns need <= 32 input channels", p.cin, p.cout);
-  const int cols = p.cout < 32 ? ((p.cout + 3) & ~3) : 32;
-  // the kernel's shared-memory carve-up uses the per-pass column count of the instantiated template
-  const int tcols = cols <= 4 ? 4 : cols <= 8 ? 8 : cols <= 16 ? 16 : cols <= 24 ? 24 : 32;
-  const size_t in_px = ksz == 3 ? (size_t)(kDtT + 2) * kDtS : (size_t)kDtThreads;
-  const size_t cache = ds_tile_caches_depthwise(ksz, p.cin, p.cout) ? (size_t)kDtThreads * kDtCP : 0;   // private depthwise rows
-  const size_t smem = (in_px * kDtCP + (size_t)p.cin * tcols + (size_t)ksz * ksz * p.cin + cache) * sizeof(float);
+  const size_t smem = ds_tile_launch_smem(ksz, p.cin, p.cout);
   if (smem > 200 * 1024) return fail("depthwise-separable layer %d -> %d exceeds the kernel's shared memory", p.cin, p.cout);
   unsigned grid;
   if (ksz == 3) {
@@ -1254,6 +1370,17 @@ static int forward_ds_tile(dcscn_handle* h, const float* x, const float* x2, flo
   return launch_ds_tile(h, p, lr.k, st);
 }
 
+static int launch_depthwise(dcscn_handle* h, const DwParams& p, cudaStream_t st) {
+  const long long total = (long long)p.n_img * p.H * p.W * (p.cpad >> 3);
+  const int grid = (int)std::min<long long>((total + 255) / 256, (long long)h->sm_count * 16);
+  if (p.ksz == 3) depthwise_planes_kernel<3><<<grid, 256, 0, st>>>(p);
+  else if (p.ksz == 5) depthwise_planes_kernel<5><<<grid, 256, 0, st>>>(p);
+  else return fail("depthwise step: kernel size %d is not supported (3 or 5)", p.ksz);
+  CUDA_TRY(cudaGetLastError());
+  h->launches++;
+  return mark(h, st);
+}
+
 // CNN1 and the tensor-core layers of one forward, in execution order, on `st` (a capturing stream when the plan's graph is
 // being built).  The last kernel (R-CNN1 gather / R-CNN1) is issued by forward_impl: it alone touches x2 and y.
 static int issue_front(dcscn_handle* h, Plan* pl, const float* x, int n, int H, int W, bool fused, cudaStream_t st) {
@@ -1276,6 +1403,7 @@ static int issue_front(dcscn_handle* h, Plan* pl, const float* x, int n, int H, 
     if (mark(h, st)) return 1;
   }
   for (size_t i = 0; i < pl->tc.size(); ++i) {
+    if (pl->dw[i].ksz && launch_depthwise(h, pl->dw[i], st)) return 1;
     const TcLaunch& L = ((int)i == pl->fused_index && !fused) ? pl->unfused : pl->tc[i];
     if (launch_tc(h, L, st)) return 1;
     if (mark(h, st)) return 1;
@@ -1290,7 +1418,7 @@ static int forward_impl(dcscn_handle* h, const float* x, const float* x2, float*
   if (h->params_dirty && finalize_params(h)) return 1;
   if (ensure_workspace(h, (size_t)n * H * W)) return 1;
   if (!h->tiling) h->tiled_last = false;
-  if (h->cfg.depthwise_separable) {
+  if (uses_ds_tile(h)) {
     h->ds_n = n; h->ds_h = H; h->ds_w = W;
     return forward_ds_tile(h, x, x2, y, n, H, W, st);
   }
@@ -1328,7 +1456,7 @@ static int forward_impl(dcscn_handle* h, const float* x, const float* x2, float*
     cudaGraphDestroy(g);
     if (ie != cudaSuccess) { pl->gexec = nullptr; return fail("forward: cudaGraphInstantiate failed: %s", cudaGetErrorString(ie)); }
     pl->g_x = x; pl->g_epoch = h->graph_epoch; pl->g_fused = fused;
-    pl->g_launches = 1 + (int)pl->tc.size();
+    pl->g_launches = 1 + pl->dw_count + (int)pl->tc.size();
     CUDA_TRY(cudaGraphLaunch(pl->gexec, st));
     h->launches += pl->g_launches;
     h->graph_replays++;
@@ -1484,7 +1612,7 @@ static int forward_any(dcscn_handle* h, const float* x, const float* x2, float* 
   if (n <= 0 || H <= 0 || W <= 0) return fail("forward: bad shape n=%d h=%d w=%d", n, H, W);
   CUDA_TRY(cudaSetDevice(h->cfg.device_id));
   if (h->params_dirty && finalize_params(h)) return 1;
-  const bool ds = h->cfg.depthwise_separable != 0;
+  const bool ds = uses_ds_tile(h);
   const size_t ws_px = workspace_shape(h).bytes_per_px(ds);
   const long long budget = h->workspace_mb << 20;
   const long long lr_total = (long long)n * H * W;
@@ -1768,7 +1896,7 @@ int dcscn_get_activation(dcscn_handle* h, const char* tensor, float* host_data, 
   if (h->tiled_last)
     return fail("dcscn_get_activation: the last forward ran tiled (option workspace_mb): the buffers hold its last batch "
                 "of windows, not the image");
-  if (h->cfg.depthwise_separable) {
+  if (uses_ds_tile(h)) {
     if (h->ds_n == 0) return fail("dcscn_get_activation: no forward has run yet");
     CUDA_TRY(cudaSetDevice(h->cfg.device_id));
     CUDA_TRY(cudaDeviceSynchronize());
@@ -1891,7 +2019,7 @@ int dcscn_get_timings(dcscn_handle* h, float* ms, int capacity, int* count, char
   *count = n;
   if (names && names_len > 0) {
     std::string s = "CNN1";
-    if (h->cfg.depthwise_separable) {
+    if (uses_ds_tile(h)) {
       s = "";
       for (const LayerDef& l : h->layers) {
         std::string nm = l.scope.substr(0, l.scope.find('/'));
@@ -1900,7 +2028,7 @@ int dcscn_get_timings(dcscn_handle* h, float* ms, int capacity, int* count, char
         s += (s.empty() ? "" : ",") + nm;
       }
     } else {
-      for (const TcLayer& t : h->tcl) s += "," + t.name;
+      for (const TcLayer& t : h->tcl) s += (t.dw_ksz ? ",dw:" + t.name : "") + "," + t.name;
       s += ",R-CNN1";
     }
     if (h->tiled_last) {   // every batch of windows: gather, the layers, stitch
@@ -2295,7 +2423,7 @@ int dcscn_dropout_mask(dcscn_handle* h, const char* tensor, uint32_t seed, int n
   } else if (t == "B1") { C = c.nin_filters2; n_total = h->a1_w + h->b1_w; col0 = h->a1_w; layer = (uint32_t)(L + 1);
   } else if (t == "B2") { C = c.nin_filters2; n_total = h->b1_w; col0 = 0; layer = (uint32_t)(L + 2);
   } else return fail("dcscn_dropout_mask: tensor '%s' has no dropout", tensor);
-  if (c.depthwise_separable) {   // train_ds.inc: dense [pixel][channel] indexing, A1 / B2 / B1 are layers L+1 / L+2 / L+3
+  if (uses_ds_tile(h)) {   // train_ds.inc: dense [pixel][channel] indexing, A1 / B2 / B1 are layers L+1 / L+2 / L+3
     n_total = C; col0 = 0;
     if (t == "B1") layer = (uint32_t)(L + 3);
   }

@@ -915,4 +915,47 @@ __global__ void __launch_bounds__(256) gather_params_kernel(const float* __restr
   }
 }
 
+// ---- wide depthwise-separable graphs: the dense train step on composed filters ----
+// One tf.nn.separable_conv2d layer's variables inside the flat parameter vectors: depthwise [taps][cin], pointwise
+// [cin][cout] and the layer's conv_W slot [taps][cin][cout], which holds the composed filter / its gradient.
+struct DsComposeParams {
+  int taps, cin, cout;
+  size_t dw, pw, wc;     // offsets into the flat vectors
+};
+
+// wc[t][ci][co] = dw[t][ci] * pw[ci][co] (one fp32 product, as the host packing forms it).
+__global__ void __launch_bounds__(256) ds_compose_kernel(const float* __restrict__ w, float* __restrict__ wc,
+                                                         const DsComposeParams p) {
+  const long long n = (long long)p.taps * p.cin * p.cout;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const int co = (int)(i % p.cout);
+    const long long tc = i / p.cout;               // t * cin + ci
+    const int ci = (int)(tc % p.cin);
+    wc[p.wc + i] = w[p.dw + tc] * w[p.pw + (size_t)ci * p.cout + co];
+  }
+}
+
+// The chain rule through the composition, from the composed filter's gradient gc[t][ci][co]:
+//   d dw[t][ci] = sum_co gc[t][ci][co] pw[ci][co],   d pw[ci][co] = sum_t gc[t][ci][co] dw[t][ci]
+// (fp64 sums); written into g, whose depthwise / pointwise slots nothing else of the dense step touches.
+__global__ void __launch_bounds__(256) ds_decompose_kernel(const float* __restrict__ w, const float* __restrict__ gc,
+                                                           float* __restrict__ g, const DsComposeParams p) {
+  const long long ndw = (long long)p.taps * p.cin, n = ndw + (long long)p.cin * p.cout;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    double s = 0.0;
+    if (i < ndw) {
+      const int ci = (int)(i % p.cin);
+      for (int co = 0; co < p.cout; ++co)
+        s += (double)gc[p.wc + (size_t)i * p.cout + co] * (double)w[p.pw + (size_t)ci * p.cout + co];
+      g[p.dw + i] = (float)s;
+    } else {
+      const long long j = i - ndw;                 // ci * cout + co
+      const int ci = (int)(j / p.cout);
+      for (int t = 0; t < p.taps; ++t)
+        s += (double)gc[p.wc + ((size_t)t * p.cin + ci) * p.cout + (j % p.cout)] * (double)w[p.dw + (size_t)t * p.cin + ci];
+      g[p.pw + j] = (float)s;
+    }
+  }
+}
+
 }  // namespace dcscn
