@@ -8,7 +8,7 @@ by the CLIs (`build_graph` -> [`build_optimizer`] -> `build_summary_saver` -> `i
 `load_model`), `do` / `do_for_file` / `do_for_evaluate[_with_output]` / `evaluate` / `evaluate_bicubic`,
 `train_batch` / `build_input_batch` and the learning-rate / status bookkeeping, and the log lines.
 Replaced: everything `sess.run` did.  Not carried over (TensorFlow-specific, SURVEY.md section 2 rows 15-17):
-tensorboard summaries, frozen-graph loading, transposed-conv upsampler, batch-norm.
+tensorboard summaries, frozen-graph loading, batch-norm.
 """
 
 import logging
@@ -23,6 +23,26 @@ from helper import engine as eng
 from helper import loader, tf_bundle, utilty as util
 
 BICUBIC_METHOD_STRING = "bicubic"
+
+
+def bilinear_kernel(size):
+    """The size x size bilinear interpolation kernel: the outer product of a tent that falls linearly from 1 at the
+    kernel's centre to 0 one factor = ceil(size / 2) away (the centre sits between two taps when size is even)."""
+    factor = (size + 1) // 2
+    center = factor - 1 if size % 2 == 1 else factor - 0.5
+    tent = 1.0 - np.abs(np.arange(size) - center) / factor
+    return np.outer(tent, tent)
+
+
+def upscale_weight(shape):
+    """Initial Up-TCNN/Tconv_W [K, K, C, C]: the bilinear kernel on every channel's own diagonal entry, zero across
+    channels, so the untrained layer is a bilinear up-scaler (utilty.py:366-390)."""
+    k, _, c, _ = shape
+    w = np.zeros(shape, np.float32)
+    kern = bilinear_kernel(k).astype(np.float32)
+    for i in range(c):
+        w[:, :, i, i] = kern
+    return w
 
 
 def _dist_rank_world():
@@ -225,8 +245,6 @@ class SuperResolution:
         problems = []
         if self.batch_norm:
             problems.append("--batch_norm")
-        if not self.pixel_shuffler:
-            problems.append("--pixel_shuffler=false (transposed-conv upsampler)")
         if not self.use_nin:
             problems.append("--use_nin=false")
         if self.channels != 1:
@@ -251,7 +269,7 @@ class SuperResolution:
             depthwise_separable=self.depthwise_separable, channels=self.channels, dropout_keep=self.dropout_rate,
             l2_decay=self.l2_decay, clipping_norm=self.clipping_norm, beta1=self.beta1, beta2=self.beta2,
             epsilon=self.epsilon, device_id=self.gpu_device_id, precision=prec, activator=self.activator,
-            optimizer=self.optimizer, momentum=self.momentum)
+            optimizer=self.optimizer, momentum=self.momentum, transposed_upsampler=not self.pixel_shuffler)
 
     def build_graph(self):
         """DCSCN.py:222-332: creates the engine (variables at their initial values) and the bookkeeping strings."""
@@ -266,7 +284,13 @@ class SuperResolution:
         pix = 1
         total = 0
         for name, shape in shapes.items():
-            if not name.endswith("conv_W"):
+            if name == "Up-TCNN/Tconv_W":   # build_transposed_conv: s*s times the pixels, K x K x C x C, +1 field
+                k, _, c, _ = shape
+                pix *= self.scale * self.scale
+                self.complexity += pix * k * k * c * c
+                self.receptive_fields += 1
+                continue
+            if not name.endswith("/conv_W"):
                 continue
             scope = name[:-len("/conv_W")]
             k, _, cin, cout = shape
@@ -302,12 +326,15 @@ class SuperResolution:
         self.saver = with_saver
 
     def init_all_variables(self):
-        """tf_graph.py:73-75: (re-)initialise weights - 'he' truncated normal (utilty.py:360-363), bias 0, alpha 0.1."""
+        """tf_graph.py:73-75: (re-)initialise weights - 'he' truncated normal (utilty.py:360-363), bias 0, alpha 0.1,
+        and the transposed upsampler's Tconv_W as a bilinear up-scaler (upscale_weight)."""
         if self.engine is None:
             raise RuntimeError("call build_graph() first")
         rng = np.random.RandomState()
         for name, shape in self.engine.param_shapes().items():
-            if name.endswith("conv_W"):
+            if name.endswith("/Tconv_W"):
+                self.engine.set_param(name, upscale_weight(shape))
+            elif name.endswith("conv_W"):
                 k, _, cin, _ = shape
                 std = {"he": math.sqrt(2.0 / (k * k * cin))}.get(self.initializer, self.weight_dev)
                 w = rng.randn(*shape)

@@ -314,6 +314,15 @@ static int planes(const dcscn_handle* h) { return h->cfg.precision == DCSCN_PREC
 // A depthwise-separable graph whose layers all run on the fp32 CUDA-core kernels (forward_ds_tile).
 static bool uses_ds_tile(const dcscn_handle* h) { return h->cfg.depthwise_separable && !h->ds_wide; }
 
+// --pixel_shuffler=false: the upsampler is Up-TCNN, one stride-s conv2d_transpose (tf_graph.py build_transposed_conv),
+// computed as a 3x3 LR convolution into s*s*C columns (tconv_filter) followed by depth_to_space(s).
+static bool tconv(const dcscn_handle* h) { return h->cfg.transposed_upsampler != 0; }
+// Whether the upsampler is two x2 pixel-shuffler stages (Up-PS at LR, Up-PS2 at 2x): x4 with the pixel shuffler.
+static bool two_stage_up(const dcscn_handle* h) { return h->cfg.scale == 4 && !tconv(h); }
+// The scope of the layer that reads Concat2 = [B2 | A1].
+static std::string up_scope(const dcscn_handle* h) { return tconv(h) ? "Up-TCNN" : "Up-PS/Up-PS_CNN"; }
+static int tconv_ksize(int s) { return 2 * s - s % 2; }   // util.get_upscale_filter_size
+
 // Filter-count schedule of the feature-extraction stack (DCSCN.py:240-244).
 static std::vector<int> feature_filters(const dcscn_config& c) {
   std::vector<int> out;
@@ -378,6 +387,7 @@ static bool ds_tile_accepts(int ksz, int cin, int cout) {
 // the fp32 CUDA-core kernels and the wide path (dcscn_handle::ds_wide).
 static bool ds_tile_fits(const dcscn_handle* h) {
   const dcscn_config& c = h->cfg;
+  if (tconv(h)) return false;   // Up-TCNN is a dense conv2d_transpose even here: it runs on the tensor cores
   int T = 0;   // concat channels with 4-aligned slots (finalize_params_ds)
   for (int f : h->filters) T += (f + 3) & ~3;
   const int cps = c.nin_filters + c.nin_filters2;
@@ -416,8 +426,10 @@ static int build_graph(dcscn_handle* h) {
   h->layers.push_back({"B1", 1, total, c.nin_filters2, true, true});
   h->layers.push_back({"B2", 3, c.nin_filters2, c.nin_filters2, true, true});
   cin = c.nin_filters + c.nin_filters2;
-  h->ps_out = c.pixel_shuffler_filters != 0 ? c.pixel_shuffler_filters : cin;
-  if (c.scale == 4) {  // DCSCN.py:298-304
+  h->ps_out = c.pixel_shuffler_filters != 0 && !c.transposed_upsampler ? c.pixel_shuffler_filters : cin;
+  if (c.transposed_upsampler) {  // DCSCN.py:310-311: C -> C at s x the resolution, no bias, no activation
+    h->layers.push_back({"Up-TCNN", 3, cin, c.scale * c.scale * cin, false, false});
+  } else if (c.scale == 4) {  // DCSCN.py:298-304
     h->layers.push_back({"Up-PS/Up-PS_CNN", c.cnn_size, cin, 4 * cin, true, false});
     h->layers.push_back({"Up-PS2/Up-PS2_CNN", c.cnn_size, cin, 4 * h->ps_out, true, false});
   } else {
@@ -427,6 +439,11 @@ static int build_graph(dcscn_handle* h) {
 
   for (const LayerDef& l : h->layers) {
     std::string base = l.scope.substr(l.scope.find_last_of('/') == std::string::npos ? 0 : l.scope.find_last_of('/') + 1);
+    if (l.scope == "Up-TCNN") {   // util.upscale_weight: [K, K, out, in]
+      const int K = tconv_ksize(c.scale);
+      add_param(h, "Up-TCNN/Tconv_W", {K, K, l.cin, l.cin}, 0.f);
+      continue;
+    }
     add_param(h, l.scope + "/conv_W", {l.k, l.k, l.cin, l.cout}, 0.f);
     if (c.depthwise_separable) {  // tf_graph.py:157-160; conv_W stays as the (dead) variable the reference also creates
       add_param(h, l.scope + "/depthwise_W", {l.k, l.k, l.cin, 1}, 0.f);
@@ -468,13 +485,45 @@ static const std::vector<float>& P(const dcscn_handle* h, const std::string& nam
 // (one input channel) and R-CNN1 (one output channel).
 // Once a handle trains, every layer is composed instead: the dense train step differentiates the composed k x k filters.
 static bool ds_split(const dcscn_handle* h, const LayerDef& l) {
-  return h->ds_wide && !h->train_enabled && l.k > 1 && l.cin > 1 && l.cout > 1;
+  return h->ds_wide && !h->train_enabled && l.k > 1 && l.cin > 1 && l.cout > 1 && l.scope != "Up-TCNN";
 }
 
-// The HWIO filter the packed form of layer `l` computes with: conv_W; on the wide depthwise-separable path the pointwise
-// filter alone for a split layer, else W[t][ci][co] = dw[t][ci] pw[ci][co] in `tmp` (exact in real arithmetic: one
-// side of the product has a single channel or a single tap).
+// Index in Up-TCNN/Tconv_W W[K][K][C][C] ([h, w, out, in]) behind every entry of its 3x3 LR filter
+// F[3][3][C][s*s*C] (HWIO), or -1 for a structural zero.  With SAME padding, pad_top = (K - s) / 2 and
+//   out[s*m + p] = sum_d in[m + d] * W[p + pad_top - s*d]   per axis,
+// and for s = 2, 3, 4 every used offset d lies in {-1, 0, 1}: F[dy+1][dx+1][ci][(py*s + px)*C + co] =
+// W[py + pad_top - s*dy][px + pad_top - s*dx][co][ci].  (phase, offset) -> tap is a bijection onto [0, K), so each
+// W entry appears in F exactly once and the map inverts without sums (tconv gradient, train_engine.inc).
+static std::vector<int> tconv_filter_map(int s, int C) {
+  const int K = tconv_ksize(s), pad = (K - s) / 2, cols = s * s * C;
+  std::vector<int> m((size_t)9 * C * cols, -1);
+  for (int dy = -1; dy <= 1; ++dy)
+    for (int dx = -1; dx <= 1; ++dx)
+      for (int py = 0; py < s; ++py)
+        for (int px = 0; px < s; ++px) {
+          const int ky = py + pad - s * dy, kx = px + pad - s * dx;
+          if (ky < 0 || ky >= K || kx < 0 || kx >= K) continue;
+          const int tap = (dy + 1) * 3 + (dx + 1);
+          for (int ci = 0; ci < C; ++ci)
+            for (int co = 0; co < C; ++co)
+              m[((size_t)tap * C + ci) * cols + (py * s + px) * C + co] = ((ky * K + kx) * C + co) * C + ci;
+        }
+  return m;
+}
+
+// The HWIO filter the packed form of layer `l` computes with: conv_W; Up-TCNN's 3x3 form of Tconv_W (tconv_filter_map,
+// a pure gather); on the wide depthwise-separable path the pointwise filter alone for a split layer, else
+// W[t][ci][co] = dw[t][ci] pw[ci][co] in `tmp` (exact in real arithmetic: one side of the product has a single channel
+// or a single tap).
 static const std::vector<float>& layer_filter(const dcscn_handle* h, const LayerDef& l, std::vector<float>& tmp) {
+  if (l.scope == "Up-TCNN") {   // shadow mode too: structural zeros stay 0, i.e. "no source" in the refresh maps
+    const std::vector<float>& W = P(h, "Up-TCNN/Tconv_W");
+    const std::vector<int> m = tconv_filter_map(h->cfg.scale, l.cin);
+    tmp.assign(m.size(), 0.f);
+    for (size_t i = 0; i < m.size(); ++i)
+      if (m[i] >= 0) tmp[i] = W[m[i]];
+    return tmp;
+  }
   // shadow mode (build_refresh_maps): a composed filter lives in the layer's conv_W slot of TrainState::d_wc
   if (!h->ds_wide || h->shadow_mode) return P(h, l.scope + "/conv_W");
   const std::vector<float>& pw = P(h, l.scope + "/pointwise_W");
@@ -724,17 +773,19 @@ static int construct_tc_layers(dcscn_handle* h) {
     fuse_columns(h, t, "B2", 0, 0);
     h->tcl.push_back(std::move(t));
   }
-  // Up-PS (+ Up-PS2): input = Concat2 = [B2 | A1]
+  // Up-PS (+ Up-PS2) or Up-TCNN: input = Concat2 = [B2 | A1]
   {
-    const LayerDef* l = find_layer(h, "Up-PS/Up-PS_CNN");
+    const std::string scope = up_scope(h);
+    const LayerDef* l = find_layer(h, scope);
     // the LAST depth_to_space layer carries the fused R-CNN1 epilogue (3x3 R-CNN1 only)
     const int fuse_unit = find_layer(h, "R-CNN1")->k == 3 ? h->ps_out : 0;
-    TcLayer t = make_tc("Up-PS", tc_ksz(h, *l), l->cin, l->cout, h->nin_pitch, c.scale == 4 ? 0 : fuse_unit);
+    TcLayer t = make_tc(tconv(h) ? "Up-TCNN" : "Up-PS", tc_ksz(h, *l), l->cin, l->cout, h->nin_pitch,
+                        two_stage_up(h) ? 0 : fuse_unit);
     for (int ci = 0; ci < c.nin_filters2; ++ci) t.in_map.push_back(ci);
     for (int ci = 0; ci < c.nin_filters; ++ci) t.in_map.push_back(h->b1_w + ci);
-    fuse_columns(h, t, "Up-PS/Up-PS_CNN", 0, 0);
+    fuse_columns(h, t, scope, 0, 0);
     h->tcl.push_back(std::move(t));
-    if (c.scale == 4) {
+    if (two_stage_up(h)) {
       const LayerDef* l2 = find_layer(h, "Up-PS2/Up-PS2_CNN");
       TcLayer t2 = make_tc("Up-PS2", tc_ksz(h, *l2), l2->cin, l2->cout, h->mid_pitch, fuse_unit);
       for (int ci = 0; ci < l2->cin; ++ci) t2.in_map.push_back(ci);
@@ -832,7 +883,7 @@ static WorkspaceShape workspace_shape(const dcscn_handle* h) {
   w.feat = h->feat_pitch;
   w.b1 = h->b1_w;
   w.nin = h->nin_pitch;
-  w.mid = c.scale == 4 ? 4 * (size_t)h->mid_pitch : 0;
+  w.mid = two_stage_up(h) ? 4 * (size_t)h->mid_pitch : 0;
   w.hr = s2 * h->ps_out;
   w.vbuf = s2 * 9 * (size_t)rdot_parts(h->tcl.empty() ? 16 : h->tcl.back().n_pad, h->ps_out);
   w.planes = planes(h);
@@ -866,7 +917,7 @@ static int ensure_workspace(dcscn_handle* h, size_t lr_px) {
   if (h->feat_hi.alloc(lr_px * ws.feat, true) || h->feat_lo.alloc(two ? lr_px * ws.feat : 0, true)) return 1;
   if (h->b1_hi.alloc(lr_px * ws.b1, true) || h->b1_lo.alloc(two ? lr_px * ws.b1 : 0, true)) return 1;
   if (h->nin_hi.alloc(lr_px * ws.nin, true) || h->nin_lo.alloc(two ? lr_px * ws.nin : 0, true)) return 1;
-  if (c.scale == 4) {
+  if (two_stage_up(h)) {
     if (h->mid_hi.alloc(lr_px * ws.mid, true) || h->mid_lo.alloc(two ? lr_px * ws.mid : 0, true)) return 1;
   }
   if (h->u_hi.alloc(lr_px * ws.u, true) || h->u_lo.alloc(two ? lr_px * ws.u : 0, true)) return 1;
@@ -1086,11 +1137,11 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
     if (add_layer_launch(h, pl.get(), h->tcl[ti++], h->b1_hi.get(), two ? h->b1_lo.get() : nullptr, h->b1_w, n, H, W, e)) return nullptr;
   }
   int HR_H = H, HR_W = W;
-  {  // Up-PS
+  {  // Up-PS, or Up-TCNN (its 3x3 LR form, then depth_to_space(s) in one step at every scale)
     EpiParams e;
     memset(&e, 0, sizeof(e));
     e.keep_prob = 1.0f;
-    if (c.scale == 4) {
+    if (two_stage_up(h)) {
       e.mode = EPI_D2S_PLANES;
       e.d2s_r = 2;
       e.d2s_cout = c.nin_filters + c.nin_filters2;
@@ -1104,10 +1155,10 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
       e.d2s_pitch = h->ps_out;
     }
     if (add_layer_launch(h, pl.get(), h->tcl[ti++], h->nin_hi.get(), two ? h->nin_lo.get() : nullptr, h->nin_pitch, n, H, W, e)) return nullptr;
-    HR_H = H * (c.scale == 4 ? 2 : c.scale);
-    HR_W = W * (c.scale == 4 ? 2 : c.scale);
+    HR_H = H * (two_stage_up(h) ? 2 : c.scale);
+    HR_W = W * (two_stage_up(h) ? 2 : c.scale);
   }
-  if (c.scale == 4) {  // Up-PS2 at 2x resolution
+  if (two_stage_up(h)) {  // Up-PS2 at 2x resolution
     EpiParams e;
     memset(&e, 0, sizeof(e));
     e.keep_prob = 1.0f;
@@ -1508,15 +1559,31 @@ static int forward_impl(dcscn_handle* h, const float* x, const float* x2, float*
 // ------------------------------------------------------------------------------ tiled inference ----
 // LR pixels of context a window core needs: the longest dependency path CNN1 .. CNNL -> B1 (1x1) -> B2 -> Up-PS
 // [-> Up-PS2 at 2x] -> R-CNN1 at HR resolution, walked back from an LR core edge.  An HR reach of q pixels past an edge
-// of s-times upscaled pixels is ceil(q / s) pixels before the upscale.
+// of s-times upscaled pixels is ceil(q / s) pixels before the upscale.  Up-TCNN and R-CNN1 are walked back together
+// (tconv_halo): the 3x3 LR form of Up-TCNN reads only one side of each LR pixel per output phase.
+static int tconv_halo(int s, int hr) {
+  const int K = tconv_ksize(s), pad = (K - s) / 2;
+  int reach = 0;
+  for (int o = -hr; o < s + hr; ++o) {   // HR pixels R-CNN1 reads around the s outputs of LR pixel 0
+    const int m = o >= 0 ? o / s : -((-o + s - 1) / s), p = o - m * s;
+    for (int d = -1; d <= 1; ++d) {
+      const int k = p + pad - s * d;
+      if (k >= 0 && k < K) reach = std::max(reach, std::abs(m + d));
+    }
+  }
+  return reach;
+}
+
 static int tile_halo(const dcscn_handle* h) {
   auto half = [](int k) { return (k - 1) / 2; };
   auto k_of = [h](const std::string& scope) { return find_layer(h, scope)->k; };
   int r = 0;
   for (int i = 0; i < h->cfg.layers; ++i) r += half(k_of("CNN" + std::to_string(i + 1)));
-  r += half(k_of("B1")) + half(k_of("B2")) + half(k_of("Up-PS/Up-PS_CNN"));
+  r += half(k_of("B1")) + half(k_of("B2"));
   const int hr = half(k_of("R-CNN1"));
-  if (h->cfg.scale == 4) r += (half(k_of("Up-PS2/Up-PS2_CNN")) + (hr + 1) / 2 + 1) / 2;
+  if (tconv(h)) return r + tconv_halo(h->cfg.scale, hr);
+  r += half(k_of("Up-PS/Up-PS_CNN"));
+  if (two_stage_up(h)) r += (half(k_of("Up-PS2/Up-PS2_CNN")) + (hr + 1) / 2 + 1) / 2;
   else r += (hr + h->cfg.scale - 1) / h->cfg.scale;
   return r;
 }
@@ -1944,11 +2011,11 @@ int dcscn_get_activation(dcscn_handle* h, const char* tensor, float* host_data, 
     hi = h->nin_hi.get(); lo = h->nin_lo.get(); pitch = h->nin_pitch; off = 0; ch = c.nin_filters2;
   } else if (t == "B1") {
     hi = h->b1_hi.get(); lo = h->b1_lo.get(); pitch = h->b1_w; off = 0; ch = c.nin_filters2;
-  } else if (t == "Up-PS" && c.scale == 4) {
+  } else if (t == "Up-PS" && two_stage_up(h)) {
     hi = h->mid_hi.get(); lo = h->mid_lo.get(); pitch = h->mid_pitch; off = 0; ch = c.nin_filters + c.nin_filters2; px *= 4;
-  } else if (((t == "Up-PS" && c.scale != 4) || (t == "Up-PS2" && c.scale == 4)) && pl->ran_fused) {
+  } else if (t == (tconv(h) ? "Up-TCNN" : two_stage_up(h) ? "Up-PS2" : "Up-PS") && pl->ran_fused) {
     return fail("dcscn_get_activation: '%s' is not materialised when the R-CNN1 fusion is on (set option fuse_last=0)", tensor);
-  } else if ((t == "Up-PS" && c.scale != 4) || (t == "Up-PS2" && c.scale == 4)) {
+  } else if (t == (tconv(h) ? "Up-TCNN" : two_stage_up(h) ? "Up-PS2" : "Up-PS")) {
     f32 = h->hr.get(); pitch = h->ps_out; ch = h->ps_out; px *= (size_t)c.scale * c.scale;
   } else {
     return fail("dcscn_get_activation: no tensor '%s'", tensor);

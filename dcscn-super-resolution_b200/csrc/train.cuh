@@ -915,6 +915,13 @@ __global__ void __launch_bounds__(256) gather_params_kernel(const float* __restr
   }
 }
 
+// Up-TCNN (--pixel_shuffler=false): dW[i] = dF[src[i]], the gradient of Tconv_W from that of its 3x3 LR form F.  Each
+// Tconv_W element is exactly one entry of F (engine.cu tconv_filter_map), so the gather is exact.
+__global__ void __launch_bounds__(256) tconv_grad_gather_kernel(const float* __restrict__ dF, const int* __restrict__ src,
+                                                                float* __restrict__ dW, int n) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) dW[i] = dF[src[i]];
+}
+
 // ---- wide depthwise-separable graphs: the dense train step on composed filters ----
 // One tf.nn.separable_conv2d layer's variables inside the flat parameter vectors: depthwise [taps][cin], pointwise
 // [cin][cout] and the layer's conv_W slot [taps][cin][cout], which holds the composed filter / its gradient.

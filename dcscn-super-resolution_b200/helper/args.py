@@ -150,7 +150,7 @@ _REFERENCE_FLAGS = [
     ("reconstruct_filters", 32, "channels of intermediate R-CNN layers"),
     ("dropout_rate", 0.8, "keep probability during training (1 disables dropout)"),
     ("activator", "prelu", "activation of CNN1..CNNL, A1, B1, B2: prelu, relu, leaky_relu, sigmoid, tanh or selu"),
-    ("pixel_shuffler", True, "sub-pixel (depth_to_space) up-sampling; the transposed-conv variant is not carried over"),
+    ("pixel_shuffler", True, "sub-pixel (depth_to_space) up-sampling; false: one bilinear-initialised transposed convolution"),
     ("pixel_shuffler_filters", 0, "channels after the pixel shuffler; 0 keeps the channel count of its input"),
     ("self_ensemble", 8, "how many of the 8 flip / rotate variants are averaged at inference (1..8)"),
     ("batch_norm", False, "not supported by this engine (rejected when set)"),

@@ -65,6 +65,7 @@ class DcscnConfig(ctypes.Structure):
         ("activator", ctypes.c_int32),
         ("optimizer", ctypes.c_int32),
         ("momentum", ctypes.c_float),
+        ("transposed_upsampler", ctypes.c_int32),
     ]
 
 
@@ -156,7 +157,9 @@ def make_config(scale=2, layers=12, filters=196, min_filters=48, filters_decay_g
                 nin_filters=64, nin_filters2=32, cnn_size=3, reconstruct_layers=1, reconstruct_filters=32,
                 pixel_shuffler_filters=0, depthwise_separable=False, channels=1, dropout_keep=0.8,
                 l2_decay=0.0001, clipping_norm=5.0, beta1=0.9, beta2=0.999, epsilon=1e-8, device_id=0,
-                precision=PRECISION_F16X3, activator="prelu", optimizer="adam", momentum=0.9):
+                precision=PRECISION_F16X3, activator="prelu", optimizer="adam", momentum=0.9,
+                transposed_upsampler=False):
+    """`transposed_upsampler`: --pixel_shuffler=false (the Up-TCNN conv2d_transpose instead of Up-PS)."""
     c = DcscnConfig()
     c.struct_size = ctypes.sizeof(DcscnConfig)
     c.scale, c.layers, c.filters, c.min_filters = scale, layers, filters, min_filters
@@ -169,6 +172,7 @@ def make_config(scale=2, layers=12, filters=196, min_filters=48, filters_decay_g
     c.device_id, c.precision = device_id, precision
     c.activator = ACTIVATORS[activator]
     c.optimizer, c.momentum = OPTIMIZERS[optimizer], momentum
+    c.transposed_upsampler = int(transposed_upsampler)
     return c
 
 

@@ -91,6 +91,7 @@ typedef struct dcscn_config {
   int32_t activator;              /* --activator: DCSCN_ACTIVATOR_* (0 = prelu) */
   int32_t optimizer;              /* --optimizer: DCSCN_OPTIMIZER_* (0 = adam) */
   float momentum;                 /* --momentum (momentum and rmsprop) */
+  int32_t transposed_upsampler;   /* --pixel_shuffler=false: Up-TCNN, one stride-`scale` conv2d_transpose (0 = Up-PS) */
 } dcscn_config;
 
 /* SuperResolution(flags) + build_graph() + init_session (DCSCN.py:29, :222; tf_graph.py:65). */
@@ -104,6 +105,8 @@ const char* dcscn_last_error(void);
  * (tf.train.Saver, tf_graph.py:263-296): "CNN1/conv_W" [k,k,cin,cout] HWIO, "CNN1/conv_B",
  * "CNN1/prelu/CNN1_prelu", "A1/...", "B1/...", "B2/...", "Up-PS/Up-PS_CNN/conv_W", "R-CNN1/conv_W" ...
  * The "<scope>/prelu/<scope>_prelu" slopes exist only with DCSCN_ACTIVATOR_PRELU; the other activators have no variable.
+ * With cfg.transposed_upsampler the Up-PS variables are replaced by "Up-TCNN/Tconv_W" [K,K,C,C] (K = 2*scale - scale%2,
+ * C = nin_filters + nin_filters2, TF's conv2d_transpose layout [h, w, out, in]; no bias, not depthwise-separable).
  */
 int dcscn_num_params(dcscn_handle* h);
 int dcscn_param_info(dcscn_handle* h, int index, char* name_buf, int name_buf_len, int64_t* dims4, int* ndim);
@@ -229,7 +232,8 @@ int dcscn_dropout_mask(dcscn_handle* h, const char* tensor, uint32_t seed, int n
 
 /*
  * Parity / debug: output of one layer of the LAST forward as fp32 NHWC [n, H_l, W_l, cout_l]
- * (`tensor` is the reference's self.H entry: "CNN1".."CNNL", "A1", "B1", "B2", "Up-PS", "Up-PS2").
+ * (`tensor` is the reference's self.H entry: "CNN1".."CNNL", "A1", "B1", "B2", "Up-PS", "Up-PS2", or "Up-TCNN"
+ * [n, s*H, s*W, C] with cfg.transposed_upsampler).
  * Fails after a forward that ran tiled (option "workspace_mb"): the buffers then hold its last batch of windows.
  */
 int dcscn_get_activation(dcscn_handle* h, const char* tensor, float* host_data, int64_t numel);
@@ -240,10 +244,11 @@ int dcscn_get_activation(dcscn_handle* h, const char* tensor, float* host_data, 
  *   "y_", "dY"        the prediction and d loss / d y_ * grad_scale, [n, s*H, s*W, 1] (fp32, exact)
  *   "dZ:<layer>"      gradient at the layer's convolution output (before bias / activation), scaled by grad_scale:
  *                     CNNi, A1, B1, B2 [n, H, W, cout]; Up-PS [n, H, W, r*r*C] (x2, x3) or [n, H, W, 4*C] (x4), and at x4
- *                     Up-PS2 [n, 2H, 2W, 4*C], in the space_to_depth column order (i*r + j)*C + c
+ *                     Up-PS2 [n, 2H, 2W, 4*C], in the space_to_depth column order (i*r + j)*C + c; Up-TCNN
+ *                     [n, H, W, s*s*C] in the same order (its equivalent 3x3 convolution, see engine.cu tconv_filter)
  *   "dH:<layer>"      output of the layer's data-gradient twin = gradient at the layer's input: CNNi (i >= 2)
- *                     [.., filters(i-1)], A1+B1 [.., concat channels], B2 [.., nin_filters2], Up-PS [.., nin_filters2 +
- *                     nin_filters] (B2 then A1), Up-PS2 [n, 2H, 2W, C]
+ *                     [.., filters(i-1)], A1+B1 [.., concat channels], B2 [.., nin_filters2], Up-PS and Up-TCNN
+ *                     [.., nin_filters2 + nin_filters] (B2 then A1), Up-PS2 [n, 2H, 2W, C]
  *   "zneg:<layer>"    the fp16 min(z, 0) plane the forward stored for CNNi, A1, B1, B2
  */
 int dcscn_get_train_tensor(dcscn_handle* h, const char* name, float* host_data, int64_t numel);
