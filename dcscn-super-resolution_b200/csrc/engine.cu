@@ -2318,7 +2318,7 @@ int dcscn_get_grad(dcscn_handle* h, const char* name, float* host_data, int64_t 
 int dcscn_get_train_tensor(dcscn_handle* h, const char* name, float* host_data, int64_t numel) {
   if (!h || !name || !host_data) return fail("dcscn_get_train_tensor: null argument");
   TrainState* t = h->train.get();
-  if (!t || t->last_px == 0) return fail("dcscn_get_train_tensor: no train step of a tensor-core graph has run yet");
+  if (!t || (t->last_px == 0 && t->last_ds_px == 0)) return fail("dcscn_get_train_tensor: no train step has run yet");
   CUDA_TRY(cudaSetDevice(h->cfg.device_id));
   CUDA_TRY(cudaDeviceSynchronize());
   const std::string s(name);
@@ -2327,6 +2327,7 @@ int dcscn_get_train_tensor(dcscn_handle* h, const char* name, float* host_data, 
   int ch = 0;
   if (s.rfind("zneg:", 0) == 0) {   // min(z, 0) planes of the last training forward (prelu / leaky_relu only)
     if (!needs_zneg(h)) return fail("dcscn_get_train_tensor: '%s': the activator keeps no min(z, 0) planes", name);
+    if (t->last_px == 0) return fail("dcscn_get_train_tensor: '%s': the fp32 depthwise-separable step keeps no min(z, 0) planes (see \"Z:\")", name);
     const std::string l = s.substr(5);
     const __half* src = nullptr;
     int pitch = 0;
@@ -2349,7 +2350,7 @@ int dcscn_get_train_tensor(dcscn_handle* h, const char* name, float* host_data, 
     px = c.px; ch = c.ch;
     if (numel != (int64_t)(px * ch)) return fail("dcscn_get_train_tensor: '%s' has %lld elements, got %lld", name, (long long)(px * ch), (long long)numel);
     if (c.f32) {
-      CUDA_TRY(cudaMemcpy(host_data, c.hi.get(), px * sizeof(float), cudaMemcpyDeviceToHost));
+      CUDA_TRY(cudaMemcpy(host_data, c.hi.get(), px * ch * sizeof(float), cudaMemcpyDeviceToHost));
       return 0;
     }
     hi.resize(px * ch);

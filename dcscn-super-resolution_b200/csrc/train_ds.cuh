@@ -135,27 +135,32 @@ __global__ void __launch_bounds__(256) ds_act_bwd_kernel(const DsActBwdParams p)
   }
 }
 
-// out[c] += sum over pixels of src[px][c]   (C <= 256; block partials, one atomicAdd per block and column)
+// out[c] += sum over pixels of src[px][c]   (block partials, one atomicAdd per block and column).  blockIdx.y takes the
+// columns [256 y, 256 y + G) with G = min(256, C - 256 y): grid.y = ceil(C / 256).
 __global__ void __launch_bounds__(256) ds_colsum_kernel(const float* __restrict__ src, long long npx, int C, float* out,
                                                         int px_per_block) {
   __shared__ float s[256];
-  const int rows = 256 / C;                      // pixel rows handled in parallel by one block
-  const int c = threadIdx.x % C, rg = threadIdx.x / C;
+  const int c0 = blockIdx.y * 256, G = C - c0 < 256 ? C - c0 : 256;
+  const int rows = 256 / G;                      // pixel rows handled in parallel by one block
+  const int c = threadIdx.x % G, rg = threadIdx.x / G;
   const long long px0 = (long long)blockIdx.x * px_per_block;
   const long long px1 = px0 + px_per_block < npx ? px0 + px_per_block : npx;
   float acc = 0.f;
   if (rg < rows)
-    for (long long px = px0 + rg; px < px1; px += rows) acc += src[px * C + c];
+    for (long long px = px0 + rg; px < px1; px += rows) acc += src[px * C + c0 + c];
   s[threadIdx.x] = (rg < rows) ? acc : 0.f;
   __syncthreads();
-  if (threadIdx.x < C) {
+  if (threadIdx.x < G) {
     float t = 0.f;
-    for (int r = 0; r < rows; ++r) t += s[r * C + threadIdx.x];
-    atomicAdd(out + threadIdx.x, t);
+    for (int r = 0; r < rows; ++r) t += s[r * G + threadIdx.x];
+    atomicAdd(out + c0 + threadIdx.x, t);
   }
 }
 
-// d pw[c][co] += sum_px u[px][c] * dz[px][co]
+// d pw[c][co] += sum_px u[px][c] * dz[px][co].  Each (c, co) pair is one fp32 FMA chain over the block's pixels in
+// order, however the pixels are staged.  blockIdx.z takes the columns [co0, co0 + G), co0 = kDsDpwCols z, G = min(kDsDpwCols,
+// cout - co0); blockIdx.y a tile of kDsDpwPairs x 256 of its cin x G pairs.  A pass stages `chunk` pixels of u and of
+// those columns of dz: chunk (cin + G) floats of dynamic shared memory (ds_dpw_chunk).
 struct DsDpwParams {
   long long npx;
   int cin, cout;
@@ -163,34 +168,47 @@ struct DsDpwParams {
   const float* dz;
   float* dpw;
   int px_per_block;
+  int chunk;
 };
 constexpr int kDsDpwPairs = 17;                        // (c, co) pairs per thread: 17 x 256 = 4352 pairs per blockIdx.y
-constexpr int kDsDpwChunk = 32;                        // pixels staged per pass
+constexpr int kDsDpwChunk = 32;                        // most pixels staged per pass
+constexpr int kDsDpwCols = 256;                        // most dz columns per blockIdx.z
+constexpr int kDsDpwSmemFloats = 48 * 1024 / 4;        // the dynamic shared memory a launch may take without opting in
+
+// Pixels per pass of ds_dpw_kernel for a layer: up to kDsDpwChunk, as many as fit the default 48 KB; 0 = none fits.
+inline int ds_dpw_chunk(int cin, int cout) {
+  const int w = cin + (cout < kDsDpwCols ? cout : kDsDpwCols);
+  return kDsDpwSmemFloats / w < kDsDpwChunk ? kDsDpwSmemFloats / w : kDsDpwChunk;
+}
 
 __global__ void __launch_bounds__(256) ds_dpw_kernel(const DsDpwParams p) {
   extern __shared__ float ds_smem[];
+  const int co0 = blockIdx.z * kDsDpwCols, G = p.cout - co0 < kDsDpwCols ? p.cout - co0 : kDsDpwCols;
   float* su = ds_smem;                                 // [chunk][cin]
-  float* sz = ds_smem + kDsDpwChunk * p.cin;           // [chunk][cout]
-  const int pairs = p.cin * p.cout;
+  float* sz = ds_smem + p.chunk * p.cin;               // [chunk][G]
+  const int pairs = p.cin * G;
   const int e0 = blockIdx.y * (kDsDpwPairs * 256) + threadIdx.x;
   float acc[kDsDpwPairs];
 #pragma unroll
   for (int k = 0; k < kDsDpwPairs; ++k) acc[k] = 0.f;
   const long long px0 = (long long)blockIdx.x * p.px_per_block;
   const long long px1 = px0 + p.px_per_block < p.npx ? px0 + p.px_per_block : p.npx;
-  for (long long base = px0; base < px1; base += kDsDpwChunk) {
-    const int P = (int)((px1 - base) < kDsDpwChunk ? (px1 - base) : kDsDpwChunk);
+  for (long long base = px0; base < px1; base += p.chunk) {
+    const int P = (int)((px1 - base) < p.chunk ? (px1 - base) : p.chunk);
     __syncthreads();
     for (int i = threadIdx.x; i < P * p.cin; i += 256) su[i] = p.u[base * p.cin + i];
-    for (int i = threadIdx.x; i < P * p.cout; i += 256) sz[i] = p.dz[base * p.cout + i];
+    for (int i = threadIdx.x; i < P * G; i += 256) {
+      const int q = i / G;
+      sz[i] = p.dz[(base + q) * p.cout + co0 + (i - q * G)];
+    }
     __syncthreads();
 #pragma unroll
     for (int k = 0; k < kDsDpwPairs; ++k) {
       const int e = e0 + k * 256;
       if (e < pairs) {
-        const int c = e / p.cout, co = e - c * p.cout;
+        const int c = e / G, co = e - c * G;
         float a = acc[k];
-        for (int q = 0; q < P; ++q) a = fmaf(su[q * p.cin + c], sz[q * p.cout + co], a);
+        for (int q = 0; q < P; ++q) a = fmaf(su[q * p.cin + c], sz[q * G + co], a);
         acc[k] = a;
       }
     }
@@ -198,7 +216,10 @@ __global__ void __launch_bounds__(256) ds_dpw_kernel(const DsDpwParams p) {
 #pragma unroll
   for (int k = 0; k < kDsDpwPairs; ++k) {
     const int e = e0 + k * 256;
-    if (e < pairs) atomicAdd(p.dpw + e, acc[k]);
+    if (e < pairs) {
+      const int c = e / G;
+      atomicAdd(p.dpw + (size_t)c * p.cout + co0 + (e - c * G), acc[k]);
+    }
   }
 }
 

@@ -552,7 +552,9 @@ class Engine:
 
     def get_train_tensor(self, name, shape):
         """A tensor of the last train step (dcscn_get_train_tensor: "y_", "dY", "dZ:<layer>", "dH:<layer>",
-        "zneg:<layer>") as fp32 of `shape`; all but "zneg:" need set_option("grad_capture", 1) before the step."""
+        "zneg:<layer>"; "Wc:" / "dWc:<layer>" on wide depthwise-separable graphs; "U:", "Z:", "H:", "E:", "dU:<layer>"
+        on the fp32 depthwise-separable step) as fp32 of `shape`; all but "zneg:" need set_option("grad_capture", 1)
+        before the step."""
         a = np.empty(shape, dtype=np.float32)
         self._check(self.lib.dcscn_get_train_tensor(self.handle, name.encode(),
                                                     a.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), a.size))

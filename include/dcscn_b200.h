@@ -238,7 +238,7 @@ int dcscn_dropout_mask(dcscn_handle* h, const char* tensor, uint32_t seed, int n
  */
 int dcscn_get_activation(dcscn_handle* h, const char* tensor, float* host_data, int64_t numel);
 /*
- * Parity / debug: a tensor of the LAST train step of a tensor-core graph as fp32 NHWC (hi + lo of its fp16 planes),
+ * Parity / debug: a tensor of the LAST train step as fp32 NHWC; on a tensor-core graph hi + lo of its fp16 planes,
  * logical channels only.  After a train step dcscn_get_activation returns that step's forward, after dropout.  Needs
  * option "grad_capture" = 1 during the step, except for the "zneg:" planes, which every prelu / leaky_relu step keeps:
  *   "y_", "dY"        the prediction and d loss / d y_ * grad_scale, [n, s*H, s*W, 1] (fp32, exact)
@@ -250,6 +250,21 @@ int dcscn_get_activation(dcscn_handle* h, const char* tensor, float* host_data, 
  *                     [.., filters(i-1)], A1+B1 [.., concat channels], B2 [.., nin_filters2], Up-PS and Up-TCNN
  *                     [.., nin_filters2 + nin_filters] (B2 then A1), Up-PS2 [n, 2H, 2W, C]
  *   "zneg:<layer>"    the fp16 min(z, 0) plane the forward stored for CNNi, A1, B1, B2
+ * A wide depthwise-separable graph (one that trains through the tensor-core step on composed filters) adds
+ *   "Wc:<layer>"      the composed filter fp32(dw * pw) the step read, [k, k, cin, cout] (fp32, exact)
+ *   "dWc:<layer>"     the composed filter's gradient before ds_decompose, scaled by grad_scale, [k, k, cin, cout]
+ * The fp32 step of a narrow depthwise-separable graph (every other one) has no grad_scale and keeps no "zneg:" planes.
+ * Its tensors are fp32 copies, per layer (CNNi, A1, B1, B2, Up-PS/Up-PS_CNN, Up-PS2/Up-PS2_CNN, R-CNN1) at the
+ * resolution of the layer's input ([n, h, w, ch]) unless stated:
+ *   "y_", "dY"        as above, with grad_scale 1
+ *   "U:<layer>"       the depthwise output u = depthwise(input, depthwise_W), [.., cin]
+ *   "Z:<layer>"       the pre-activation z = u . pointwise_W + conv_B, [.., cout] (pixel shufflers: before depth_to_space)
+ *   "H:<layer>"       the output after activation and dropout, [.., cout]; pixel shufflers the whole depth_to_space
+ *                     output [n, r*h, r*w, C] (all but R-CNN1, whose output is "y_")
+ *   "dZ:<layer>"      d loss / d z, [.., cout];  "E:<layer>" (prelu) d loss / d h * min(z, 0), whose sums are d alpha
+ *   "dU:<layer>"      d loss / d u, [.., cin]
+ *   "dH:<layer>"      the gradient buffer at the layer's input as the layer's data-gradient kernel left it, [.., cin]:
+ *                     B1 writes the concat gradient, A1 then adds to it, CNNi+1 adds to CNNi's channels of it
  */
 int dcscn_get_train_tensor(dcscn_handle* h, const char* name, float* host_data, int64_t numel);
 

@@ -137,8 +137,10 @@ class Checker:
         return [(k, v) for k, v in self.worst.items() if not v <= 1.0]
 
 
-def check_step(eng, kw, w, x, x2, y, keep, seed, chk):
-    """Every backward kernel of the last train step of `eng` (run with grad_capture = 1) against its isolated reference."""
+def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None):
+    """Every backward kernel of the last train step of `eng` (run with grad_capture = 1) against its isolated reference.
+    `get_grad(name)` returns a variable's gradient as get_grad does (default: eng.get_grad); a wide depthwise-separable
+    graph passes its composed filters as the conv_W entries of `w` and reads their gradients from "dWc:"."""
     cfg = O.OracleConfig(**kw)
     n, h, wd = x.shape[:3]
     s = cfg.scale
@@ -159,7 +161,7 @@ def check_step(eng, kw, w, x, x2, y, keep, seed, chk):
         return t64(eng.get_activation(name, (n, r * h, r * wd, c)))
 
     def grad(name):
-        return torch.from_numpy(eng.get_grad(name)).to(dev(), torch.float64)
+        return torch.from_numpy((get_grad or eng.get_grad)(name)).to(dev(), torch.float64)
 
     def finalize(name, ssum, bar_sum):
         """get_grad of a variable whose fp32 sum (scaled by G) is `ssum` with accumulation bar `bar_sum`."""
