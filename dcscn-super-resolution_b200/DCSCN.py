@@ -636,15 +636,60 @@ class SuperResolution:
 
     # ------------------------------------------------------------------ inference ----
     def evaluate(self, test_filenames):
-        """DCSCN.py:534-545"""
+        """DCSCN.py:534-545.  On the device path (_device_evaluation) the test images are decoded once and kept in the
+        engine's evaluation store while the files stay the same (train.py evaluates after every epoch): each later call
+        uploads nothing and makes one engine call per image."""
         total_psnr = total_ssim = 0
         if len(test_filenames) == 0:
             return 0, 0
-        for filename in test_filenames:
-            psnr, ssim = self.do_for_evaluate(filename, print_console=False)
+        slots = self._eval_store(test_filenames) if self._device_evaluation() else [None] * len(test_filenames)
+        for filename, slot in zip(test_filenames, slots):
+            if slot is None:
+                psnr, ssim = self.do_for_evaluate(filename, print_console=False)
+            else:
+                psnr, ssim = self.engine.evaluate_image(slot, self.self_ensemble, self.max_value, self.psnr_calc_border_size)
             total_psnr += psnr
             total_ssim += ssim
         return total_psnr / len(test_filenames), total_ssim / len(test_filenames)
+
+    # ---- evaluation on the device (helper/engine.py: set_eval_images / evaluate_image) ----
+    def _device_evaluation(self):
+        """do_for_evaluate / evaluate_bicubic / evaluate run on the device in a single process with an engine that has
+        the evaluation call; under torchrun the host path keeps its flip sharding."""
+        return (_dist_rank_world()[1] == 1 and getattr(self, "engine", None) is not None
+                and hasattr(self.engine, "evaluate_image") and getattr(self, "channels", 1) == 1
+                and self.resampling_method == BICUBIC_METHOD_STRING)
+
+    def _device_eval_image(self, file_path):
+        """The decoded image the device path evaluates, or None for one it leaves to the host path (not 1 or 3 uint8
+        channels, or smaller than one scale x scale block)."""
+        image = util.load_image(file_path, print_console=False)
+        if (image.dtype != np.uint8 or image.ndim != 3 or image.shape[2] not in (1, 3)
+                or image.shape[0] < self.scale or image.shape[1] < self.scale):
+            return None
+        return image
+
+    @staticmethod
+    def _file_key(file_path):
+        st = os.stat(file_path)
+        return file_path, st.st_size, st.st_mtime_ns
+
+    def _eval_store(self, test_filenames):
+        """Store slot (or None: host path) of every file.  The store is rebuilt only when a file's (path, size, mtime)
+        changes; it does not depend on the weights."""
+        keys = [self._file_key(f) for f in test_filenames]
+        cached = getattr(self, "_eval_cache", None)
+        if cached is None or cached[0] != keys or cached[2] is not self.engine:
+            images, slots = [], []
+            for filename in test_filenames:
+                image = self._device_eval_image(filename)
+                slots.append(None if image is None else len(images))
+                if image is not None:
+                    images.append(image)
+            if images:
+                self.engine.set_eval_images(images)
+            self._eval_cache = cached = (keys, slots, self.engine)
+        return cached[1]
 
     def _run(self, image, bicubic):
         """What `sess.run(self.y_, {x:[1,h,w,1], x2:[1,sh,sw,1], dropout:1, is_training:0})` returned."""
@@ -752,7 +797,19 @@ class SuperResolution:
                 "true_y": util.convert_rgb_to_y(true_image) if color else true_image}
 
     def do_for_evaluate(self, file_path, print_console=False):
-        """DCSCN.py:672-703: PSNR / SSIM of the super-resolved luma against the ground truth (border = scale)."""
+        """DCSCN.py:672-703: PSNR / SSIM of the super-resolved luma against the ground truth (border = scale).  In a
+        single process the image is decoded here and everything after the decode runs on the device, equal to the host
+        path (_do_for_evaluate_host) bit for bit."""
+        image = self._device_eval_image(file_path) if self._device_evaluation() else None
+        if image is None:
+            return self._do_for_evaluate_host(file_path, print_console)
+        psnr, ssim = self.engine.evaluate_image(image, self.self_ensemble, self.max_value, self.psnr_calc_border_size)
+        if print_console:
+            print("[%s] PSNR:%f, SSIM:%f" % (file_path, psnr, ssim))
+        return psnr, ssim
+
+    def _do_for_evaluate_host(self, file_path, print_console=False):
+        """do_for_evaluate with the inputs and the metric formed on the host (numpy, scipy, Pillow)."""
         s = self._evaluation_set(file_path)
         if s is None:
             return None, None
@@ -799,7 +856,17 @@ class SuperResolution:
         return psnr, ssim
 
     def evaluate_bicubic(self, file_path, print_console=False):
-        """DCSCN.py:705-725: the bicubic baseline through the same metric."""
+        """DCSCN.py:705-725: the bicubic baseline through the same metric (on the device like do_for_evaluate)."""
+        image = self._device_eval_image(file_path) if self._device_evaluation() else None
+        if image is None:
+            return self._evaluate_bicubic_host(file_path, print_console)
+        psnr, ssim = self.engine.evaluate_image(image, 1, self.max_value, self.psnr_calc_border_size, bicubic=True)
+        if print_console:
+            print("PSNR:%f, SSIM:%f" % (psnr, ssim))
+        return psnr, ssim
+
+    def _evaluate_bicubic_host(self, file_path, print_console=False):
+        """evaluate_bicubic on the host."""
         s = self._evaluation_set(file_path)
         if s is None:
             return None, None

@@ -27,6 +27,7 @@
 #include "wgrad_tc.cuh"
 #include "train_ds.cuh"
 #include "tile.cuh"
+#include "eval.cuh"
 
 using namespace dcscn;
 
@@ -261,6 +262,18 @@ struct dcscn_handle {
   DeviceArray<CropJob> crop_jobs;
   DeviceArray<float> crop_f;
   DeviceArray<uint8_t> crop_u8;
+  // evaluation (dcscn_eval_store_set / dcscn_evaluate_image): the decoded test images and their table, the upload of a
+  // host image, the per-image planes (fp32 / uint8 / float64), the SSE accumulators; all separate from the training stores
+  DeviceArray<uint8_t> ev_pixels;
+  std::vector<ImageEntry> ev_host;
+  DeviceArray<uint8_t> ev_upload, ev_u8;
+  DeviceArray<float> ev_f;
+  DeviceArray<double> ev_y64, ev_map;
+  DeviceArray<unsigned long long> ev_acc;
+  std::vector<Event> eval_ev;        // timing events of the last evaluation (option "timing") and the names of its steps
+  int eval_marks = 0;
+  std::string eval_names;
+  bool eval_timed = false;           // the last call that recorded timings was dcscn_evaluate_image
   // Pillow-bicubic resampling tables per (input size, output size) and the float32 intermediate of the two passes
   struct PilTable { int in = 0, out = 0, ksize = 0; DeviceArray<double> k; DeviceArray<int> bounds; };
   std::vector<PilTable> pil_tables;
@@ -1675,6 +1688,7 @@ static int forward_tiled(dcscn_handle* h, const float* x, const float* x2, float
 // Every inference forward: whole-image (forward_impl) unless option workspace_mb is set and the image's workspace
 // would exceed it.
 static int forward_any(dcscn_handle* h, const float* x, const float* x2, float* y, int n, int H, int W, cudaStream_t st) {
+  h->eval_timed = false;
   if (h->workspace_mb <= 0) return forward_impl(h, x, x2, y, n, H, W, st);
   if (n <= 0 || H <= 0 || W <= 0) return fail("forward: bad shape n=%d h=%d w=%d", n, H, W);
   CUDA_TRY(cudaSetDevice(h->cfg.device_id));
@@ -2079,6 +2093,15 @@ int dcscn_set_option(dcscn_handle* h, const char* key, int64_t value) {
 int dcscn_get_timings(dcscn_handle* h, float* ms, int capacity, int* count, char* names, int names_len) {
   if (!h || !count) return fail("dcscn_get_timings: null argument");
   *count = 0;
+  if (h->eval_timed) {   // the last timed call was dcscn_evaluate_image: its steps, the forward or ensemble as one
+    if (h->eval_marks < 2) return 0;
+    CUDA_TRY(cudaEventSynchronize(h->eval_ev[h->eval_marks - 1].get()));
+    const int n = h->eval_marks - 1;
+    for (int i = 0; i < n && i < capacity; ++i) CUDA_TRY(cudaEventElapsedTime(&ms[i], h->eval_ev[i].get(), h->eval_ev[i + 1].get()));
+    *count = n;
+    if (names && names_len > 0) snprintf(names, names_len, "%s", h->eval_names.c_str());
+    return 0;
+  }
   if (h->ev_used < 2) return 0;
   CUDA_TRY(cudaEventSynchronize(h->ev[h->ev_used - 1].get()));
   const int n = h->ev_used - 1;
@@ -2301,6 +2324,182 @@ int dcscn_crop_gather(dcscn_handle* h, const int32_t* crops, int n, int patch_si
   CUDA_TRY(cudaMemcpyAsync(y, h->io_y.get(), hr_px * sizeof(float), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
   return 0;
+}
+
+// ------------------------------------------------------------------------------------------ evaluation ----
+// What DCSCN._evaluation_set -> do(lr, bicubic) -> util.compute_psnr_and_ssim compute for one test image (DCSCN.py:672-703,
+// :705-725), on the device.  The store holds the decoded test images (util.load_image), one upload per test set.
+int dcscn_eval_store_set(dcscn_handle* h, const uint8_t* pixels, int64_t bytes, const int64_t* offsets, const int32_t* heights,
+                         const int32_t* widths, const int32_t* channels, int count) {
+  if (!h || !pixels || !offsets || !heights || !widths || !channels) return fail("dcscn_eval_store_set: null argument");
+  if (count <= 0 || bytes <= 0) return fail("dcscn_eval_store_set: empty store");
+  std::vector<ImageEntry> table((size_t)count);
+  for (int i = 0; i < count; ++i) {
+    if (heights[i] <= 0 || widths[i] <= 0 || (channels[i] != 1 && channels[i] != 3))
+      return fail("dcscn_eval_store_set: image %d is %d x %d x %d (1 or 3 channels expected)", i, heights[i], widths[i], channels[i]);
+    const int64_t size = (int64_t)heights[i] * widths[i] * channels[i];
+    if (offsets[i] < 0 || offsets[i] > bytes - size)
+      return fail("dcscn_eval_store_set: image %d (%lld bytes at offset %lld) lies outside the %lld-byte store", i,
+                  (long long)size, (long long)offsets[i], (long long)bytes);
+    table[i] = ImageEntry{(long long)offsets[i], heights[i], widths[i], channels[i]};
+  }
+  CUDA_TRY(cudaSetDevice(h->cfg.device_id));
+  h->ev_host.clear();
+  if (h->ev_pixels.alloc((size_t)bytes)) return 1;
+  CUDA_TRY(cudaMemcpy(h->ev_pixels.get(), pixels, (size_t)bytes, cudaMemcpyHostToDevice));
+  h->ev_host = std::move(table);
+  return 0;
+}
+
+static int eval_mark(dcscn_handle* h, const char* name, cudaStream_t st) {
+  if (!h->timing) return 0;
+  if (h->eval_marks >= (int)h->eval_ev.size()) {
+    cudaEvent_t e;
+    CUDA_TRY(cudaEventCreate(&e));
+    h->eval_ev.emplace_back(e);
+  }
+  CUDA_TRY(cudaEventRecord(h->eval_ev[h->eval_marks++].get(), st));
+  if (name) h->eval_names += (h->eval_names.empty() ? "" : ",") + std::string(name);
+  return 0;
+}
+
+static int evaluate_impl(dcscn_handle* h, const EvalImage& im, int lh, int lw, int flips, double max_value, int border,
+                         const double* ssim_params, uint64_t* sse, int64_t* pixels, int64_t* nan_pixels, double* ssim_map,
+                         int64_t map_capacity) {
+  const int s = h->cfg.scale;
+  const int ah = im.height / s * s, aw = im.width / s * s;   // util.set_image_alignment
+  if (ah <= 0 || aw <= 0) return fail("evaluate_image: a %d x %d image is smaller than the scale %d", im.height, im.width, s);
+  if ((long long)lh * s != ah || (long long)lw * s != aw)
+    return fail("evaluate_image: an LR image of %d x %d does not up-scale to the aligned %d x %d at scale %d", lh, lw, ah, aw, s);
+  if (flips < 0 || flips > 8) return fail("evaluate_image: flips must be 0 (bicubic) or 1..8 (got %d)", flips);
+  if (!(max_value > 0.0)) return fail("evaluate_image: max_value must be positive (got %g)", max_value);
+  const int b = border > 0 ? border : 0;                   // the host shaves only a positive border
+  const int hs = std::max(ah - 2 * b, 0), ws = std::max(aw - 2 * b, 0);
+  const int64_t map_n = hs >= 11 ? (int64_t)(hs - 10) * ws : 0;
+  if (map_n > 0 && (!ssim_map || !ssim_params || map_capacity < map_n))
+    return fail("evaluate_image: the SSIM map needs %lld doubles and the filter weights (capacity %lld)", (long long)map_n,
+                (long long)map_capacity);
+  CUDA_TRY(cudaSetDevice(h->cfg.device_id));
+  const size_t hr = (size_t)ah * aw, lr = (size_t)lh * lw;
+  // fp32 planes: truth, mode-'F' input, down-scaled, up-scaled, x, x2, forward output, trimmed output (16-byte aligned)
+  auto up = [](size_t n) { return (n + 63) & ~(size_t)63; };
+  const size_t fsz[8] = {hr, hr, lr, hr, lr, hr, hr, hr};
+  size_t foff[8], ftotal = 0;
+  for (int i = 0; i < 8; ++i) { foff[i] = ftotal; ftotal += up(fsz[i]); }
+  // uint8 planes: mode-'L' input, horizontal pass down, down-scaled, horizontal pass up, up-scaled
+  const size_t usz[5] = {hr, (size_t)ah * lw, lr, (size_t)lh * aw, hr};
+  size_t uoff[5], utotal = 0;
+  for (int i = 0; i < 5; ++i) { uoff[i] = utotal; utotal += up(usz[i]); }
+  const bool rgb = im.channels == 3;
+  if (h->ev_f.grow(ftotal) || (!rgb && h->ev_u8.grow(utotal)) || (flips > 1 && h->ev_y64.grow(hr)) ||
+      (map_n > 0 && h->ev_map.grow((size_t)map_n)) || h->ev_acc.grow(2))
+    return 1;
+  float* F = h->ev_f.get();
+  float *truth = F + foff[0], *f_in = F + foff[1], *f_small = F + foff[2], *f_big = F + foff[3];
+  float *x = F + foff[4], *x2 = F + foff[5], *y32 = F + foff[6], *out = F + foff[7];
+  uint8_t* U = h->ev_u8.get();
+  uint8_t *l_in = rgb ? nullptr : U + uoff[0], *l_t1 = rgb ? nullptr : U + uoff[1], *l_small = rgb ? nullptr : U + uoff[2];
+  uint8_t *l_t2 = rgb ? nullptr : U + uoff[3], *l_big = rgb ? nullptr : U + uoff[4];
+  auto grid = [&](size_t total) { return (int)std::min<size_t>((total + 255) / 256, (size_t)h->sm_count * 16); };
+  cudaStream_t st = 0;
+  h->eval_marks = 0;
+  h->eval_names.clear();
+  if (eval_mark(h, nullptr, st)) return 1;
+
+  // 1. aligned crop, Y and the truth
+  eval_prepare_kernel<<<grid(hr), 256, 0, st>>>(im, ah, aw, truth, f_in, l_in);
+  CUDA_TRY(cudaGetLastError());
+  h->launches++;
+  if (eval_mark(h, "eval_prepare", st)) return 1;
+  // 2. LR = Pillow bicubic down by 1 / scale, bicubic = the LR up by scale (mode 'F' for Y, the 8-bit path for 'L')
+  if (rgb) {
+    if (pil_resize_impl(h, f_in, f_small, 1, ah, aw, lh, lw, st) || pil_resize_impl(h, f_small, f_big, 1, lh, lw, ah, aw, st)) return 1;
+  } else {
+    PilAxis dx, dy, ux, uy;
+    if (pil_axis(h, aw, lw, &dx) || pil_axis(h, ah, lh, &dy) || pil_axis(h, lw, aw, &ux) || pil_axis(h, lh, ah, &uy)) return 1;
+    pil_resample8_h_kernel<<<grid(usz[1]), 256, 0, st>>>(l_in, l_t1, ah, aw, lw, dx);
+    pil_resample8_v_kernel<<<grid(lr), 256, 0, st>>>(l_t1, l_small, 1, ah, lh, lw, dy);
+    pil_resample8_h_kernel<<<grid(usz[3]), 256, 0, st>>>(l_small, l_t2, lh, lw, aw, ux);
+    pil_resample8_v_kernel<<<grid(hr), 256, 0, st>>>(l_t2, l_big, 1, lh, ah, aw, uy);
+    CUDA_TRY(cudaGetLastError());
+    h->launches += 4;
+  }
+  if (eval_mark(h, "eval_resize", st)) return 1;
+  // 3.-4. forward or self-ensemble, then trim_image_as_file of its output (the bicubic baseline trims the up-scale)
+  if (flips > 0) {
+    const double scale = max_value / 255.0;
+    eval_place_kernel<<<grid(lr), 256, 0, st>>>(f_small, l_small, x, (long long)lr, scale);
+    eval_place_kernel<<<grid(hr), 256, 0, st>>>(f_big, l_big, x2, (long long)hr, scale);
+    CUDA_TRY(cudaGetLastError());
+    h->launches += 2;
+    if (eval_mark(h, "eval_place", st)) return 1;
+    if (flips == 1) {
+      if (forward_any(h, x, x2, y32, 1, lh, lw, st)) return 1;
+    } else if (ensemble_impl(h, x, x2, h->ev_y64.get(), lh, lw, (1 << flips) - 1, (double)flips, st)) {
+      return 1;
+    }
+    if (eval_mark(h, flips == 1 ? "forward" : "ensemble", st)) return 1;
+    const double back = 255.0 / max_value;
+    eval_trim_kernel<<<grid(hr), 256, 0, st>>>(flips > 1 ? h->ev_y64.get() : nullptr, flips == 1 ? y32 : nullptr, nullptr, out,
+                                               (long long)hr, back);
+  } else {
+    eval_trim_kernel<<<grid(hr), 256, 0, st>>>(nullptr, rgb ? f_big : nullptr, l_big, out, (long long)hr, 1.0);
+  }
+  CUDA_TRY(cudaGetLastError());
+  h->launches++;
+  if (eval_mark(h, "eval_trim", st)) return 1;
+  // 5. the metric on the region left after shaving the border
+  CUDA_TRY(cudaMemsetAsync(h->ev_acc.get(), 0, 2 * sizeof(unsigned long long), st));
+  if ((size_t)hs * ws > 0) {
+    eval_sse_kernel<<<grid((size_t)hs * ws), 256, 0, st>>>(truth, out, aw, b, hs, ws, h->ev_acc.get());
+    CUDA_TRY(cudaGetLastError());
+    h->launches++;
+    if (eval_mark(h, "eval_sse", st)) return 1;
+  }
+  if (map_n > 0) {
+    EvalSsim p;
+    for (int i = 0; i < 6; ++i) p.w[i] = ssim_params[i];
+    p.c1 = ssim_params[6];
+    p.c2 = ssim_params[7];
+    eval_ssim_kernel<<<grid((size_t)map_n), 256, 0, st>>>(truth, out, aw, b, hs, ws, p, h->ev_map.get());
+    CUDA_TRY(cudaGetLastError());
+    h->launches++;
+    if (eval_mark(h, "eval_ssim", st)) return 1;
+    CUDA_TRY(cudaMemcpyAsync(ssim_map, h->ev_map.get(), (size_t)map_n * sizeof(double), cudaMemcpyDeviceToHost, st));
+  }
+  unsigned long long acc[2];
+  CUDA_TRY(cudaMemcpyAsync(acc, h->ev_acc.get(), sizeof(acc), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  *sse = acc[0];
+  *pixels = (int64_t)hs * ws;
+  *nan_pixels = (int64_t)acc[1];
+  h->eval_timed = h->timing != 0;
+  return 0;
+}
+
+int dcscn_evaluate_image(dcscn_handle* h, int index, const uint8_t* pixels, int height, int width, int channels, int lr_height,
+                         int lr_width, int flips, double max_value, int border, const double* ssim_params, uint64_t* sse,
+                         int64_t* pixel_count, int64_t* nan_pixels, double* ssim_map, int64_t map_capacity) {
+  if (!h || !sse || !pixel_count || !nan_pixels) return fail("dcscn_evaluate_image: null argument");
+  EvalImage im;
+  if (index >= 0) {
+    if (index >= (int)h->ev_host.size())
+      return fail("dcscn_evaluate_image: image %d of an evaluation store of %d (call dcscn_eval_store_set first)", index,
+                  (int)h->ev_host.size());
+    const ImageEntry& e = h->ev_host[index];
+    im = EvalImage{h->ev_pixels.get() + e.offset, e.height, e.width, e.channels};
+  } else {
+    if (!pixels) return fail("dcscn_evaluate_image: null pixels");
+    if (height <= 0 || width <= 0 || (channels != 1 && channels != 3))
+      return fail("dcscn_evaluate_image: the image is %d x %d x %d (1 or 3 channels expected)", height, width, channels);
+    const size_t bytes = (size_t)height * width * channels;
+    CUDA_TRY(cudaSetDevice(h->cfg.device_id));
+    if (h->ev_upload.grow(bytes)) return 1;
+    CUDA_TRY(cudaMemcpyAsync(h->ev_upload.get(), pixels, bytes, cudaMemcpyHostToDevice, 0));
+    im = EvalImage{h->ev_upload.get(), height, width, channels};
+  }
+  return evaluate_impl(h, im, lr_height, lr_width, flips, max_value, border, ssim_params, sse, pixel_count, nan_pixels, ssim_map,
+                       map_capacity);
 }
 
 int dcscn_get_grad(dcscn_handle* h, const char* name, float* host_data, int64_t numel) {

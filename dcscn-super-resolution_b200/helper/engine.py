@@ -8,6 +8,7 @@ library is missing or no H100 is present, construction raises.
 """
 
 import ctypes
+import math
 import os
 
 import numpy as np
@@ -78,6 +79,7 @@ EXPORTED_SYMBOLS = [
     "dcscn_patch_store_set", "dcscn_train_step_indexed", "dcscn_patch_gather", "dcscn_dropout_mask", "dcscn_grad_buffer", "dcscn_apply_gradients", "dcscn_apply_gradients_avg", "dcscn_reset_optimizer", "dcscn_graph_replays",
     "dcscn_tile_halo", "dcscn_optimizer_slot_count", "dcscn_get_optimizer_slot", "dcscn_set_optimizer_slot",
     "dcscn_get_train_tensor", "dcscn_image_store_set", "dcscn_train_step_crops", "dcscn_crop_gather",
+    "dcscn_eval_store_set", "dcscn_evaluate_image",
 ]
 
 _lib = None
@@ -139,6 +141,9 @@ def load_library(path=None):
     lib.dcscn_image_store_set.argtypes = [vp, vp, c64, c64p, i32p, i32p, i32p, ci]
     lib.dcscn_train_step_crops.argtypes = [vp, i32p, ci, ci, cf, cf, u32, ci, fp, fp]
     lib.dcscn_crop_gather.argtypes = [vp, i32p, ci, ci, cf, vp, vp, vp]
+    u64p = ctypes.POINTER(ctypes.c_uint64)
+    lib.dcscn_eval_store_set.argtypes = [vp, vp, c64, c64p, i32p, i32p, i32p, ci]
+    lib.dcscn_evaluate_image.argtypes = [vp, ci, vp, ci, ci, ci, ci, ci, ci, ctypes.c_double, ci, vp, u64p, c64p, c64p, vp, c64]
     lib.dcscn_launch_count.argtypes = [vp]
     lib.dcscn_launch_count.restype = c64
     lib.dcscn_device_bytes.argtypes = [vp]
@@ -174,6 +179,44 @@ def make_config(scale=2, layers=12, filters=196, min_filters=48, filters_decay_g
     c.optimizer, c.momentum = OPTIMIZERS[optimizer], momentum
     c.transposed_upsampler = int(transposed_upsampler)
     return c
+
+
+def eval_geometry(height, width, scale, border):
+    """Sizes of one evaluated image as the host forms them (DCSCN._evaluation_set, util.compute_psnr_and_ssim): the
+    aligned ground truth (util.set_image_alignment), the LR input (util.resize_image_by_pil by 1.0 / scale), its bicubic
+    up-scale and the region left after shaving `border` pixels from each side (border > 0 only).
+    Returns (ah, aw), (lh, lw), (bh, bw), (rh, rw)."""
+    ah, aw = height // scale * scale, width // scale * scale
+    lh, lw = int(ah * (1.0 / scale)), int(aw * (1.0 / scale))
+    bh, bw = int(lh * scale), int(lw * scale)
+    b = border if border > 0 else 0
+    return (ah, aw), (lh, lw), (bh, bw), (max(ah - 2 * b, 0), max(aw - 2 * b, 0))
+
+
+_SSIM_PARAMS = None
+
+
+def ssim_params():
+    """{w0 .. w5, c1, c2} of util._ssim_columns: scipy's gaussian_filter1d(sigma 1.5, truncate 3.5) taps, read off the
+    filter's response to a unit impulse (so they are scipy's own numbers), and the constants (0.01 * 255)^2,
+    (0.03 * 255)^2."""
+    global _SSIM_PARAMS
+    if _SSIM_PARAMS is None:
+        from scipy.ndimage import gaussian_filter1d
+        impulse = np.zeros(11)
+        impulse[5] = 1.0
+        taps = gaussian_filter1d(impulse, 1.5, axis=0, truncate=3.5, mode="reflect")
+        _SSIM_PARAMS = np.ascontiguousarray(np.concatenate([taps[5:], [(0.01 * 255) ** 2, (0.03 * 255) ** 2]]))
+    return _SSIM_PARAMS
+
+
+def finish_psnr(sse, pixels, nan_pixels):
+    """util.compute_psnr_and_ssim's PSNR from the exact squared-error sum: err = sse / n, 10 log10(255^2 / err), inf at
+    err = 0; nan for an empty region or a NaN output pixel (as np.mean gives)."""
+    if nan_pixels or pixels == 0:
+        return float("nan")
+    err = float(sse) / pixels
+    return float("inf") if err == 0 else 10.0 * math.log10(255.0 * 255.0 / err)
 
 
 class Engine:
@@ -417,6 +460,61 @@ class Engine:
                                                float(max_value), x.ctypes.data, x2.ctypes.data, y.ctypes.data))
         return x, x2, y
 
+    # ---- evaluation: test images resident in HBM, inputs and metric formed on the device ----
+    @staticmethod
+    def _pack_images(images):
+        arrays = [np.ascontiguousarray(np.atleast_3d(a), dtype=np.uint8) for a in images]
+        shapes = np.array([a.shape for a in arrays], dtype=np.int64).reshape(-1, 3)
+        sizes = np.array([a.size for a in arrays], dtype=np.int64)
+        offsets = np.ascontiguousarray(np.concatenate([[0], np.cumsum(sizes)[:-1]]), dtype=np.int64)
+        pixels = np.concatenate([a.reshape(-1) for a in arrays]) if arrays else np.zeros(0, np.uint8)
+        heights, widths, channels = (np.ascontiguousarray(shapes[:, k], dtype=np.int32) for k in range(3))
+        return pixels, offsets, heights, widths, channels
+
+    def set_eval_images(self, images):
+        """Decoded uint8 test images [h, w, 3] (RGB) or [h, w(, 1)] (mode 'L'), as util.load_image returns them -> the
+        device evaluation store, once per test set.  evaluate_image(i, ...) evaluates image i of this list.  The training
+        stores are not touched."""
+        pixels, offsets, heights, widths, channels = self._pack_images(images)
+        i32 = ctypes.POINTER(ctypes.c_int32)
+        self._check(self.lib.dcscn_eval_store_set(self.handle, pixels.ctypes.data, int(pixels.size),
+                                                  offsets.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)),
+                                                  heights.ctypes.data_as(i32), widths.ctypes.data_as(i32),
+                                                  channels.ctypes.data_as(i32), len(heights)))
+        self._eval_shapes = [tuple(int(v) for v in t) for t in zip(heights, widths, channels)]
+
+    def evaluate_image(self, image, flips, max_value, border, bicubic=False):
+        """(PSNR, SSIM) of one test image, equal to the host's DCSCN.do_for_evaluate (or evaluate_bicubic with bicubic=True)
+        at self_ensemble = flips: image i of the evaluation store (an int) or a decoded uint8 image (util.load_image).
+        The device forms the luma, the LR / bicubic inputs, the forward or self-ensemble, the trimmed output, the exact
+        squared-error sum and the SSIM map; the host finishes PSNR and the numpy mean of the map."""
+        s = int(self.config.scale)
+        if isinstance(image, (int, np.integer)):
+            index, ptr, a = int(image), None, None
+            if not 0 <= index < len(getattr(self, "_eval_shapes", ())):
+                raise EngineError("evaluate_image: no image %d in the evaluation store" % index)
+            h, w, c = self._eval_shapes[index]
+        else:
+            a = np.atleast_3d(np.asarray(image))
+            if a.dtype != np.uint8:
+                raise EngineError("evaluate_image: a decoded uint8 image is expected, got %s" % a.dtype)
+            a = np.ascontiguousarray(a)
+            index, ptr = -1, a.ctypes.data
+            h, w, c = a.shape
+        _, (lh, lw), _, (rh, rw) = eval_geometry(h, w, s, border)
+        rows = rh - 10 if rh >= 11 else 0
+        ssim_map = np.empty((rows, rw), np.float64)
+        sse, pixels, nans = ctypes.c_uint64(), ctypes.c_int64(), ctypes.c_int64()
+        params = ssim_params()
+        self._check(self.lib.dcscn_evaluate_image(self.handle, index, ptr, h, w, c, lh, lw, 0 if bicubic else max(int(flips), 1),
+                                                  float(max_value), int(border), params.ctypes.data, ctypes.byref(sse),
+                                                  ctypes.byref(pixels), ctypes.byref(nans), ssim_map.ctypes.data,
+                                                  int(ssim_map.size)))
+        psnr = finish_psnr(int(sse.value), int(pixels.value), int(nans.value))
+        # the host's np.mean(s[5:-5, :]) of a contiguous slice of this shape: the same reduction, bit for bit
+        ssim = float(np.mean(ssim_map)) if rows > 0 and rw > 0 else float("nan")
+        return psnr, ssim
+
     def train_step_host(self, x, x2, y, lr, seed, apply_update=True):
         """One optimisation step on host fp32 arrays x [n,h,w,1], x2 / y [n,sh,sw,1]; returns (image_loss, mse)."""
         xa, x2a, ya = _host_array(x), _host_array(x2), _host_array(y)
@@ -570,7 +668,8 @@ class Engine:
         return int(r.value)
 
     def timings(self):
-        """[(launch name, ms)] of the last forward (needs set_option("timing", 1) before it)."""
+        """[(launch name, ms)] of the last forward, or of the steps of the last evaluate_image call when that came
+        after it (needs set_option("timing", 1) before it)."""
         cap = 64
         while True:   # a tiled forward has one sequence of launches per batch of windows
             ms = (ctypes.c_float * cap)()

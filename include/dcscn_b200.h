@@ -292,13 +292,44 @@ int dcscn_get_train_tensor(dcscn_handle* h, const char* name, float* host_data, 
 int dcscn_set_option(dcscn_handle* h, const char* key, int64_t value);
 /* With option "timing" = 1 every launch of a forward is bracketed by CUDA events on its stream; this returns the
  * device time in ms of each launch of the LAST forward (in launch order) and their comma-separated names.  A tiled
- * forward lists tile_gather, its layers and tile_stitch once per batch of windows. */
+ * forward lists tile_gather, its layers and tile_stitch once per batch of windows.  After dcscn_evaluate_image it lists
+ * that call's steps instead (see there), until the next forward. */
 int dcscn_get_timings(dcscn_handle* h, float* ms, int capacity, int* count, char* names, int names_len);
 /* LR pixels of context a window of a tiled forward carries around its core (option "workspace_mb"): the receptive
  * radius of the graph, walked back from R-CNN1 at HR resolution (15 for the 12-layer 3x3 graphs, 10 for 7 layers).
  * A core computed with this much context is bit-identical to the same pixels of the whole-image forward, which also
  * lets a caller split one image over several GPUs. */
 int dcscn_tile_halo(dcscn_handle* h, int* lr_pixels);
+/*
+ * Evaluation on the device (reference DCSCN.py:672-703 do_for_evaluate, :705-725 evaluate_bicubic): one call computes
+ * for one test image what _evaluation_set -> do(lr, bicubic) -> util.compute_psnr_and_ssim compute on the host, bit for
+ * bit.  dcscn_eval_store_set copies decoded uint8 test images (layout of dcscn_image_store_set) into HBM once; it
+ * replaces the previous evaluation store and touches neither the training stores nor anything else.
+ * dcscn_evaluate_image evaluates image `index` of that store, or with index < 0 the height x width x channels image at
+ * host `pixels`:
+ *   1. crop to the top-left (height / s * s) x (width / s * s) pixels; RGB becomes the float64 Y of
+ *      util.convert_rgb_to_y, the truth clip(rint(Y), 0, 255); a mode-'L' pixel is its own truth;
+ *   2. LR = Pillow bicubic down to lr_height x lr_width (the host's int(side * (1.0 / s)), passed in; it must up-scale
+ *      back to the aligned size), bicubic = the LR up by s: mode 'F' for Y, Pillow's 8-bit path for 'L';
+ *   3. flips 1..8: both multiplied by max_value / 255 under numpy's dtype rules, then the forward (flips = 1) or the
+ *      self-ensemble of the first `flips` transforms; the output times 255 / max_value (fp32 for one flip, float64 for
+ *      the ensemble mean), rint, clip to [0, 255].  flips = 0: the bicubic up-scale itself, rint, clip (no forward);
+ *   4. on the region left after shaving `border` pixels from each side (border > 0 only): *sse = the exact sum of
+ *      squared differences of the integer-valued planes over the non-NaN output pixels, *pixel_count = the region's
+ *      pixels, *nan_pixels = its NaN output pixels; and when the region has at least 11 rows, rows 5 .. rows - 6 of
+ *      util._ssim_columns' SSIM map ((rows - 10) x columns float64, row-major) into ssim_map, which must hold that many.
+ *      ssim_params = {w0, w1, .. w5, c1, c2}: the centre and side taps of scipy's gaussian_filter1d(sigma 1.5,
+ *      truncate 3.5) and the SSIM constants.  The caller finishes PSNR = 10 log10(255^2 / (sse / pixel_count)) and
+ *      SSIM = the numpy mean of the map rows.
+ * The planes are the handle's own; option "workspace_mb" tiles the forward as usual.  With option "timing" = 1,
+ * dcscn_get_timings then lists eval_prepare, eval_resize, eval_place, forward (or ensemble), eval_trim, eval_sse,
+ * eval_ssim (the steps that ran), until the next forward.
+ */
+int dcscn_eval_store_set(dcscn_handle* h, const uint8_t* pixels, int64_t bytes, const int64_t* offsets, const int32_t* heights,
+                         const int32_t* widths, const int32_t* channels, int count);
+int dcscn_evaluate_image(dcscn_handle* h, int index, const uint8_t* pixels, int height, int width, int channels, int lr_height,
+                         int lr_width, int flips, double max_value, int border, const double* ssim_params, uint64_t* sse,
+                         int64_t* pixel_count, int64_t* nan_pixels, double* ssim_map, int64_t map_capacity);
 /* Number of kernels this handle has launched so far (bench.py "gpu_launches"). */
 int64_t dcscn_launch_count(dcscn_handle* h);
 /* Forwards served by a CUDA-graph replay so far (option "graph"). */
