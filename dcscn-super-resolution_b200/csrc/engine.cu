@@ -424,7 +424,9 @@ static int build_graph(dcscn_handle* h) {
   if (!c.use_nin) return fail("use_nin=false is not supported (no shipped checkpoint uses it)");
   if (c.channels != 1) return fail("channels must be 1 (helper/args.py: 'Now it should be 1')");
   if (std::max(c.reconstruct_layers, 1) != 1) return fail("reconstruct_layers > 1 is not supported");
-  if (c.scale < 2 || c.scale > 4) return fail("scale must be 2, 3 or 4");
+  // x4 is two x2 stages; every other factor is one Up-PS / Up-TCNN into s*s columns (DCSCN.py:293-311).  x8 is the
+  // largest factor the tests verify.
+  if (c.scale < 2 || c.scale > 8) return fail("scale must be in 2..8 (got %d)", c.scale);
   if (c.cnn_size != 3 && c.cnn_size != 1 && c.cnn_size != 5) return fail("cnn_size %d is not supported", c.cnn_size);
   if (c.layers < 2) return fail("layers must be >= 2");
 
@@ -504,7 +506,7 @@ static bool ds_split(const dcscn_handle* h, const LayerDef& l) {
 // Index in Up-TCNN/Tconv_W W[K][K][C][C] ([h, w, out, in]) behind every entry of its 3x3 LR filter
 // F[3][3][C][s*s*C] (HWIO), or -1 for a structural zero.  With SAME padding, pad_top = (K - s) / 2 and
 //   out[s*m + p] = sum_d in[m + d] * W[p + pad_top - s*d]   per axis,
-// and for s = 2, 3, 4 every used offset d lies in {-1, 0, 1}: F[dy+1][dx+1][ci][(py*s + px)*C + co] =
+// and for every s >= 2 every used offset d lies in {-1, 0, 1}: F[dy+1][dx+1][ci][(py*s + px)*C + co] =
 // W[py + pad_top - s*dy][px + pad_top - s*dx][co][ci].  (phase, offset) -> tap is a bijection onto [0, K), so each
 // W entry appears in F exactly once and the map inverts without sums (tconv gradient, train_engine.inc).
 static std::vector<int> tconv_filter_map(int s, int C) {

@@ -137,7 +137,7 @@ flags = _FlagModule()
 # the default's Python type.
 _REFERENCE_FLAGS = [
     # --- network ---
-    ("scale", 2, "upscaling factor: 2, 3 or 4"),
+    ("scale", 2, "upscaling factor, 2 to 8"),
     ("layers", 12, "depth of the feature-extraction stack (CNN1..CNNn)"),
     ("filters", 196, "output channels of CNN1"),
     ("min_filters", 48, "output channels of the last feature-extraction layer"),

@@ -68,7 +68,7 @@ enum {
  */
 typedef struct dcscn_config {
   int32_t struct_size;            /* sizeof(dcscn_config), for ABI checking */
-  int32_t scale;                  /* --scale (2, 3 or 4) */
+  int32_t scale;                  /* --scale, 2..8: x4 is two x2 pixel-shuffler stages, every other factor one */
   int32_t layers;                 /* --layers */
   int32_t filters;                /* --filters */
   int32_t min_filters;            /* --min_filters */
