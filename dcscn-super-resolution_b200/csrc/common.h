@@ -22,6 +22,8 @@ enum EpilogueMode : int {
   EPI_D2S_PLANES = 2,  // depth_to_space scatter into fp16 hi/lo planes
   EPI_D2S_RDOT = 3,    // depth_to_space fused with the per-pixel half of the final cout=1 conv (R-CNN1):
                        // writes, per HR pixel and filter tap, dot(h[pixel, :], w_last[tap, :])
+  EPI_D2S_TAPS = 4,    // the same tap-planar values from a layer folded with R-CNN1 (engine.cu build_fold): column
+                       // ij * rdot_taps + t of sub-pixel ij is tap t, stored at rdot_out[t][N][rH][rW]
 };
 
 // Point-wise activation of CNN1..CNNL, A1, B1 and B2 (--activator, tf_graph.py:77-102); values of DCSCN_ACTIVATOR_*.
@@ -62,7 +64,8 @@ struct EpiParams {
   int d2s_cout;        // channels after depth_to_space
   float* dst_f32;      // EPI_D2S_F32 destination [N, r*H, r*W, d2s_pitch]
   int d2s_pitch;
-  // EPI_D2S_RDOT: final conv weights [taps][d2s_cout] and tap-planar output [taps][N][rH][rW]
+  // EPI_D2S_RDOT: final conv weights [taps][d2s_cout] and tap-planar output [taps][N][rH][rW] (EPI_D2S_TAPS: the output
+  // and rdot_taps only)
   const float* rdot_w;
   float* rdot_out;
   int rdot_taps;

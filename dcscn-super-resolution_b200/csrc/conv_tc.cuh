@@ -336,7 +336,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
               if (last && valid) rdot_flush(p.epi, g, img, y, x, ij, p.epi.rdot_parts > 1 ? cc / (per * 16) : 0, v9);
             }
           } else if (valid) {
-            epilogue_store16(p.epi, g, n_total, img, y, x, cg, v);
+            if (p.epi.mode == EPI_D2S_TAPS) taps_store16(p.epi, g, img, y, x, cg, v);
+            else epilogue_store16(p.epi, g, n_total, img, y, x, cg, v);
           }
         }
       }

@@ -169,6 +169,7 @@ struct GatherJob {   // training: dst[i] = d_w[map[i]] where map[i] >= 0 (biases
 struct TcLaunch {
   int layer_index = -1;          // index into dcscn_handle::tcl (forward) or ::bwd (dgrad twins): the layer whose CURRENT
   bool layer_bwd = false;        // power-of-two weight scale the epilogue has to undo (it changes when a layer is re-packed)
+  bool layer_fold = false;       // the layer is dcscn_handle::fold
   CUtensorMap tm_hi, tm_lo;
   ConvTCParams p;
   ConvRefParams ref;
@@ -224,6 +225,7 @@ struct dcscn_handle {
   // packed layers
   std::vector<TcLayer> tcl;          // CNN2..CNNL, A1+B1, B2, Up-PS [, Up-PS2]
   std::vector<TcLayer> bwd;          // data-gradient twins (transposed, flipped filters), see build_bwd_layers
+  TcLayer fold;                      // the last depth_to_space layer folded with R-CNN1 (build_fold; cout == 0: none)
   bool train_enabled = false;
   DeviceArray<float> ens_x, ens_x2, ens_y;   // self-ensemble: transformed copies / per-flip outputs
   DeviceArray<float> ensio_x, ensio_x2;      // host-call staging of the ensemble entry point
@@ -813,12 +815,89 @@ static int construct_tc_layers(dcscn_handle* h) {
   return 0;
 }
 
+// Partial plane sets of the fused R-CNN1 epilogue: an epilogue thread owns n_pad / kColSplit GEMM columns; when that share
+// is a fraction of one sub-pixel's `cout` channels, `cout / share` threads each write their own tap-planar partials.
+static int rdot_parts(int n_pad, int cout) {
+  const int nch = n_pad >> 4, per16 = ((nch + kColSplit - 1) / kColSplit) * 16;
+  if (cout <= 0 || per16 % cout == 0) return 1;
+  return (cout % per16 == 0) ? cout / per16 : 1;
+}
+
+// Whether get_plan fuses R-CNN1 into the last depth_to_space layer, whose column tiles are n_pad wide: a 3x3 R-CNN1 and
+// epilogue threads that own whole sub-pixels or an equal share of one.
+static bool last_fuses(const dcscn_handle* h, int n_pad) {
+  const int cout = h->ps_out, nch = n_pad >> 4, per = (nch + kColSplit - 1) / kColSplit;
+  return find_layer(h, "R-CNN1")->k == 3 && cout % 16 == 0 && cout <= 128 && nch % kColSplit == 0 &&
+         ((per * 16) % cout == 0 || (rdot_parts(n_pad, cout) > 1 && n_pad % (per * 16) == 0));
+}
+
+// sum over c of a[c] w[c]: exact products of fp32 values, added in fp64 in ascending c.  fold_kernel (train.cuh) forms
+// the same sum, so host and device folds round to the same fp32 value.
+static double fold_dot(const float* a, const float* w, int C) {
+  double s = 0.0;
+  for (int c = 0; c < C; ++c) s += (double)a[c] * (double)w[c];
+  return s;
+}
+
+// The shape of the fold of `up` (s^2 sub-pixels of C channels) with a 3x3 R-CNN1: s^2 * 9 columns in `up`'s column-tile
+// width, same input, taps and depthwise step; no activation.
+static TcLayer fold_shape(const TcLayer& up, int C) {
+  TcLayer f;
+  f.name = up.name;
+  f.ksz = up.ksz;
+  f.cin = up.cin;
+  f.cin_pad = up.cin_pad;
+  f.in_map = up.in_map;
+  f.cout = f.n_valid = up.cout / C * 9;
+  f.n_pad = up.n_pad;
+  f.n_tiles = (f.cout + f.n_pad - 1) / f.n_pad;
+  f.w_host.assign((size_t)f.ksz * f.ksz * f.cin * f.cout, 0.f);
+  f.bias_host.assign((size_t)f.n_tiles * f.n_pad, 0.f);
+  f.alpha_host.assign((size_t)f.n_tiles * f.n_pad, 1.f);
+  f.dw_ksz = up.dw_ksz;
+  f.dw_host = up.dw_host;
+  return f;
+}
+
+// The last depth_to_space layer (Up-PS, Up-PS2 at x4, Up-TCNN) and R-CNN1 are both linear at inference, so where get_plan
+// fuses them and the operands are f16x3, R-CNN1's reduction over the C channels of a sub-pixel is done once, on the
+// weights:
+//   W'[tap][ci][ij * 9 + t] = sum_c W[tap][ci][ij * C + c] w_r[t][c],   b'[ij * 9 + t] = sum_c b[ij * C + c] w_r[t][c]
+// and the layer computes s^2 * 9 columns instead of s^2 * C.  Column (ij, t) at LR pixel (y, x) is R-CNN1 tap t's
+// product at HR pixel (s y + i, s x + j), the value EPI_D2S_RDOT writes.  f16x1 keeps EPI_D2S_RDOT: that mode is each
+// layer on its own fp16-rounded weights, and a folded filter rounded to fp16 would be a different quantised model.
+static void build_fold(dcscn_handle* h) {
+  h->fold = TcLayer();
+  const TcLayer& up = h->tcl.back();
+  if (planes(h) != 2 || !last_fuses(h, up.n_pad)) return;
+  std::vector<float> tmp;
+  const std::vector<float>& wr = layer_filter(h, *find_layer(h, "R-CNN1"), tmp);   // [9][C]
+  const int C = h->ps_out, sub = up.cout / C;
+  TcLayer f = fold_shape(up, C);
+  const size_t rows = (size_t)up.ksz * up.ksz * up.cin;
+  for (size_t r = 0; r < rows; ++r)
+    for (int ij = 0; ij < sub; ++ij)
+      for (int t = 0; t < 9; ++t)
+        f.w_host[r * f.cout + ij * 9 + t] = (float)fold_dot(&up.w_host[r * up.cout + (size_t)ij * C], &wr[(size_t)t * C], C);
+  for (int ij = 0; ij < sub; ++ij)
+    for (int t = 0; t < 9; ++t) f.bias_host[ij * 9 + t] = (float)fold_dot(&up.bias_host[(size_t)ij * C], &wr[(size_t)t * C], C);
+  h->fold = std::move(f);
+}
+
+// A re-built layer keeps the device allocations of its previous packing.
+static void adopt_arrays(TcLayer& t, TcLayer& old) {
+  t.d_wpack = std::move(old.d_wpack); t.d_bias = std::move(old.d_bias); t.d_alpha = std::move(old.d_alpha);
+  t.d_wref = std::move(old.d_wref); t.d_in_map = std::move(old.d_in_map); t.d_img_map = std::move(old.d_img_map);
+  t.d_dw = std::move(old.d_dw);
+}
+
 static int finalize_params(dcscn_handle* h) {
   const dcscn_config& c = h->cfg;
   if (sync_host_params(h)) return 1;
   if (uses_ds_tile(h)) return finalize_params_ds(h);
   std::vector<TcLayer> old_tcl = std::move(h->tcl);
   std::vector<TcLayer> old_bwd = std::move(h->bwd);
+  TcLayer old_fold = std::move(h->fold);
   h->tcl.clear();
   h->bwd.clear();
   h->refresh_ready = false;
@@ -834,16 +913,17 @@ static int finalize_params(dcscn_handle* h) {
   auto repack = [&](std::vector<TcLayer>& cur, std::vector<TcLayer>& old) {
     for (size_t i = 0; i < cur.size(); ++i) {
       TcLayer& t = cur[i];
-      if (i < old.size()) {
-        t.d_wpack = std::move(old[i].d_wpack); t.d_bias = std::move(old[i].d_bias); t.d_alpha = std::move(old[i].d_alpha);
-        t.d_wref = std::move(old[i].d_wref); t.d_in_map = std::move(old[i].d_in_map); t.d_img_map = std::move(old[i].d_img_map);
-        t.d_dw = std::move(old[i].d_dw);
-      }
+      if (i < old.size()) adopt_arrays(t, old[i]);
       if (pack_tc_layer(h, t, &moved)) return 1;
     }
     return 0;
   };
   if (repack(h->tcl, old_tcl) || repack(h->bwd, old_bwd)) return 1;
+  build_fold(h);
+  if (h->fold.cout > 0) {
+    adopt_arrays(h->fold, old_fold);
+    if (pack_tc_layer(h, h->fold, &moved)) return 1;
+  }
   // R-CNN1 (CUDA cores): [taps][C]
   {
     std::vector<float> tmp;
@@ -856,14 +936,6 @@ static int finalize_params(dcscn_handle* h) {
   h->graph_epoch++;          // captured launches bake the epilogue's 1 / weight-scale
   h->params_dirty = false;
   return 0;
-}
-
-// Partial plane sets of the fused R-CNN1 epilogue: an epilogue thread owns n_pad / kColSplit GEMM columns; when that share
-// is a fraction of one sub-pixel's `cout` channels, `cout / share` threads each write their own tap-planar partials.
-static int rdot_parts(int n_pad, int cout) {
-  const int nch = n_pad >> 4, per16 = ((nch + kColSplit - 1) / kColSplit) * 16;
-  if (cout <= 0 || per16 % cout == 0) return 1;
-  return (cout % per16 == 0) ? cout / per16 : 1;
 }
 
 // ----------------------------------------------------------------------------------- workspace ----
@@ -1194,9 +1266,24 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
     const int parts = rdot_parts(L.p.n_pad, cout);
     pl->unfused = L;
     pl->fused_index = (int)pl->tc.size() - 1;
-    pl->fused_last = (klast == 3) && (cout % 16 == 0) && (cout <= 128) && (nch % kColSplit == 0) &&
-                     (((per * 16) % cout == 0) || (parts > 1 && L.p.n_pad % (per * 16) == 0));
-    if (pl->fused_last) {
+    pl->fused_last = last_fuses(h, L.p.n_pad);
+    if (pl->fused_last && h->fold.cout > 0) {
+      // the folded layer (build_fold): same input, patch, rings and column-tile width, fewer column tiles
+      const TcLayer& f = h->fold;
+      L.layer_index = -1;
+      L.layer_fold = true;
+      L.p.n_tiles = f.n_tiles;
+      L.p.wpack = f.d_wpack.get();
+      L.p.epi.bias = f.d_bias.get();
+      L.p.epi.alpha = f.d_alpha.get();
+      L.p.epi.out_scale = 1.0f / f.wscale;
+      L.p.epi.n_valid = f.n_valid;
+      L.p.epi.mode = EPI_D2S_TAPS;
+      L.p.epi.rdot_out = h->vbuf.get();
+      L.p.epi.rdot_taps = 9;
+      L.p.epi.rdot_parts = 1;
+      L.grid = (int)std::min<long long>((long long)n * L.p.g.tiles_x * L.p.g.tiles_y * f.n_tiles, h->sm_count);
+    } else if (pl->fused_last) {
       L.p.epi.rdot_parts = ((per * 16) % cout == 0) ? 1 : parts;
       L.p.epi.mode = EPI_D2S_RDOT;
       L.p.epi.rdot_w = h->d_last_w.get();
@@ -1261,7 +1348,9 @@ static int launch_tc(dcscn_handle* h, const TcLaunch& Lc, cudaStream_t st) {
   // Cached plans outlive weight re-packs.  A re-pack keeps the device allocations (so the plan's pointers stay valid) but
   // may choose a different power-of-two weight scale: take the epilogue's 1 / scale from the layer as it is NOW.
   TcLaunch& L = const_cast<TcLaunch&>(Lc);
-  if (L.layer_index >= 0) {
+  if (L.layer_fold) {
+    L.p.epi.out_scale = 1.0f / h->fold.wscale;
+  } else if (L.layer_index >= 0) {
     const std::vector<TcLayer>& ls = L.layer_bwd ? h->bwd : h->tcl;
     if (L.layer_index < (int)ls.size()) L.p.epi.out_scale = 1.0f / ls[L.layer_index].wscale;
   }
@@ -2033,6 +2122,11 @@ int dcscn_get_activation(dcscn_handle* h, const char* tensor, float* host_data, 
     return fail("dcscn_get_activation: '%s' is not materialised when the R-CNN1 fusion is on (set option fuse_last=0)", tensor);
   } else if (t == (tconv(h) ? "Up-TCNN" : two_stage_up(h) ? "Up-PS2" : "Up-PS")) {
     f32 = h->hr.get(); pitch = h->ps_out; ch = h->ps_out; px *= (size_t)c.scale * c.scale;
+  } else if (t == "R-CNN1/taps" && pl->ran_fused) {   // the fused R-CNN1's tap-planar products [parts][9][N][sH][sW]
+    const size_t count = px * c.scale * c.scale * 9 * pl->gather.parts;
+    if (numel != (int64_t)count) return fail("dcscn_get_activation: '%s' has %lld elements, got %lld", tensor, (long long)count, (long long)numel);
+    CUDA_TRY(cudaMemcpy(host_data, h->vbuf.get(), count * sizeof(float), cudaMemcpyDeviceToHost));
+    return 0;
   } else {
     return fail("dcscn_get_activation: no tensor '%s'", tensor);
   }

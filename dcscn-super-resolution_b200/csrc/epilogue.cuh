@@ -248,4 +248,28 @@ __device__ __forceinline__ void rdot_flush(const EpiParams& e, const ConvGeom& g
   rdot_flush(e, g, img, y, x, ij, 0, v);
 }
 
+// EPI_D2S_TAPS: 16 linear (bias only) columns of the folded last upsampler, column ij * taps + t = R-CNN1 tap t of
+// sub-pixel ij, stored element-wise into the tap-planar layout rdot_flush writes (one partial set).
+__device__ __forceinline__ void taps_store16(const EpiParams& e, const ConvGeom& g, int img, int y, int x, int cg,
+                                             const float (&acc)[16]) {
+  const int r = e.d2s_r, taps = e.rdot_taps;
+  const size_t HR_H = (size_t)g.H * r, HR_W = (size_t)g.W * r;
+  const size_t plane = (size_t)g.n_img * HR_H * HR_W;
+  const float4* b4 = reinterpret_cast<const float4*>(e.bias + cg);
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const float4 b = __ldg(b4 + q);
+    const float bq[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int col = cg + 4 * q + u;
+      if (col >= e.n_valid) continue;
+      const int ij = col / taps, tap = col - ij * taps;
+      const int i = ij / r, j = ij - i * r;
+      const size_t pix = ((size_t)img * HR_H + (size_t)(y * r + i)) * HR_W + (size_t)(x * r + j);
+      e.rdot_out[(size_t)tap * plane + pix] = fmaf(acc[4 * q + u], e.out_scale, bq[u]);
+    }
+  }
+}
+
 }  // namespace dcscn

@@ -906,6 +906,42 @@ __global__ void __launch_bounds__(256) repack_kernel(const RepackParams p) {
   if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(p.wmax, __float_as_uint(m));
 }
 
+// The folded last upsampler (engine.cu build_fold) from the master weights:
+//   wf[r][ij * 9 + t] = sum_c W[r][ij * C + c] w_r[t][c]  for the filter rows r = (tap, ci),
+//   bf[ij * 9 + t]    = sum_c b[ij * C + c] w_r[t][c]
+// exact fp32 products added in fp64, c ascending, rounded once: the bits fold_dot gives on the host.  The maps hold
+// each W / w_r / b element's index in the master weights (-1 = structural zero).
+struct FoldParams {
+  const float* w;
+  const int* wu_map;   // [rows][sub * C]
+  const int* wr_map;   // [9][C]
+  const int* bu_map;   // [sub * C]
+  int rows, sub, C;
+  float* wf;           // [rows][sub * 9], read by repack_kernel through the folded layer's image map
+  float* bf;           // [sub * 9], the folded layer's bias
+};
+
+__global__ void __launch_bounds__(256) fold_kernel(const FoldParams p) {
+  const int cols = p.sub * 9;
+  const long long n = (long long)(p.rows + 1) * cols;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const int col = (int)(i % cols);
+    const long long r = i / cols;
+    const int ij = col / 9, t = col - ij * 9;
+    const int* am = (r < p.rows ? p.wu_map + (size_t)r * p.sub * p.C : p.bu_map) + (size_t)ij * p.C;
+    const int* wm = p.wr_map + (size_t)t * p.C;
+    double s = 0.0;
+    for (int c = 0; c < p.C; ++c) {
+      const int ia = __ldg(am + c), iw = __ldg(wm + c);
+      const float a = ia >= 0 ? __ldg(p.w + ia) : 0.f;
+      const float b = iw >= 0 ? __ldg(p.w + iw) : 0.f;
+      s += (double)a * (double)b;   // the product is exact in fp64, so a fused multiply-add gives the same sum
+    }
+    if (r < p.rows) p.wf[i] = (float)s;
+    else p.bf[col] = (float)s;
+  }
+}
+
 __global__ void __launch_bounds__(256) gather_params_kernel(const float* __restrict__ w, const int* __restrict__ map,
                                                             float* __restrict__ dst, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;

@@ -233,7 +233,9 @@ int dcscn_dropout_mask(dcscn_handle* h, const char* tensor, uint32_t seed, int n
 /*
  * Parity / debug: output of one layer of the LAST forward as fp32 NHWC [n, H_l, W_l, cout_l]
  * (`tensor` is the reference's self.H entry: "CNN1".."CNNL", "A1", "B1", "B2", "Up-PS", "Up-PS2", or "Up-TCNN"
- * [n, s*H, s*W, C] with cfg.transposed_upsampler).
+ * [n, s*H, s*W, C] with cfg.transposed_upsampler).  After a forward that fused R-CNN1 into the last upsampler,
+ * "R-CNN1/taps" is its tap-planar products [parts, 9, n, s*H, s*W]: R-CNN1 tap t's contribution from each HR pixel,
+ * in `parts` partial sets to be added (1 where the upsampler is folded with R-CNN1, see DESIGN 4.2).
  * Fails after a forward that ran tiled (option "workspace_mb"): the buffers then hold its last batch of windows.
  */
 int dcscn_get_activation(dcscn_handle* h, const char* tensor, float* host_data, int64_t numel);
