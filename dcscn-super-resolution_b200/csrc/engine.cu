@@ -108,6 +108,21 @@ class DeviceArray {
   size_t n_ = 0;
 };
 
+// The hi and lo fp16 planes of one tensor (hi + lo = the value) at some channel offset.  In f16x1 there is no lo plane:
+// lo stays null at every offset.
+struct PlaneView {
+  __half* hi = nullptr;
+  __half* lo = nullptr;
+  PlaneView at(size_t off) const { return {hi ? hi + off : nullptr, lo ? lo + off : nullptr}; }
+};
+struct Planes {
+  DeviceArray<__half> hi, lo;
+  // n zero-filled elements per plane; lo stays empty unless `two`
+  int alloc(size_t n, bool two) { return hi.alloc(n, true) || lo.alloc(two ? n : 0, true); }
+  PlaneView at(size_t off) const { return PlaneView{hi.get(), lo.get()}.at(off); }
+  int64_t bytes() const { return (int64_t)((hi.size() + lo.size()) * sizeof(__half)); }
+};
+
 struct StreamDeleter { void operator()(cudaStream_t s) const { cudaStreamDestroy(s); } };
 struct EventDeleter { void operator()(cudaEvent_t e) const { cudaEventDestroy(e); } };
 using Stream = std::unique_ptr<std::remove_pointer_t<cudaStream_t>, StreamDeleter>;
@@ -166,10 +181,27 @@ struct GatherJob {   // training: dst[i] = d_w[map[i]] where map[i] >= 0 (biases
   int n;
 };
 
+// The buffers a named activation lives in: the fp16 planes dcscn_handle::feat / nin / b1 / mid and the fp32 hr of the
+// tensor-core graphs, or the fp32 ds_* buffers of forward_ds_tile.
+enum ActBuf { BUF_FEAT, BUF_NIN, BUF_B1, BUF_MID, BUF_HR };
+
+// A named activation (act_view): where it lives, and the dropout stream the forward, the backward and the CPU oracles
+// (dcscn_dropout_mask) must agree on.
+struct ActView {
+  ActBuf buf;
+  PlaneView planes;               // tensor-core layouts: the planes at the tensor's first channel
+  const float* f32;               // fp32 buffers: the tensor's first channel
+  int pitch, off, ch;             // channels per pixel of the buffer, the tensor's first channel, its logical channels
+  int px_mul;                     // pixels per LR pixel
+  uint32_t drop_layer;            // dropout stream (0: no dropout); keep-mask element px * drop_stride + drop_col0 + channel
+  int drop_stride, drop_col0;
+};
+
 struct TcLaunch {
   int layer_index = -1;          // index into dcscn_handle::tcl (forward) or ::bwd (dgrad twins): the layer whose CURRENT
   bool layer_bwd = false;        // power-of-two weight scale the epilogue has to undo (it changes when a layer is re-packed)
   bool layer_fold = false;       // the layer is dcscn_handle::fold
+  const ActView* act[kMaxSegments] = {};  // activated layers: the tensor behind each epilogue segment (in Plan::act), else null
   CUtensorMap tm_hi, tm_lo;
   ConvTCParams p;
   ConvRefParams ref;
@@ -180,6 +212,7 @@ struct TcLaunch {
 
 struct Plan {
   int n = 0, h = 0, w = 0;
+  std::vector<ActView> act;      // per entry of dcscn_handle::layers: the activated layers' outputs (act_view)
   ConvFirstParams first;
   std::vector<TcLaunch> tc;      // in execution order
   std::vector<DwParams> dw;      // depthwise step in front of tc[i] (ksz 0: none; wide depthwise-separable graphs)
@@ -243,11 +276,8 @@ struct dcscn_handle {
 
   // workspace (grow-only)
   size_t cap_px = 0;                 // LR pixels the buffers can hold
-  DeviceArray<__half> feat_hi, feat_lo;
-  DeviceArray<__half> b1_hi, b1_lo;
-  DeviceArray<__half> nin_hi, nin_lo;
-  DeviceArray<__half> mid_hi, mid_lo;
-  DeviceArray<__half> u_hi, u_lo;    // wide depthwise-separable graphs: a layer's depthwise output, read by its pointwise
+  Planes feat, b1, nin, mid;         // the activation buffers (act_view)
+  Planes u;                          // wide depthwise-separable graphs: a layer's depthwise output, read by its pointwise
   DeviceArray<float> hr;
   DeviceArray<float> vbuf;           // tap-planar partial products of the fused R-CNN1 [9][N][sH][sW]
   DeviceArray<float> io_x, io_x2, io_y;  // staging for forward_host
@@ -301,7 +331,7 @@ struct dcscn_handle {
   std::vector<DsDev> ds;             // same order as `layers`
   DsDev ds_ab;                       // fused A1 | B1 1x1 layer of the tile kernels: [concat positions][A1 cols | B1 cols], scales folded
   DeviceArray<float> ds_feat, ds_b1, ds_nin, ds_mid, ds_hr;
-  int ds_total = 0;                  // channels of the (unpadded) concat buffer
+  int ds_total = 0;                  // channels of the concat buffer (4-aligned slots at ds_off, see build_graph)
   int ds_n = 0, ds_h = 0, ds_w = 0;  // geometry of the last DS forward
   std::vector<int> ds_off;
 
@@ -482,8 +512,58 @@ static int build_graph(dcscn_handle* h) {
   h->a1_w = pad16(c.nin_filters);
   h->nin_pitch = h->b1_w + h->a1_w;  // [B2 | A1]  (Concat2 order, DCSCN.py:281)
   h->mid_pitch = pad16(cin);
+  // the fp32 concat buffer of forward_ds_tile: every CNNi slot starts on a multiple of 4 channels (16-byte loads /
+  // stores); the pad channels are never written (the buffer is zero-filled once) and meet zero rows in the A1 / B1 filters
+  off = 0;
+  for (int f : h->filters) {
+    h->ds_off.push_back(off);
+    off += (f + 3) & ~3;
+  }
+  h->ds_total = off;
   h->ds_wide = c.depthwise_separable && !ds_tile_fits(h);
   return 0;
+}
+
+// Resolves an activation name of the C ABI (CNNi, A1, B1, B2, Up-PS, Up-PS2 at x4, Up-TCNN; the pixel-shuffler output
+// is named after the layer that writes it) against the buffers the graph runs on.  False: no such tensor.
+// The dropout streams are stated here and nowhere else.  The tensor-core layout numbers them CNNi = i, A1 = B1 = L+1
+// (one keep mask over the fused A1+B1 GEMM's a1_w + b1_w columns, B1 from column a1_w), B2 = L+2; forward_ds_tile's
+// dense [px][C] layout numbers A1 = L+1, B2 = L+2, B1 = L+3.
+static bool act_view(const dcscn_handle* h, const std::string& name, ActView* v) {
+  const dcscn_config& c = h->cfg;
+  const int L = c.layers, na = c.nin_filters, nb = c.nin_filters2, cps = na + nb;
+  const bool ds = uses_ds_tile(h);
+  if (name.rfind("CNN", 0) == 0) {
+    const int i = atoi(name.c_str() + 3) - 1;
+    if (i < 0 || i >= L) return false;
+    *v = ds ? ActView{BUF_FEAT, {}, nullptr, h->ds_total, h->ds_off[i], h->filters[i], 1, (uint32_t)(i + 1), h->filters[i], 0}
+            : ActView{BUF_FEAT, {}, nullptr, h->feat_pitch, h->feat_off[i], h->filters[i], 1, (uint32_t)(i + 1), h->feat_w[i], 0};
+  } else if (name == "A1") {
+    *v = ds ? ActView{BUF_NIN, {}, nullptr, cps, nb, na, 1, (uint32_t)(L + 1), na, 0}
+            : ActView{BUF_NIN, {}, nullptr, h->nin_pitch, h->b1_w, na, 1, (uint32_t)(L + 1), h->a1_w + h->b1_w, 0};
+  } else if (name == "B1") {
+    *v = ds ? ActView{BUF_B1, {}, nullptr, nb, 0, nb, 1, (uint32_t)(L + 3), nb, 0}
+            : ActView{BUF_B1, {}, nullptr, h->b1_w, 0, nb, 1, (uint32_t)(L + 1), h->a1_w + h->b1_w, h->a1_w};
+  } else if (name == "B2") {
+    *v = ActView{BUF_NIN, {}, nullptr, ds ? cps : h->nin_pitch, 0, nb, 1, (uint32_t)(L + 2), ds ? nb : h->b1_w, 0};
+  } else if (name == "Up-PS" && two_stage_up(h)) {
+    *v = ActView{BUF_MID, {}, nullptr, ds ? cps : h->mid_pitch, 0, cps, 4, 0, 0, 0};
+  } else if (name == (tconv(h) ? "Up-TCNN" : two_stage_up(h) ? "Up-PS2" : "Up-PS")) {
+    *v = ActView{BUF_HR, {}, nullptr, h->ps_out, 0, h->ps_out, c.scale * c.scale, 0, 0, 0};
+  } else {
+    return false;
+  }
+  auto at = [&](auto* base) { return base ? base + v->off : nullptr; };
+  if (ds) {
+    const DeviceArray<float>* bufs[] = {&h->ds_feat, &h->ds_nin, &h->ds_b1, &h->ds_mid, &h->ds_hr};
+    v->f32 = at(bufs[v->buf]->get());
+  } else if (v->buf == BUF_HR) {
+    v->f32 = at(h->hr.get());
+  } else {
+    const Planes* bufs[] = {&h->feat, &h->nin, &h->b1, &h->mid};
+    v->planes = bufs[v->buf]->at(v->off);
+  }
+  return true;
 }
 
 static const LayerDef* find_layer(const dcscn_handle* h, const std::string& scope) {
@@ -688,15 +768,6 @@ static int finalize_params_ds(dcscn_handle* h) {
   h->ds_ab = dcscn_handle::DsDev();
   h->ds.clear();
   h->ds.resize(h->layers.size());
-  // concat buffer: every CNNi slot starts on a multiple of 4 channels (16-byte loads / stores); the pad channels are never
-  // written (the buffer is zero-filled once) and meet zero rows in the A1 / B1 filters
-  h->ds_off.clear();
-  int off = 0;
-  for (int f : h->filters) {
-    h->ds_off.push_back(off);
-    off += (f + 3) & ~3;
-  }
-  h->ds_total = off;
   const int T = h->ds_total, L = h->cfg.layers;
   std::vector<float> ab_pw, ab_bias, ab_alpha;
   const int na = h->cfg.nin_filters, nb = h->cfg.nin_filters2;
@@ -1001,13 +1072,9 @@ static int ensure_workspace(dcscn_handle* h, size_t lr_px) {
   h->plans.clear();
   h->last_plan = nullptr;
   const bool two = ws.planes == 2;
-  if (h->feat_hi.alloc(lr_px * ws.feat, true) || h->feat_lo.alloc(two ? lr_px * ws.feat : 0, true)) return 1;
-  if (h->b1_hi.alloc(lr_px * ws.b1, true) || h->b1_lo.alloc(two ? lr_px * ws.b1 : 0, true)) return 1;
-  if (h->nin_hi.alloc(lr_px * ws.nin, true) || h->nin_lo.alloc(two ? lr_px * ws.nin : 0, true)) return 1;
-  if (two_stage_up(h)) {
-    if (h->mid_hi.alloc(lr_px * ws.mid, true) || h->mid_lo.alloc(two ? lr_px * ws.mid : 0, true)) return 1;
-  }
-  if (h->u_hi.alloc(lr_px * ws.u, true) || h->u_lo.alloc(two ? lr_px * ws.u : 0, true)) return 1;
+  if (h->feat.alloc(lr_px * ws.feat, two) || h->b1.alloc(lr_px * ws.b1, two) || h->nin.alloc(lr_px * ws.nin, two) ||
+      h->mid.alloc(lr_px * ws.mid, two) || h->u.alloc(lr_px * ws.u, two))
+    return 1;
   if (h->hr.alloc(lr_px * ws.hr, true) || h->vbuf.alloc(lr_px * ws.vbuf, true)) return 1;
   h->cap_px = lr_px;
   return 0;
@@ -1016,8 +1083,8 @@ static int ensure_workspace(dcscn_handle* h, size_t lr_px) {
 // Device bytes of the activation workspace and the tiled-inference staging buffers (dcscn_device_bytes).
 static int64_t workspace_bytes(const dcscn_handle* h) {
   auto bytes = [](const auto&... a) { return (int64_t)(0 + ... + (a.size() * sizeof(*a.get()))); };
-  return bytes(h->feat_hi, h->feat_lo, h->b1_hi, h->b1_lo, h->nin_hi, h->nin_lo, h->mid_hi, h->mid_lo, h->u_hi, h->u_lo, h->hr, h->vbuf,
-               h->ds_feat, h->ds_b1, h->ds_nin, h->ds_mid, h->ds_hr, h->tile_x, h->tile_x2, h->tile_y);
+  return h->feat.bytes() + h->b1.bytes() + h->nin.bytes() + h->mid.bytes() + h->u.bytes() +
+         bytes(h->hr, h->vbuf, h->ds_feat, h->ds_b1, h->ds_nin, h->ds_mid, h->ds_hr, h->tile_x, h->tile_x2, h->tile_y);
 }
 
 // --------------------------------------------------------------------------------------- plans ----
@@ -1069,8 +1136,8 @@ static int encode_map(dcscn_handle* h, CUtensorMap* tm, const __half* base, int 
   return 0;
 }
 
-static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, const __half* src_hi, const __half* src_lo,
-                         int src_pitch, int n, int H, int W, const EpiParams& epi) {
+static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, PlaneView src, int src_pitch, int n, int H, int W,
+                         const EpiParams& epi) {
   TcLaunch L;
   memset(&L, 0, sizeof(L));
   int TH = 0, TW = 0;
@@ -1081,9 +1148,9 @@ static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, const __ha
     return fail("internal: layer %s: patch width %d is not a whole number of swizzle atoms", t.name.c_str(), TW);
   ConvGeom g{n, H, W, (W + TW - 1) / TW, (H + TH - 1) / TH, TW, TH};
   const int box_rows = TH + t.ksz - 1;   // a k x k layer's box carries the rows of all k ky taps
-  if (encode_map(h, &L.tm_hi, src_hi, t.cin_pad, src_pitch, n, H, W, box_rows, TW)) return 1;
+  if (encode_map(h, &L.tm_hi, src.hi, t.cin_pad, src_pitch, n, H, W, box_rows, TW)) return 1;
   if (planes(h) == 2) {
-    if (encode_map(h, &L.tm_lo, src_lo, t.cin_pad, src_pitch, n, H, W, box_rows, TW)) return 1;
+    if (encode_map(h, &L.tm_lo, src.lo, t.cin_pad, src_pitch, n, H, W, box_rows, TW)) return 1;
   } else {
     L.tm_lo = L.tm_hi;
   }
@@ -1109,7 +1176,6 @@ static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, const __ha
     L.layer_bwd = true;
   }
   L.p.epi.n_valid = t.n_valid;
-  L.p.epi.drop_ntotal = pad16(t.cout);   // keep-mask index stride = slot width, whatever the column tiling
 
   // Ring depths.  The consumers release a slot one weight tile late, so each ring needs at least two slots.  A k x k layer
   // reads k weight tiles per activation slot: three activation slots when four weight tiles still fit, else two.
@@ -1140,8 +1206,8 @@ static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, const __ha
   L.ref.ksz = t.ksz;
   L.ref.cin = t.cin;
   L.ref.cout = t.cout;
-  L.ref.src_hi = src_hi;
-  L.ref.src_lo = planes(h) == 2 ? src_lo : nullptr;
+  L.ref.src_hi = src.hi;
+  L.ref.src_lo = src.lo;
   L.ref.src_pitch = src_pitch;
   L.ref.in_map = t.d_in_map.get();
   L.ref.w = t.d_wref.get();
@@ -1154,42 +1220,65 @@ static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, const __ha
 
 // A forward layer: its depthwise step when it has one (the 1x1 pointwise then reads u instead of the source), then
 // its tensor-core launch.  pl->dw stays parallel to pl->tc.
-static int add_layer_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, const __half* src_hi, const __half* src_lo,
-                            int src_pitch, int n, int H, int W, const EpiParams& epi) {
+static int add_layer_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, PlaneView src, int src_pitch, int n, int H, int W,
+                            const EpiParams& epi) {
   DwParams d;
   memset(&d, 0, sizeof(d));
   if (t.dw_ksz) {
-    d = DwParams{n, H, W, t.dw_ksz, t.cin_pad, src_hi, src_lo, src_pitch, t.d_dw.get(), h->u_hi.get(), planes(h) == 2 ? h->u_lo.get() : nullptr};
-    src_hi = d.u_hi;
-    src_lo = d.u_lo;
+    const PlaneView u = h->u.at(0);
+    d = DwParams{n, H, W, t.dw_ksz, t.cin_pad, src.hi, src.lo, src_pitch, t.d_dw.get(), u.hi, u.lo};
+    src = u;
     src_pitch = t.cin_pad;
     pl->dw_count++;
   }
   pl->dw.push_back(d);
-  return add_tc_launch(h, pl, t, src_hi, src_lo, src_pitch, n, H, W, epi);
+  return add_tc_launch(h, pl, t, src, src_pitch, n, H, W, epi);
 }
 
-static EpiParams epi_planes(__half* hi, __half* lo, int pitch, int col_begin, int col_end) {
+// One EPI_PLANES segment: GEMM columns [0, cols) to `dst`.
+static EpiParams epi_planes(PlaneView dst, int pitch, int cols) {
   EpiParams e;
   memset(&e, 0, sizeof(e));
   e.mode = EPI_PLANES;
   e.num_seg = 1;
-  e.seg[0] = {col_begin, col_end, hi, lo, pitch};
+  e.seg[0] = {0, cols, dst.hi, dst.lo, pitch};
   e.keep_prob = 1.0f;
   e.out_scale = 1.0f;
   return e;
+}
+
+// The epilogue of an activated layer: one segment per output tensor, over the GEMM columns its keep mask indexes.
+static EpiParams epi_activated(const dcscn_handle* h, std::initializer_list<const ActView*> outs) {
+  EpiParams e = epi_planes({}, 0, 0);
+  e.num_seg = 0;
+  for (const ActView* v : outs) {
+    e.seg[e.num_seg++] = {v->drop_col0, v->drop_col0 + pad16(v->ch), v->planes.hi, v->planes.lo, v->pitch};
+    e.drop_ntotal = v->drop_stride;
+  }
+  e.act = h->cfg.activator;
+  return e;
+}
+
+static int add_activated_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, const ActView& src, int n, int H, int W,
+                                std::initializer_list<const ActView*> outs) {
+  if (add_layer_launch(h, pl, t, src.planes, src.pitch, n, H, W, epi_activated(h, outs))) return 1;
+  std::copy(outs.begin(), outs.end(), pl->tc.back().act);
+  return 0;
 }
 
 static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
   for (auto& p : h->plans)
     if (p->n == n && p->h == H && p->w == W) return p.get();
   const dcscn_config& c = h->cfg;
+  const int L = c.layers;
   std::unique_ptr<Plan> pl(new Plan());
   pl->n = n;
   pl->h = H;
   pl->w = W;
-  const bool two = planes(h) == 2;
-  auto lo = [&](__half* p, size_t off) -> __half* { return two ? p + off : nullptr; };
+  pl->act.resize(h->layers.size());
+  for (size_t li = 0; li < h->layers.size(); ++li)
+    if (h->layers[li].act) act_view(h, h->layers[li].scope, &pl->act[li]);
+  const ActView* a = pl->act.data();   // CNN1 .. CNNL, A1, B1, B2 (build_graph's layer order)
 
   // CNN1
   memset(&pl->first, 0, sizeof(pl->first));
@@ -1197,32 +1286,17 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
   pl->first.ksz = find_layer(h, "CNN1")->k;
   pl->first.n_pad = h->feat_w[0];
   pl->first.w = h->d_first_w.get();
-  pl->first.epi = epi_planes(h->feat_hi.get(), lo(h->feat_lo.get(), 0), h->feat_pitch, 0, h->feat_w[0]);
+  pl->first.epi = epi_activated(h, {&a[0]});
   pl->first.epi.bias = h->d_first_bias.get();
   pl->first.epi.alpha = h->d_first_alpha.get();
-  pl->first.epi.act = c.activator;
   pl->first.epi.n_valid = h->filters[0];
 
   size_t ti = 0;
-  for (int i = 1; i < c.layers; ++i, ++ti) {
-    EpiParams e = epi_planes(h->feat_hi.get() + h->feat_off[i], lo(h->feat_lo.get(), h->feat_off[i]), h->feat_pitch, 0, h->feat_w[i]);
-    e.act = c.activator;
-    if (add_layer_launch(h, pl.get(), h->tcl[ti], h->feat_hi.get() + h->feat_off[i - 1], lo(h->feat_lo.get(), h->feat_off[i - 1]),
-                      h->feat_pitch, n, H, W, e))
-      return nullptr;
-  }
-  {  // A1+B1: columns [0,a1_w) -> nin[:, b1_w:], columns [a1_w, a1_w+b1_w) -> b1
-    EpiParams e = epi_planes(h->nin_hi.get() + h->b1_w, lo(h->nin_lo.get(), h->b1_w), h->nin_pitch, 0, h->a1_w);
-    e.num_seg = 2;
-    e.seg[1] = {h->a1_w, h->a1_w + h->b1_w, h->b1_hi.get(), two ? h->b1_lo.get() : nullptr, h->b1_w};
-    e.act = c.activator;
-    if (add_layer_launch(h, pl.get(), h->tcl[ti++], h->feat_hi.get(), lo(h->feat_lo.get(), 0), h->feat_pitch, n, H, W, e)) return nullptr;
-  }
-  {  // B2 -> nin[:, 0:b1_w]
-    EpiParams e = epi_planes(h->nin_hi.get(), lo(h->nin_lo.get(), 0), h->nin_pitch, 0, h->b1_w);
-    e.act = c.activator;
-    if (add_layer_launch(h, pl.get(), h->tcl[ti++], h->b1_hi.get(), two ? h->b1_lo.get() : nullptr, h->b1_w, n, H, W, e)) return nullptr;
-  }
+  for (int i = 1; i < L; ++i)
+    if (add_activated_launch(h, pl.get(), h->tcl[ti++], a[i - 1], n, H, W, {&a[i]})) return nullptr;
+  // A1+B1 reads the whole concat buffer (CNN1's slot starts at channel 0)
+  if (add_activated_launch(h, pl.get(), h->tcl[ti++], a[0], n, H, W, {&a[L], &a[L + 1]})) return nullptr;
+  if (add_activated_launch(h, pl.get(), h->tcl[ti++], a[L + 1], n, H, W, {&a[L + 2]})) return nullptr;   // B1 -> B2
   int HR_H = H, HR_W = W;
   {  // Up-PS, or Up-TCNN (its 3x3 LR form, then depth_to_space(s) in one step at every scale)
     EpiParams e;
@@ -1233,7 +1307,7 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
       e.d2s_r = 2;
       e.d2s_cout = c.nin_filters + c.nin_filters2;
       e.num_seg = 1;
-      e.seg[0] = {0, 0, h->mid_hi.get(), two ? h->mid_lo.get() : nullptr, h->mid_pitch};
+      e.seg[0] = {0, 0, h->mid.hi.get(), h->mid.lo.get(), h->mid_pitch};
     } else {
       e.mode = EPI_D2S_F32;
       e.d2s_r = c.scale;
@@ -1241,7 +1315,7 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
       e.dst_f32 = h->hr.get();
       e.d2s_pitch = h->ps_out;
     }
-    if (add_layer_launch(h, pl.get(), h->tcl[ti++], h->nin_hi.get(), two ? h->nin_lo.get() : nullptr, h->nin_pitch, n, H, W, e)) return nullptr;
+    if (add_layer_launch(h, pl.get(), h->tcl[ti++], h->nin.at(0), h->nin_pitch, n, H, W, e)) return nullptr;
     HR_H = H * (two_stage_up(h) ? 2 : c.scale);
     HR_W = W * (two_stage_up(h) ? 2 : c.scale);
   }
@@ -1254,8 +1328,7 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
     e.d2s_cout = h->ps_out;
     e.dst_f32 = h->hr.get();
     e.d2s_pitch = h->ps_out;
-    if (add_layer_launch(h, pl.get(), h->tcl[ti++], h->mid_hi.get(), two ? h->mid_lo.get() : nullptr, h->mid_pitch, n, HR_H, HR_W, e))
-      return nullptr;
+    if (add_layer_launch(h, pl.get(), h->tcl[ti++], h->mid.at(0), h->mid_pitch, n, HR_H, HR_W, e)) return nullptr;
     HR_H *= 2;
     HR_W *= 2;
   }
@@ -1536,27 +1609,30 @@ static int launch_depthwise(dcscn_handle* h, const DwParams& p, cudaStream_t st)
   return mark(h, st);
 }
 
+// CNN1 (the forward's and the train step's): the 3x3 fast path, storing min(z, 0) when the epilogue asks for it, or the
+// general kernel.
+static int launch_first(dcscn_handle* h, const ConvFirstParams& p, cudaStream_t st) {
+  if (p.ksz > 5) return fail("cnn_size %d is not supported by the first-layer kernel", p.ksz);
+  const long long total = (long long)p.g.n_img * p.g.H * p.g.W;
+  if (p.ksz == 3 && p.n_pad <= 256) {
+    const int grid = (int)std::min<long long>((total + 7) / 8, (long long)h->sm_count * 8);
+    if (p.epi.seg[0].dst_zneg != nullptr) conv_first3x3_kernel<true><<<grid, 256, 0, st>>>(p);
+    else conv_first3x3_kernel<false><<<grid, 256, 0, st>>>(p);
+  } else {
+    const int grid = (int)std::min<long long>((total + 255) / 256, (long long)h->sm_count * 8);
+    conv_first_kernel<<<grid, 256, (size_t)p.ksz * p.ksz * p.n_pad * sizeof(float), st>>>(p);
+  }
+  CUDA_TRY(cudaGetLastError());
+  h->launches++;
+  return 0;
+}
+
 // CNN1 and the tensor-core layers of one forward, in execution order, on `st` (a capturing stream when the plan's graph is
 // being built).  The last kernel (R-CNN1 gather / R-CNN1) is issued by forward_impl: it alone touches x2 and y.
-static int issue_front(dcscn_handle* h, Plan* pl, const float* x, int n, int H, int W, bool fused, cudaStream_t st) {
-  {  // CNN1
-    ConvFirstParams p = pl->first;
-    p.x = x;
-    if (p.ksz > 5) return fail("cnn_size %d is not supported by the first-layer kernel", p.ksz);
-    const long long total = (long long)n * H * W;
-    const int grid = (int)std::min<long long>((total + 255) / 256, (long long)h->sm_count * 8);
-    const size_t smem = (size_t)p.ksz * p.ksz * p.n_pad * sizeof(float);
-    if (p.ksz == 3 && p.n_pad <= 256) {
-      const int first_grid = (int)std::min<long long>((total + 7) / 8, (long long)h->sm_count * 8);
-      if (p.epi.seg[0].dst_zneg != nullptr) conv_first3x3_kernel<true><<<first_grid, 256, 0, st>>>(p);
-      else conv_first3x3_kernel<false><<<first_grid, 256, 0, st>>>(p);
-    } else {
-      conv_first_kernel<<<grid, 256, smem, st>>>(p);
-    }
-    CUDA_TRY(cudaGetLastError());
-    h->launches++;
-    if (mark(h, st)) return 1;
-  }
+static int issue_front(dcscn_handle* h, Plan* pl, const float* x, bool fused, cudaStream_t st) {
+  ConvFirstParams first = pl->first;
+  first.x = x;
+  if (launch_first(h, first, st) || mark(h, st)) return 1;
   for (size_t i = 0; i < pl->tc.size(); ++i) {
     if (pl->dw[i].ksz && launch_depthwise(h, pl->dw[i], st)) return 1;
     const TcLaunch& L = ((int)i == pl->fused_index && !fused) ? pl->unfused : pl->tc[i];
@@ -1601,7 +1677,7 @@ static int forward_impl(dcscn_handle* h, const float* x, const float* x2, float*
     if (pl->gexec) { cudaGraphExecDestroy(pl->gexec); pl->gexec = nullptr; }
     const int64_t before = h->launches;
     CUDA_TRY(cudaStreamBeginCapture(h->cap_stream.get(), cudaStreamCaptureModeThreadLocal));
-    const int rc = issue_front(h, pl, x, n, H, W, fused, h->cap_stream.get());
+    const int rc = issue_front(h, pl, x, fused, h->cap_stream.get());
     cudaGraph_t g = nullptr;
     const cudaError_t ce = cudaStreamEndCapture(h->cap_stream.get(), &g);
     h->launches = before;
@@ -1616,7 +1692,7 @@ static int forward_impl(dcscn_handle* h, const float* x, const float* x2, float*
     h->launches += pl->g_launches;
     h->graph_replays++;
   } else {
-    if (issue_front(h, pl, x, n, H, W, fused, st)) return 1;
+    if (issue_front(h, pl, x, fused, st)) return 1;
     pl->eager_runs++;
   }
   pl->last_x = x;
@@ -2068,80 +2144,35 @@ int dcscn_get_activation(dcscn_handle* h, const char* tensor, float* host_data, 
   if (h->tiled_last)
     return fail("dcscn_get_activation: the last forward ran tiled (option workspace_mb): the buffers hold its last batch "
                 "of windows, not the image");
-  if (uses_ds_tile(h)) {
-    if (h->ds_n == 0) return fail("dcscn_get_activation: no forward has run yet");
-    CUDA_TRY(cudaSetDevice(h->cfg.device_id));
-    CUDA_TRY(cudaDeviceSynchronize());
-    const dcscn_config& c = h->cfg;
-    const std::string t(tensor);
-    const int cps = c.nin_filters + c.nin_filters2;
-    const float* src = nullptr;
-    int pitch = 0, off = 0, ch = 0;
-    size_t px = (size_t)h->ds_n * h->ds_h * h->ds_w;
-    if (t.rfind("CNN", 0) == 0) {
-      int i = atoi(t.c_str() + 3) - 1;
-      if (i < 0 || i >= c.layers) return fail("dcscn_get_activation: no tensor '%s'", tensor);
-      src = h->ds_feat.get(); pitch = h->ds_total; off = h->ds_off[i]; ch = h->filters[i];
-    } else if (t == "A1") { src = h->ds_nin.get(); pitch = cps; off = c.nin_filters2; ch = c.nin_filters;
-    } else if (t == "B2") { src = h->ds_nin.get(); pitch = cps; off = 0; ch = c.nin_filters2;
-    } else if (t == "B1") { src = h->ds_b1.get(); pitch = c.nin_filters2; off = 0; ch = c.nin_filters2;
-    } else if (t == "Up-PS" && c.scale == 4) { src = h->ds_mid.get(); pitch = cps; off = 0; ch = cps; px *= 4;
-    } else if ((t == "Up-PS" && c.scale != 4) || (t == "Up-PS2" && c.scale == 4)) {
-      src = h->ds_hr.get(); pitch = h->ps_out; off = 0; ch = h->ps_out; px *= (size_t)c.scale * c.scale;
-    } else return fail("dcscn_get_activation: no tensor '%s'", tensor);
-    if (numel != (int64_t)(px * ch)) return fail("dcscn_get_activation: '%s' has %lld elements, got %lld", tensor, (long long)(px * ch), (long long)numel);
-    std::vector<float> full(px * pitch);
-    CUDA_TRY(cudaMemcpy(full.data(), src, full.size() * sizeof(float), cudaMemcpyDeviceToHost));
-    for (size_t p = 0; p < px; ++p)
-      for (int k = 0; k < ch; ++k) host_data[p * ch + k] = full[p * pitch + off + k];
-    return 0;
-  }
-  Plan* pl = h->last_plan;
-  if (!pl) return fail("dcscn_get_activation: no forward has run yet");
+  const bool ds = uses_ds_tile(h);
+  const Plan* pl = h->last_plan;
+  if (ds ? h->ds_n == 0 : !pl) return fail("dcscn_get_activation: no forward has run yet");
   CUDA_TRY(cudaSetDevice(h->cfg.device_id));
   CUDA_TRY(cudaDeviceSynchronize());
-  const dcscn_config& c = h->cfg;
   const std::string t(tensor);
-  const __half *hi = nullptr, *lo = nullptr;
-  const float* f32 = nullptr;
-  int pitch = 0, off = 0, ch = 0;
-  size_t px = (size_t)pl->n * pl->h * pl->w;
-  if (t.rfind("CNN", 0) == 0) {
-    int i = atoi(t.c_str() + 3) - 1;
-    if (i < 0 || i >= c.layers) return fail("dcscn_get_activation: no tensor '%s'", tensor);
-    hi = h->feat_hi.get(); lo = h->feat_lo.get(); pitch = h->feat_pitch; off = h->feat_off[i]; ch = h->filters[i];
-  } else if (t == "A1") {
-    hi = h->nin_hi.get(); lo = h->nin_lo.get(); pitch = h->nin_pitch; off = h->b1_w; ch = c.nin_filters;
-  } else if (t == "B2") {
-    hi = h->nin_hi.get(); lo = h->nin_lo.get(); pitch = h->nin_pitch; off = 0; ch = c.nin_filters2;
-  } else if (t == "B1") {
-    hi = h->b1_hi.get(); lo = h->b1_lo.get(); pitch = h->b1_w; off = 0; ch = c.nin_filters2;
-  } else if (t == "Up-PS" && two_stage_up(h)) {
-    hi = h->mid_hi.get(); lo = h->mid_lo.get(); pitch = h->mid_pitch; off = 0; ch = c.nin_filters + c.nin_filters2; px *= 4;
-  } else if (t == (tconv(h) ? "Up-TCNN" : two_stage_up(h) ? "Up-PS2" : "Up-PS") && pl->ran_fused) {
-    return fail("dcscn_get_activation: '%s' is not materialised when the R-CNN1 fusion is on (set option fuse_last=0)", tensor);
-  } else if (t == (tconv(h) ? "Up-TCNN" : two_stage_up(h) ? "Up-PS2" : "Up-PS")) {
-    f32 = h->hr.get(); pitch = h->ps_out; ch = h->ps_out; px *= (size_t)c.scale * c.scale;
-  } else if (t == "R-CNN1/taps" && pl->ran_fused) {   // the fused R-CNN1's tap-planar products [parts][9][N][sH][sW]
-    const size_t count = px * c.scale * c.scale * 9 * pl->gather.parts;
+  const size_t lr_px = ds ? (size_t)h->ds_n * h->ds_h * h->ds_w : (size_t)pl->n * pl->h * pl->w;
+  if (!ds && pl->ran_fused && t == "R-CNN1/taps") {   // the fused R-CNN1's tap-planar products [parts][9][N][sH][sW]
+    const size_t count = lr_px * h->cfg.scale * h->cfg.scale * 9 * pl->gather.parts;
     if (numel != (int64_t)count) return fail("dcscn_get_activation: '%s' has %lld elements, got %lld", tensor, (long long)count, (long long)numel);
     CUDA_TRY(cudaMemcpy(host_data, h->vbuf.get(), count * sizeof(float), cudaMemcpyDeviceToHost));
     return 0;
-  } else {
-    return fail("dcscn_get_activation: no tensor '%s'", tensor);
   }
-  if (numel != (int64_t)(px * ch)) return fail("dcscn_get_activation: '%s' has %lld elements, got %lld", tensor, (long long)(px * ch), (long long)numel);
-  std::vector<float> full(px * pitch);
-  if (f32) {
-    CUDA_TRY(cudaMemcpy(full.data(), f32, full.size() * sizeof(float), cudaMemcpyDeviceToHost));
-  } else {
-    DeviceArray<float> tmp;
-    if (tmp.alloc(full.size())) return 1;
-    planes_to_f32_kernel<<<1024, 256>>>(hi, planes(h) == 2 ? lo : nullptr, tmp.get(), full.size());
-    CUDA_TRY(cudaMemcpy(full.data(), tmp.get(), full.size() * sizeof(float), cudaMemcpyDeviceToHost));
+  ActView v;
+  if (!act_view(h, t, &v)) return fail("dcscn_get_activation: no tensor '%s'", tensor);
+  if (!ds && pl->ran_fused && v.buf == BUF_HR)
+    return fail("dcscn_get_activation: '%s' is not materialised when the R-CNN1 fusion is on (set option fuse_last=0)", tensor);
+  const size_t px = lr_px * v.px_mul;
+  if (numel != (int64_t)(px * v.ch)) return fail("dcscn_get_activation: '%s' has %lld elements, got %lld", tensor, (long long)(px * v.ch), (long long)numel);
+  const float* src = v.f32;
+  DeviceArray<float> tmp;
+  if (!src) {   // fp16 planes: hi + lo in fp32, from the tensor's first channel on
+    const size_t count = px * v.pitch - v.off;
+    if (tmp.alloc(count)) return 1;
+    planes_to_f32_kernel<<<1024, 256>>>(v.planes.hi, v.planes.lo, tmp.get(), count);
+    src = tmp.get();
   }
-  for (size_t p = 0; p < px; ++p)
-    for (int k = 0; k < ch; ++k) host_data[p * ch + k] = full[p * pitch + off + k];
+  const size_t row = v.ch * sizeof(float);
+  CUDA_TRY(cudaMemcpy2D(host_data, row, src, v.pitch * sizeof(float), row, px, cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -2623,20 +2654,12 @@ int dcscn_get_train_tensor(dcscn_handle* h, const char* name, float* host_data, 
   if (s.rfind("zneg:", 0) == 0) {   // min(z, 0) planes of the last training forward (prelu / leaky_relu only)
     if (!needs_zneg(h)) return fail("dcscn_get_train_tensor: '%s': the activator keeps no min(z, 0) planes", name);
     if (t->last_px == 0) return fail("dcscn_get_train_tensor: '%s': the fp32 depthwise-separable step keeps no min(z, 0) planes (see \"Z:\")", name);
-    const std::string l = s.substr(5);
-    const __half* src = nullptr;
-    int pitch = 0;
-    if (l.rfind("CNN", 0) == 0) {
-      const int i = atoi(l.c_str() + 3) - 1;
-      if (i < 0 || i >= h->cfg.layers) return fail("dcscn_get_train_tensor: no tensor '%s'", name);
-      src = t->zneg_feat.get() + h->feat_off[i]; pitch = h->feat_pitch; ch = h->filters[i];
-    } else if (l == "A1") { src = t->zneg_nin.get() + h->b1_w; pitch = h->nin_pitch; ch = h->cfg.nin_filters;
-    } else if (l == "B2") { src = t->zneg_nin.get(); pitch = h->nin_pitch; ch = h->cfg.nin_filters2;
-    } else if (l == "B1") { src = t->zneg_b1.get(); pitch = h->b1_w; ch = h->cfg.nin_filters2;
-    } else return fail("dcscn_get_train_tensor: no tensor '%s'", name);
+    ActView v;
+    if (!act_view(h, s.substr(5), &v) || !v.drop_layer) return fail("dcscn_get_train_tensor: no tensor '%s'", name);   // activated ones only
     px = t->last_px;
+    ch = v.ch;
     hi.resize(px * ch);
-    CUDA_TRY(cudaMemcpy2D(hi.data(), ch * sizeof(__half), src, pitch * sizeof(__half), ch * sizeof(__half), px, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy2D(hi.data(), ch * sizeof(__half), zneg_of(h, v), v.pitch * sizeof(__half), ch * sizeof(__half), px, cudaMemcpyDeviceToHost));
   } else {
     auto it = t->captured.find(s);
     if (it == t->captured.end())
@@ -2773,28 +2796,15 @@ float dcscn_last_grad_norm(dcscn_handle* h) { return (h && h->train) ? h->train-
 
 int dcscn_dropout_mask(dcscn_handle* h, const char* tensor, uint32_t seed, int n, int height, int width, uint8_t* mask, int64_t numel) {
   if (!h || !tensor || !mask) return fail("dcscn_dropout_mask: null argument");
-  const dcscn_config& c = h->cfg;
-  const std::string t(tensor);
-  const int L = c.layers;
-  int C = 0, n_total = 0, col0 = 0;
-  uint32_t layer = 0;
-  if (t.rfind("CNN", 0) == 0) {
-    const int i = atoi(t.c_str() + 3) - 1;
-    if (i < 0 || i >= L) return fail("dcscn_dropout_mask: no tensor '%s'", tensor);
-    C = h->filters[i]; n_total = h->feat_w[i]; col0 = 0; layer = (uint32_t)(i + 1);
-  } else if (t == "A1") { C = c.nin_filters; n_total = h->a1_w + h->b1_w; col0 = 0; layer = (uint32_t)(L + 1);
-  } else if (t == "B1") { C = c.nin_filters2; n_total = h->a1_w + h->b1_w; col0 = h->a1_w; layer = (uint32_t)(L + 1);
-  } else if (t == "B2") { C = c.nin_filters2; n_total = h->b1_w; col0 = 0; layer = (uint32_t)(L + 2);
-  } else return fail("dcscn_dropout_mask: tensor '%s' has no dropout", tensor);
-  if (uses_ds_tile(h)) {   // train_ds.inc: dense [pixel][channel] indexing, A1 / B2 / B1 are layers L+1 / L+2 / L+3
-    n_total = C; col0 = 0;
-    if (t == "B1") layer = (uint32_t)(L + 3);
-  }
+  ActView v;
+  if (!act_view(h, tensor, &v) || !v.drop_layer)
+    return fail(strncmp(tensor, "CNN", 3) == 0 ? "dcscn_dropout_mask: no tensor '%s'" : "dcscn_dropout_mask: tensor '%s' has no dropout", tensor);
   const size_t px = (size_t)n * height * width;
+  const int C = v.ch;
   if (numel != (int64_t)(px * C)) return fail("dcscn_dropout_mask: expected %lld elements", (long long)(px * C));
   for (size_t q = 0; q < px; ++q)
     for (int k = 0; k < C; ++k)
-      mask[q * C + k] = dropout_keep(seed, layer, (uint64_t)q * (uint64_t)n_total + col0 + k, c.dropout_keep) ? 1 : 0;
+      mask[q * C + k] = dropout_keep(seed, v.drop_layer, (uint64_t)q * (uint64_t)v.drop_stride + v.drop_col0 + k, h->cfg.dropout_keep) ? 1 : 0;
   return 0;
 }
 
