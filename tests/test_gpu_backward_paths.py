@@ -13,7 +13,10 @@ power-of-two scale (quantise, test_gpu_forward_paths.py).  With S = sum |a| |w| 
   s2d_planes_kernel       a copy: bit for bit
   dgrad twins             conv_tc_kernel at K = k^2 cin_pad of the twin: tc_units + 1 (epilogue scale) 2^-23 S, stored
   act_grad[8]_kernel      dZ = (g1 + g2) * mask * fp32(1 / keep) * slope: 4 roundings, 2^-22 |dZ|, stored; bias and
-                          slope sums are fp32 over the pixels: (n + 4) 2^-24 sum |terms|
+                          slope sums are fp32 over the pixels: (n + 4) 2^-24 sum |terms|.  relu, sigmoid, tanh and selu
+                          take f' from h = fp32(stored output * fp32(keep)), the f' of check_step's act_grad in fp64 from
+                          that h: relu exact, sigmoid h (1 - h) 2 2^-24 |f'|, tanh 1 - h h 2^-24 (h^2 + |f'|), selu
+                          h + lambda alpha 2^-24 |f'|; then one more rounding for the product
   wgrad_tc_kernel         one fp32 wgmma accumulator per (tap, 128 x n_pad tile) and CTA over chunks / ksplit chunks of
                           32 pixels, 6 k16 steps per chunk (a_lo z_hi, a_hi z_lo, a_hi z_hi, each over 2 x 16 pixels).
                           A step aligns its 16 products and the accumulator to the largest exponent and truncates each
@@ -37,7 +40,7 @@ import torch.nn.functional as F
 
 import dcscn_oracle as O
 from conftest import GOLDEN, MODEL_FLAGS, load_golden_weights
-from test_gpu_forward_paths import quantise, tc_units
+from test_gpu_forward_paths import LEAKY, SELU_SCALE, SELU_SCALE_ALPHA, quantise, tc_units
 from test_gpu_train import CDCSCN, GRADIENT_CASES, assert_kernels_ran, launched_kernels, setup
 
 pytestmark = pytest.mark.gpu
@@ -124,6 +127,7 @@ class Checker:
 
     def __init__(self):
         self.worst, self.signed = {}, {}
+        self.gm = {}      # per activated layer: the output gradient after dropout, g mask fp32(1 / keep) (check_step)
 
     def add(self, name, got, ref, bar, signed=False):
         got = torch.as_tensor(got).to(dev(), torch.float64) if not torch.is_tensor(got) else got.to(dev(), torch.float64)
@@ -137,10 +141,11 @@ class Checker:
         return [(k, v) for k, v in self.worst.items() if not v <= 1.0]
 
 
-def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None):
-    """Every backward kernel of the last train step of `eng` (run with grad_capture = 1) against its isolated reference.
-    `get_grad(name)` returns a variable's gradient as get_grad does (default: eng.get_grad); a wide depthwise-separable
-    graph passes its composed filters as the conv_W entries of `w` and reads their gradients from "dWc:"."""
+def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None, act="prelu"):
+    """Every backward kernel of the last train step of `eng` (run with grad_capture = 1, activator `act`) against its
+    isolated reference.  `get_grad(name)` returns a variable's gradient as get_grad does (default: eng.get_grad); a wide
+    depthwise-separable graph passes its composed filters as the conv_W entries of `w` and reads their gradients from
+    "dWc:"."""
     cfg = O.OracleConfig(**kw)
     n, h, wd = x.shape[:3]
     s = cfg.scale
@@ -157,7 +162,7 @@ def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None):
     def T(name, shape):
         return t64(eng.get_train_tensor(name, shape))
 
-    def act(name, c, r=1):
+    def plane(name, c, r=1):
         return t64(eng.get_activation(name, (n, r * h, r * wd, c)))
 
     def grad(name):
@@ -178,7 +183,7 @@ def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None):
 
     # ---- R-CNN1: filter gradient and data gradient (in space_to_depth form)
     up_name, r_last = ("Up-PS2", 2) if s == 4 else ("Up-PS", s)
-    hr = act(up_name, ps_out, s)
+    hr = plane(up_name, ps_out, s)
     wr = w["R-CNN1/conv_W"]
     kr = wr.shape[0]
     ssum, sabs = wgrad(hr, dY, kr), wgrad(hr.abs(), dY.abs(), kr)
@@ -207,10 +212,10 @@ def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None):
 
     # ---- pixel shuffler(s)
     b1w, a1w = pad16(cfg.nin_filters2), pad16(cfg.nin_filters)
-    nin_in = torch.cat([act("B2", cfg.nin_filters2), act("A1", cfg.nin_filters)], dim=1)
+    nin_in = torch.cat([plane("B2", cfg.nin_filters2), plane("A1", cfg.nin_filters)], dim=1)
     if s == 4:
         sc = "Up-PS2/Up-PS2_CNN"
-        a_up = act("Up-PS", cps, 2)
+        a_up = plane("Up-PS", cps, 2)
         ref, bar = wgrad_tc(sc + "/conv_W", a_up, dz_last, k, cps, 4 * ps_out, 2 * h, 2 * wd)
         chk.add("wgrad_tc Up-PS2", grad(sc + "/conv_W"), ref, bar, signed=True)
         conv_b(sc + "/conv_B", dz_last)
@@ -234,35 +239,58 @@ def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None):
     chk.add("dgrad twin Up-PS", dnin, v, bar)
 
     # ---- activation gradients
-    def act_grad(scope, c, g, layer_zneg):
-        zn = T("zneg:" + scope, (n, h, wd, c)) if layer_zneg else None
+    def act_grad(scope, c, g):
         mask = t64(eng.dropout_mask(scope, seed, n, h, wd, c).astype(np.float32)) if keep < 1.0 else 1.0
         inv_keep = float(np.float32(1.0) / np.float32(keep))
         gm = g * mask * inv_keep
-        alpha = torch.from_numpy(w["%s/prelu/%s_prelu" % (scope, scope)].astype(np.float32)).to(dev(), torch.float64)
-        neg = zn < 0
-        dz = torch.where(neg, gm * alpha.view(1, -1, 1, 1), gm)
+        chk.gm[scope] = gm
         got = T("dZ:" + scope, (n, h, wd, c))
-        chk.add("act_grad dZ", got, dz, 4 * U24 * dz.abs() + stored(dz))
+        if act in ("prelu", "leaky_relu"):    # the slope below zero, decided by the min(z, 0) plane
+            zn = T("zneg:" + scope, (n, h, wd, c))
+            neg = zn < 0
+            if act == "prelu":
+                slope = torch.from_numpy(w["%s/prelu/%s_prelu" % (scope, scope)].astype(np.float32)).to(dev(), torch.float64).view(1, -1, 1, 1)
+            else:
+                slope = LEAKY
+            dz = torch.where(neg, gm * slope, gm)
+            bar = 4 * U24 * dz.abs()
+        else:   # f'(h) at h = fp32(stored * fp32(keep)) of the GPU's own stored output (act_deriv_from_output)
+            hv = (torch.from_numpy(eng.get_activation(scope, (n, h, wd, c))).to(dev()) * torch.tensor(np.float32(keep), device=dev()))
+            hv = hv.permute(0, 3, 1, 2).double()
+            if act == "relu":
+                d, dbar = (hv > 0).double(), 0.0
+            elif act == "sigmoid":      # h * (1 - h): two roundings
+                d = hv * (1 - hv)
+                dbar = 2 * U24 * d.abs()
+            elif act == "tanh":         # 1 - h * h: the square's rounding, then the cancellation's
+                d = 1 - hv * hv
+                dbar = U24 * hv * hv + U24 * d.abs()
+            else:                       # selu: h + kSeluScaleAlpha below zero, kSeluScale (exact) above
+                d = torch.where(hv < 0, hv + SELU_SCALE_ALPHA, torch.full_like(hv, SELU_SCALE))
+                dbar = U24 * (hv < 0).double() * d.abs()
+            dz = gm * d
+            bar = (4 if act == "relu" else 5) * U24 * dz.abs() + gm.abs() * dbar
+        chk.add("act_grad dZ", got, dz, bar + stored(dz))
         conv_b(scope + "/conv_B", dz)
-        term = torch.where(neg, gm * zn, torch.zeros_like(gm))
-        pn = "%s/prelu/%s_prelu" % (scope, scope)
-        ref, bar = finalize(pn, term.sum(dim=(0, 2, 3)), (n * h * wd + 4) * U24 * term.abs().sum(dim=(0, 2, 3)))
-        chk.add("act_grad slope sums", grad(pn), ref, bar)
+        if act == "prelu":
+            term = torch.where(neg, gm * zn, torch.zeros_like(gm))
+            pn = "%s/prelu/%s_prelu" % (scope, scope)
+            ref, bar = finalize(pn, term.sum(dim=(0, 2, 3)), (n * h * wd + 4) * U24 * term.abs().sum(dim=(0, 2, 3)))
+            chk.add("act_grad slope sums", grad(pn), ref, bar)
         return got
 
     nin2 = cfg.nin_filters2
-    dz_a1 = act_grad("A1", cfg.nin_filters, dnin[:, nin2:], True)
-    dz_b2 = act_grad("B2", nin2, dnin[:, :nin2], True)
-    b1 = act("B1", nin2)
+    dz_a1 = act_grad("A1", cfg.nin_filters, dnin[:, nin2:])
+    dz_b2 = act_grad("B2", nin2, dnin[:, :nin2])
+    b1 = plane("B1", nin2)
     ref, bar = wgrad_tc("B2/conv_W", b1, dz_b2, 3, nin2, nin2, h, wd)
     chk.add("wgrad_tc B2", grad("B2/conv_W"), ref, bar, signed=True)
     (wq,) = quantise([w["B2/conv_W"]], 2)
     v, bar = twin("B2", dz_b2, wq, b1w, 3)
     db1 = T("dH:B2", (n, h, wd, nin2))
     chk.add("dgrad twin B2", db1, v, bar)
-    dz_b1 = act_grad("B1", nin2, db1, True)
-    feats = [act("CNN%d" % (i + 1), f[i]) for i in range(L)]
+    dz_b1 = act_grad("B1", nin2, db1)
+    feats = [plane("CNN%d" % (i + 1), f[i]) for i in range(L)]
     concat = torch.cat(feats, dim=1)
     feat_pitch = sum(pad16(c) for c in f)
     for nm, dz, cols in (("A1", dz_a1, cfg.nin_filters), ("B1", dz_b1, nin2)):
@@ -282,7 +310,7 @@ def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None):
         g = dcat[:, offs[i]:offs[i + 1]]
         if dnext is not None:
             g = g + dnext
-        dz = act_grad(sc, f[i], g, True)
+        dz = act_grad(sc, f[i], g)
         if i == 0:
             a = t64(x)
             ssum, sabs = wgrad(a, dz, k), wgrad(a.abs(), dz.abs(), k)

@@ -20,6 +20,9 @@ Tensor-core graphs are held to two references:
                         (conv_tc.cuh; the correction chain's truncations are 2^-10 of that, counted as one more step)
       fp32 CUDA cores   CNN1, R-CNN1 and the fused R-CNN1 gather: k^2 C 2^-24 S
       epilogue          scale + bias and the PReLU product, each rounded once: 2^-23 (S + |bias|)
+      activation        relu / leaky_relu as PReLU; sigmoid, tanh, selu: act_curve's libdevice error (CURVE_U) and the
+                        bar of z carried through max |f'| (activation); the train step's dropout: 2^-24 more, dropped
+                        elements exactly 0
 The fused R-CNN1 output is checked against R-CNN1(Up-PS_ref) + x2, where Up-PS_ref is the last pixel-shuffler layer
 computed from the GPU's own input to it; its accumulation bar is carried through |R-CNN1 filter|.
 
@@ -166,63 +169,115 @@ def prelu(h, alpha):
     return torch.where(h > 0, h, a * h)
 
 
-def isolated_layers(eng, cfg, w, x, x2, y, npl, seg, fused):
-    """{layer: max err / bar} of one forward whose activations `eng` still holds (see module docstring)."""
+# The kernels' fp32 constants (epilogue.cuh: kLeakySlope, kSeluScale, kSeluScaleAlpha).
+LEAKY = float(np.float32(0.1))
+SELU_SCALE = float(np.float32(1.0507009873554805))
+SELU_SCALE_ALPHA = float(np.float32(1.7580993408473766))
+# act_curve's error in units of 2^-24 |f|: sigmoid 1 / (1 + expf(-z)) (expf within 2 ulp, then the add and the divide),
+# tanhf within 2 ulp, selu kSeluScaleAlpha * expm1f(z) (expm1f within 1 ulp, then the product; z > 0 one product)
+CURVE_U = {"sigmoid": 6, "tanh": 4, "selu": 3}
+
+
+def activation(act, z, bar, alpha=None):
+    """(f(z), its bar) of an activated layer whose fp32 pre-activation lies within `bar` of the fp64 `z`.  prelu, relu
+    and leaky_relu have slope at most 1 and their slope product is one of the epilogue roundings `bar` counts; sigmoid,
+    tanh and selu add act_curve's libdevice error and carry `bar` through max |f'| over [z - bar, z + bar].  Sigmoid is
+    0 once expf(-z) overflows (z < -88), where f(z) < 2^-126."""
+    if act == "prelu":
+        return prelu(z, alpha), bar
+    if act == "relu":
+        return z.clamp_min(0.0), bar
+    if act == "leaky_relu":
+        return torch.where(z > 0, z, LEAKY * z), bar
+    near0 = torch.minimum(torch.maximum(torch.zeros_like(z), z - bar), z + bar)   # where f' peaks on the interval
+    floor = 0.0
+    if act == "sigmoid":
+        v, s0 = torch.sigmoid(z), torch.sigmoid(near0)
+        d, floor = s0 * (1 - s0), 2.0 ** -126
+    elif act == "tanh":
+        v, d = torch.tanh(z), 1 - torch.tanh(near0) ** 2
+    elif act == "selu":
+        v = torch.where(z < 0, SELU_SCALE_ALPHA * torch.expm1(z), SELU_SCALE * z)
+        d = SELU_SCALE_ALPHA * torch.exp(torch.clamp_max(z + bar, 0.0))     # >= kSeluScale once the interval reaches 0
+    else:
+        raise ValueError(act)
+    return v, d * bar + CURVE_U[act] * U24 * (v.abs() + d * bar) + floor
+
+
+def isolated_layers(eng, cfg, w, x, x2, y, npl, seg, fused, act="prelu", masks=None, keep=1.0, pre=None):
+    """{layer: max err / bar} of one forward whose activations `eng` still holds (see module docstring), for activator
+    `act`.  With `masks` ({layer: dropout_mask}, the train step's forward) a kept element's reference is
+    f(z) fp32(1 / keep), one more 2^-24 rounding, and a dropped element must be exactly 0.  `pre`, if given, receives
+    {activated layer: (fp64 pre-activation z, bar of the GPU's fp32 z)}."""
     n, h, wd = x.shape[:3]
     f = O.feature_filters(cfg)
     k = cfg.cnn_size
     cps = cfg.nin_filters + cfg.nin_filters2
     ps_out = cfg.pixel_shuffler_filters or cps
+    inv_keep = float(np.float32(1.0) / np.float32(keep))
     out = {}
 
-    def act(name, c, r=1):
+    def plane(name, c, r=1):
         return nchw(eng.get_activation(name, (n, r * h, r * wd, c)))
 
-    def check(name, got, ref, bar):
-        out[name] = float((np.abs(got - ref) / bar).max())
+    def check(name, got, ref, bar, dropped=None):
+        ratio = np.abs(got - ref) / (bar + 1e-300)     # the floor keeps an exact zero (bar 0) from giving 0 / 0
+        if dropped is not None:
+            ratio = np.where(dropped, np.where(got == 0, 0.0, np.inf), ratio)
+        out[name] = float(ratio.max())
 
-    def tc_layer(a, wq, b, alpha, kk, cin_pad):
-        """(value, accumulation + epilogue bar) of one tensor-core layer on the GPU's input `a`."""
+    def tc_layer(a, wq, b, kk, cin_pad):
+        """(pre-activation, accumulation + epilogue bar) of one tensor-core layer on the GPU's input `a`."""
         v = conv(a, wq) + torch.from_numpy(b.astype(np.float64)).view(1, -1, 1, 1)
         s = conv(a.abs(), np.abs(wq))
         bar = tc_units(kk, cin_pad, seg, npl) * U23 * s + U23 * (s + torch.from_numpy(np.abs(b).astype(np.float64)).view(1, -1, 1, 1))
-        if alpha is not None:
-            v = prelu(v, alpha)
         return v, bar
 
-    def store_check(name, got, v, bar):
+    def activated(scope, z, bar):
+        """(stored value, bar, dropped elements or None) of an activated layer from its pre-activation."""
+        if pre is not None:
+            pre[scope] = (z, bar)
+        alpha = w["%s/prelu/%s_prelu" % (scope, scope)] if act == "prelu" else None
+        v, bar = activation(act, z, bar, alpha)
+        if masks is None:
+            return v, bar, None
+        m = nchw(masks[scope])
+        v = v * inv_keep
+        return v * m, bar * inv_keep + U24 * v.abs(), (m == 0).numpy()
+
+    def store_check(name, got, v, bar, dropped=None):
         vn = v.numpy()
-        check(name, got.numpy(), vn, bar.numpy() + stored_rounding(vn, npl))
+        check(name, got.numpy(), vn, bar.numpy() + stored_rounding(vn, npl), dropped)
 
     # CNN1 (fp32 CUDA cores on x)
     a = nchw(x)
     w1 = w["CNN1/conv_W"].astype(np.float64)
     s = conv(a.abs(), np.abs(w1))
     b1 = w["CNN1/conv_B"].astype(np.float64)
-    v = prelu(conv(a, w1) + torch.from_numpy(b1).view(1, -1, 1, 1), w["CNN1/prelu/CNN1_prelu"])
-    bar = k * k * U24 * s + U23 * (s + torch.from_numpy(np.abs(b1)).view(1, -1, 1, 1))
-    feats = [act("CNN1", f[0])]
-    store_check("CNN1", feats[0], v, bar)
+    v, bar, dropped = activated("CNN1", conv(a, w1) + torch.from_numpy(b1).view(1, -1, 1, 1),
+                                k * k * U24 * s + U23 * (s + torch.from_numpy(np.abs(b1)).view(1, -1, 1, 1)))
+    feats = [plane("CNN1", f[0])]
+    store_check("CNN1", feats[0], v, bar, dropped)
     for i in range(1, cfg.layers):
         sc = "CNN%d" % (i + 1)
         (wq,) = quantise([w[sc + "/conv_W"]], npl)
-        v, bar = tc_layer(feats[-1], wq, w[sc + "/conv_B"], w["%s/prelu/%s_prelu" % (sc, sc)], k, pad16(f[i - 1]))
-        feats.append(act(sc, f[i]))
-        store_check(sc, feats[-1], v, bar)
+        v, bar, dropped = activated(sc, *tc_layer(feats[-1], wq, w[sc + "/conv_B"], k, pad16(f[i - 1])))
+        feats.append(plane(sc, f[i]))
+        store_check(sc, feats[-1], v, bar, dropped)
     # A1 and B1: one packed layer over the concat, one scale
     hc = torch.cat(feats, dim=1)
     wa, wb = quantise([w["A1/conv_W"], w["B1/conv_W"]], npl)
     cin_pad = sum(pad16(c) for c in f)
-    a1 = act("A1", cfg.nin_filters)
-    b1g = act("B1", cfg.nin_filters2)
-    v, bar = tc_layer(hc, wa, w["A1/conv_B"], w["A1/prelu/A1_prelu"], 1, cin_pad)
-    store_check("A1", a1, v, bar)
-    v, bar = tc_layer(hc, wb, w["B1/conv_B"], w["B1/prelu/B1_prelu"], 1, cin_pad)
-    store_check("B1", b1g, v, bar)
+    a1 = plane("A1", cfg.nin_filters)
+    b1g = plane("B1", cfg.nin_filters2)
+    v, bar, dropped = activated("A1", *tc_layer(hc, wa, w["A1/conv_B"], 1, cin_pad))
+    store_check("A1", a1, v, bar, dropped)
+    v, bar, dropped = activated("B1", *tc_layer(hc, wb, w["B1/conv_B"], 1, cin_pad))
+    store_check("B1", b1g, v, bar, dropped)
     (wq,) = quantise([w["B2/conv_W"]], npl)
-    v, bar = tc_layer(b1g, wq, w["B2/conv_B"], w["B2/prelu/B2_prelu"], 3, pad16(cfg.nin_filters2))
-    b2 = act("B2", cfg.nin_filters2)
-    store_check("B2", b2, v, bar)
+    v, bar, dropped = activated("B2", *tc_layer(b1g, wq, w["B2/conv_B"], 3, pad16(cfg.nin_filters2)))
+    b2 = plane("B2", cfg.nin_filters2)
+    store_check("B2", b2, v, bar, dropped)
     # pixel shuffler(s): the last one is fp32 (EPI_D2S_F32) or feeds the fused R-CNN1
     src, cin_pad = torch.cat([b2, a1], dim=1), pad16(cfg.nin_filters2) + pad16(cfg.nin_filters)
     stages = [("Up-PS", "Up-PS/Up-PS_CNN", 2, cps), ("Up-PS2", "Up-PS2/Up-PS2_CNN", 2, ps_out)] if cfg.scale == 4 else \
@@ -230,14 +285,14 @@ def isolated_layers(eng, cfg, w, x, x2, y, npl, seg, fused):
     mult = 1
     for si, (name, scope, r, c) in enumerate(stages):
         (wq,) = quantise([w[scope + "/conv_W"]], npl)
-        v, bar = tc_layer(src, wq, w[scope + "/conv_B"], None, k, cin_pad)
+        v, bar = tc_layer(src, wq, w[scope + "/conv_B"], k, cin_pad)
         v, bar = O.depth_to_space(v, r), O.depth_to_space(bar, r)
         mult *= r
         if si + 1 < len(stages):            # x4 Up-PS: fp16 planes
-            src, cin_pad = act(name, c, mult), pad16(c)
+            src, cin_pad = plane(name, c, mult), pad16(c)
             store_check(name, src, v, bar)
         elif not fused:
-            up = act(name, c, mult)
+            up = plane(name, c, mult)
             check(name, up.numpy(), v.numpy(), bar.numpy())
     # R-CNN1 + x2 (fp32)
     wr = w["R-CNN1/conv_W"].astype(np.float64)
