@@ -1,4 +1,4 @@
-"""The non-Adam optimizers of --optimizer (gd, momentum, adadelta, adagrad, rmsprop) on the GPU, against the fp64 rules of
+"""The optimizers of --optimizer (adam, gd, momentum, adadelta, adagrad, rmsprop) on the GPU, against the fp64 rules of
 tests/optimizer_oracle.py.
 
 Isolated kernel parity: the gradient buffer and the slots are set to chosen fp32 values, so the reference starts from the
@@ -9,6 +9,17 @@ Each rounds to within u = 2^-24 relative, and no step of any chain cancels (the 
 is added to the weight once at the end), so a result's error is at most (number of roundings) * u times the sum of the
 magnitudes of the terms that form it.  The bar is 32 u times that sum: the 1-ulp freedom of the fp32 square root of the
 fp64 norm sum (its summation order is the device's) is inside it.
+
+Adam (adam_kernel) is held to 16 u, from this count.  The reference takes the kernel's own constants: lr, beta1, beta2 and
+epsilon as the fp32 values the config holds (1 - beta is exact in fp32 for beta in [0.5, 1]), and lr_t in fp64 from
+them.  With M = beta1 |m| + (1 - beta1) |g|, V = beta2 v + (1 - beta2) g^2 and S = lr_t M / (sqrt(V) + eps):
+  m:  two products and a sum, 3 roundings of M (the two terms may cancel), and 1 more from g's clip-scale freedom;
+  v:  g * g, two products and a sum, 4 roundings of V (no cancellation), and 2 more from g;
+  w:  lr_t rounded once from fp64 (1), m (4), sqrt(v) (1 + half of v's 6 = 4), + eps (1), lr_t * m (1) and the division
+      (1): 12 roundings of S, then w - step, 1 rounding of |w| + S.
+So every output is within 13 u of its sum of term magnitudes (|w| + S, M, V), which the bar of 16 u covers.  Forming
+lr_t in fp32 instead (powf, sqrtf) cancels in 1 - beta2^t: at t = 2 that alone is 56 u of S, so the step cases where S
+dominates |w| see it.
 
 End-to-end steps: the gradient of each tensor is within delta = 2e-3 * max|g| of fp64 autograd (2e-4 on depthwise-
 separable graphs), the bar test_gradients_match_oracle and test_depthwise_separable_gradients_match_oracle establish;
@@ -40,11 +51,12 @@ DS4 = dict(scale=4, layers=4, filters=14, min_filters=5, filters_decay_gamma=1.2
 MU = 0.9
 
 
-def _engine(kw, kind, keep=0.8, clip=5.0, seed=3):
+def _engine(kw, kind, keep=0.8, clip=5.0, seed=3, **adam):
+    """`adam`: beta1 / beta2 / epsilon of the engine config (make_config's defaults otherwise)."""
     from helper import engine as E
     cfg = O.OracleConfig(**kw)
     wts = {k: v.astype(np.float64) for k, v in O.he_init_weights(cfg, seed=seed).items()}
-    eng = E.Engine(E.make_config(dropout_keep=keep, clipping_norm=clip, optimizer=kind, momentum=MU, **kw))
+    eng = E.Engine(E.make_config(dropout_keep=keep, clipping_norm=clip, optimizer=kind, momentum=MU, **kw, **adam))
     eng.set_params({k: v.astype(np.float32) for k, v in wts.items()})
     return cfg, wts, eng
 
@@ -58,9 +70,13 @@ def _batch(cfg, n, h, w, seed):
     return x, x2, y
 
 
-def _terms(kind, w, g, s, lr):
+def _terms(kind, w, g, s, lr, **adam):
     """Sum of the magnitudes of the terms forming each output (new w, then each new slot), float64."""
     aw, ag = np.abs(w), np.abs(g)
+    if kind == "adam":
+        b1, b2 = adam["beta1"], adam["beta2"]
+        mm, vv = b1 * np.abs(s[0]) + (1 - b1) * ag, b2 * s[1] + (1 - b2) * g * g
+        return [aw + OO.adam_lr(lr, adam["t"], b1, b2) * mm / (np.sqrt(vv) + adam["epsilon"]), mm, vv]
     w1, s1 = OO.update(kind, w, g, s, lr, MU)
     if kind == "gd":
         return [aw + lr * ag]
@@ -75,14 +91,54 @@ def _terms(kind, w, g, s, lr):
     return [aw + mom, s1[0], mom]
 
 
-KERNEL_CASES = [(k, m) for k in KINDS for m in ("noclip", "clip", "avg")]
+def rule_errors(kind, eng, w0, s0, gc, lr, rule):
+    """Every weight and slot of `eng` after one update of weights w0 and slots s0 (fp32, per variable) with the flat
+    clipped fp32 gradient gc, against the fp64 rule at the module docstring's bar (16 u for adam, 32 u for the others).
+    `rule`: adam's t / beta1 / beta2 / epsilon.  Returns ([(variable, output, error / bar)] of the violations, the
+    largest error / bar)."""
+    nu = 16 if kind == "adam" else 32
+    shapes = eng.param_shapes()
+    off, bad, worst = 0, [], 0.0
+    for n in shapes:
+        k = int(np.prod(shapes[n]))
+        g = gc[off:off + k].reshape(shapes[n]).astype(np.float64)
+        off += k
+        s = [a.astype(np.float64) for a in s0[n]]
+        want = OO.update(kind, w0[n].astype(np.float64), g, s, lr, MU, **rule)
+        bars = _terms(kind, w0[n].astype(np.float64), g, s, lr, **rule)
+        got = [eng.get_param(n)] + [eng.get_optimizer_slot(n, i) for i in range(len(s))]
+        for j, (gv, wv, b) in enumerate(zip(got, [want[0]] + want[1], bars)):
+            ratio = np.abs(gv.astype(np.float64) - wv) / (nu * U * b + 1e-44)
+            worst = max(worst, float(ratio.max()))
+            if not (ratio <= 1).all():
+                bad.append((n, j, float(ratio.max())))
+    assert off == gc.size
+    return bad, worst
 
 
-@pytest.mark.parametrize("kind,mode", KERNEL_CASES, ids=["%s-%s" % c for c in KERNEL_CASES])
-def test_optimizer_kernel_matches_fp64_rule(kind, mode):
-    """One update from chosen gradients and slots: zeros, tiny (1e-20), ordinary and large (1e3) values of both signs,
-    with clipping off, with clipping that triggers, and through apply_gradients_avg with grad_scale = 0.5."""
-    cfg, _, eng = _engine(SMALL, kind, clip=0.0 if mode == "noclip" else 5.0)
+def adam_rule(t, beta1=0.9, beta2=0.999, epsilon=1e-8):
+    """OO.update's adam arguments for update t of an engine configured with these values: the fp32 values it holds."""
+    f32 = lambda a: float(np.float32(a))
+    return dict(t=t, beta1=f32(beta1), beta2=f32(beta2), epsilon=f32(epsilon))
+
+
+ADAM_CFG = dict(beta1=0.5, beta2=0.9, epsilon=1e-3)      # not the defaults: a constant baked into the kernel fails
+KERNEL_CASES = ([(k, m, None, {}) for k in KINDS + ("adam",) for m in ("noclip", "clip", "avg")]
+                + [("adam", "clip", t, {}) for t in (0, 1, 9, 999, 10 ** 6)] + [("adam", "clip", 1, ADAM_CFG)])
+
+
+def _kernel_id(c):
+    kind, mode, t, adam = c
+    return "%s-%s" % (kind, mode) + ("" if t is None else "-t%d" % t) + ("-b0.5-0.9-e1e-3" if adam else "")
+
+
+@pytest.mark.parametrize("kind,mode,t0,adam", KERNEL_CASES, ids=[_kernel_id(c) for c in KERNEL_CASES])
+def test_optimizer_kernel_matches_fp64_rule(kind, mode, t0, adam):
+    """One update from chosen gradients and slots: zeros, tiny (1e-20), ordinary and large (1e3) values of both signs
+    (Adam's v: of one sign), with clipping off, with clipping that triggers, and through apply_gradients_avg with
+    grad_scale = 0.5.  Adam also starts from update counts set through set_adam_step (the checkpoint-resume path: the
+    update is then number t0 + 1) and from a non-default beta1 / beta2 / epsilon."""
+    cfg, _, eng = _engine(SMALL, kind, clip=0.0 if mode == "noclip" else 5.0, **adam)
     x, x2, y = _batch(cfg, 1, 8, 8, 1)
     eng.train_step_host(x, x2, y, lr=0.01, seed=1, apply_update=False)
     shapes = eng.param_shapes()
@@ -100,14 +156,20 @@ def test_optimizer_kernel_matches_fp64_rule(kind, mode):
         w0[n] = eng.get_param(n)
         s0[n] = []
         for i, init in enumerate(OO.SLOT_INIT[kind]):
-            if (kind, i) in (("momentum", 0), ("rmsprop", 1)):       # signed slots
+            if kind == "adam":                                        # m signed, v >= 0, the gradients' magnitudes
+                v = np.choose(r.randint(0, 4, k), [np.zeros(k), np.full(k, 1e-20), 10.0 ** r.uniform(-4, 0, k),
+                                                   10.0 ** r.uniform(2, 3, k)])
+                v = v * np.where(r.rand(k) < 0.5, -1.0, 1.0) if i == 0 else v
+            elif (kind, i) in (("momentum", 0), ("rmsprop", 1)):     # signed slots
                 v = r.randn(k) * 10.0 ** r.uniform(-4, 0, k)
             else:                                                     # accumulators: positive
                 v = 10.0 ** r.uniform(-3, 0, k)
             s0[n].append(v.astype(np.float32).reshape(shapes[n]))
-            eng.set_optimizer_slot(n, i, s0[n][i])
+            (eng.set_adam_slot if kind == "adam" else eng.set_optimizer_slot)(n, i, s0[n][i])
         off += k
     assert off == total
+    if t0 is not None:
+        eng.adam_step = t0
     lr = 0.01
     if mode == "avg":
         eng.apply_gradients_avg(lr, 0.5)
@@ -116,26 +178,20 @@ def test_optimizer_kernel_matches_fp64_rule(kind, mode):
         eng.apply_gradients(lr)
         g32 = raw
     torch.cuda.synchronize()
+    rule = {}
+    if kind == "adam":
+        assert eng.adam_step == (t0 or 0) + 1
+        rule = adam_rule((t0 or 0) + 1, **adam)
+        lr = float(np.float32(lr))                                    # the fp32 lr the ABI passes
     scale = np.float32(1.0)
     if mode != "noclip":
         norm = np.float32(np.sqrt(np.sum(g32.astype(np.float64) ** 2)))
         assert norm > 5.0                                             # the clip triggers
         scale = np.float32(5.0) / max(norm, np.float32(5.0))
     gc = (g32 * scale).astype(np.float32)
-    off, bad = 0, []
-    for n in names:
-        k = int(np.prod(shapes[n]))
-        g = gc[off:off + k].reshape(shapes[n]).astype(np.float64)
-        off += k
-        s = [a.astype(np.float64) for a in s0[n]]
-        want = OO.update(kind, w0[n].astype(np.float64), g, s, lr, MU)
-        bars = _terms(kind, w0[n].astype(np.float64), g, s, lr)
-        got = [eng.get_param(n)] + [eng.get_optimizer_slot(n, i) for i in range(len(s))]
-        for j, (gv, wv, b) in enumerate(zip(got, [want[0]] + want[1], bars)):
-            err = np.abs(gv.astype(np.float64) - wv)
-            if not (err <= 32 * U * b + 1e-44).all():
-                bad.append((n, j, float((err / (32 * U * b + 1e-44)).max())))
+    bad, worst = rule_errors(kind, eng, w0, s0, gc, lr, rule)
     eng.close()
+    print("%s: largest error / bar: %.3f" % (_kernel_id((kind, mode, t0, adam)), worst))
     assert not bad, bad[:8]
 
 
@@ -249,6 +305,53 @@ def test_gd_step_that_shrinks_a_layer_past_its_packed_scale_falls_back_to_the_ho
     assert np.abs(fresh.forward_host(x, x2) - yy).max() <= 1e-5
     fresh.close()
     eng.close()
+
+
+GROW_CASES = [("Up-PS", None, "Up-PS/Up-PS_CNN/conv_W"),
+              # R-CNN1 itself is an fp32 gather: only the folded upsampler's image (its wmax slot) leaves its window
+              ("R-CNN1-folded-L12-x2", "dcscn_L12_F196to48_NIN_A64_PS_R1F32", "R-CNN1/conv_W")]
+
+
+@pytest.mark.parametrize("weights,target", [c[1:] for c in GROW_CASES], ids=[c[0] for c in GROW_CASES])
+def test_gd_step_that_grows_a_layer_past_its_packed_scale_falls_back_to_the_host_repack(weights, target):
+    """The other edge of the window: a gd step with gradient -w on one variable and lr 7 multiplies it by 8.  The packed
+    scale put max |w * scale| in (8192, 16384]; eight times that is past 49152, and past fp16's 65504, so the old scale
+    would pack inf (four times would stay finite where max |w * scale| <= 16376).  The host re-pack takes over: the
+    forward matches fp64 on the new weights and a fresh engine packed from them.  Inputs in [0, 1] keep the fp64 bar of
+    the shrink test meaningful at the full L12 width."""
+    from conftest import MODEL_FLAGS, load_golden_weights
+    from helper import engine as E
+    kw = SMALL if weights is None else MODEL_FLAGS[weights]
+    cfg = O.OracleConfig(**kw)
+    w = O.he_init_weights(cfg, seed=3) if weights is None else load_golden_weights(weights)
+    eng = E.Engine(E.make_config(dropout_keep=1.0, clipping_norm=0.0, optimizer="gd", **kw))
+    eng.set_params(w)
+    x, x2, y = (a / np.float32(255) for a in _batch(cfg, 1, 10, 12, 4))
+    eng.train_step_host(x, x2, y, lr=0.0, seed=1)               # first update: host pack, then the device refresh maps
+    eng.train_step_host(x, x2, y, lr=0.0, seed=2)               # an update through the device refresh
+    eng.train_step_host(x, x2, y, lr=0.0, seed=3, apply_update=False)
+    shapes = eng.param_shapes()
+    before = {k: eng.get_param(k) for k in shapes}
+    g = np.concatenate([(-before[k] if k == target else np.zeros_like(before[k])).ravel() for k in shapes])
+    gt = eng.grad_tensor()
+    gt[:g.size] = torch.from_numpy(g).to(gt.device)
+    eng.apply_gradients(7.0)
+    torch.cuda.synchronize()
+    after = {k: eng.get_param(k) for k in shapes}
+    np.testing.assert_allclose(after[target], before[target] * 8, rtol=2.0 ** -22, atol=0)
+    assert all(np.array_equal(after[k], before[k]) for k in shapes if k != target)
+    yy = eng.forward_host(x, x2)
+    assert np.isfinite(yy).all()
+    ref = O.Oracle(cfg, {k: v.astype(np.float64) for k, v in after.items()}, torch.float64).forward(x.astype(np.float64), x2.astype(np.float64))
+    err = float(np.abs(yy - ref).max())
+    fresh = E.Engine(E.make_config(dropout_keep=1.0, **kw))
+    fresh.set_params(after)
+    err_host = float(np.abs(fresh.forward_host(x, x2) - yy).max())
+    fresh.close()
+    eng.close()
+    print("%s x8: max |y - oracle(fp64)| = %.3e, max |y - fresh host pack| = %.3e" % (target, err, err_host))
+    assert err <= 1e-3
+    assert err_host <= 1e-5
 
 
 # ------------------------------------------------------------------------------------------------- checkpoints ----

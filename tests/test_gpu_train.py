@@ -193,37 +193,6 @@ def test_adam_step_matches_oracle_and_loss_decreases():
     eng.close()
 
 
-@pytest.mark.parametrize("kw,weights", [(SMALL, "he"), (SMALL4, "he"), (SMALL3, "he"), (K5, "he"), (None, CDCSCN[3])],
-                         ids=["x2", "x4", "x3", "k5-x2", "cdcscn-x3"])
-def test_device_refresh_equals_host_repack(kw, weights):
-    """After an optimizer step the packed tensor-core weight images (forward layers and dgrad twins), fused bias / PReLU
-    vectors and the CNN1 / R-CNN1 filters are refreshed on the device through index maps derived from the host packing
-    code.  A fresh engine that packs the same weights on the host must give the same forward output and the same
-    gradients (only the power-of-two weight scale may differ, which is exact).  The cases cover 3x3 and 5x5 twins, a
-    9-column Up-PS (x3 with one R-CNN1 input channel) and a one-channel R-CNN1 filter."""
-    from helper import engine as E
-    if weights != "he":
-        kw = MODEL_FLAGS[weights]
-    cfg, wts, eng, x, x2, y = setup(kw, 0.8, 2, 12, 14, seed=3, weights=weights)
-    for i in range(4):
-        eng.train_step_host(x, x2, y, lr=0.01, seed=50 + i)
-    y_dev = eng.forward_host(x, x2)
-    eng.train_step_host(x, x2, y, lr=0.01, seed=99, apply_update=False)
-    params = {n: eng.get_param(n) for n in wts}
-    grads_dev = {n: eng.get_grad(n) for n in wts}
-    assert any(np.abs(params[n] - wts[n]).max() > 1e-3 for n in wts)      # the weights did move
-    fresh = E.Engine(E.make_config(dropout_keep=0.8, **kw))
-    fresh.set_params(params)
-    y_host = fresh.forward_host(x, x2)
-    fresh.train_step_host(x, x2, y, lr=0.01, seed=99, apply_update=False)
-    assert np.abs(y_dev - y_host).max() <= 1e-5
-    for n in wts:
-        g = fresh.get_grad(n)
-        assert np.abs(g - grads_dev[n]).max() <= 1e-4 * np.abs(g).max() + 1e-9, n   # fp32 atomics reorder sums
-    eng.close()
-    fresh.close()
-
-
 def test_train_step_refuses_f16x1_and_handle_keeps_working():
     """The train step needs the fp16x3 operand planes of the tensor-core graph: an f16x1 engine refuses it with
     EngineError, and the refusal leaves the handle as it was, so the forward still runs and gives the same output."""
@@ -449,3 +418,170 @@ def test_depthwise_separable_adam_steps_and_forward_follow():
     more = [eng.train_step_host(x, x2, y, lr=0.002, seed=400 + i)[1] for i in range(40)]
     assert np.mean(more[-5:]) < first
     eng.close()
+
+
+# ------------------------------------------------------------------------------------------ device refresh ----
+def train_tensors(eng, names):
+    """{name: fp32 values} of those of `names` the last capture step kept.  dcscn_get_train_tensor refuses a wrong
+    element count with "'<name>' has <count> elements", and a name it did not capture with "no tensor": the count of
+    each kept tensor is read from the first refusal."""
+    import re
+    from helper import engine as E
+    out = {}
+    for name in names:
+        try:
+            out[name] = eng.get_train_tensor(name, (1,))
+        except E.EngineError as e:
+            m = re.search(r"has (\d+) elements", str(e))
+            if m:
+                out[name] = eng.get_train_tensor(name, (int(m.group(1)),))
+            else:
+                assert "no tensor" in str(e), str(e)
+    return out
+
+
+def scale_exponent(img):
+    """pack_tc_layer's power-of-two weight scale of a packed image: 2^floor(log2(16384 / max |w|))."""
+    return int(np.floor(np.log2(16384.0 / float(np.abs(img).max()))))
+
+
+def composed(p, scope):
+    """The filter a layer packs: fp32(depthwise * pointwise) on a wide depthwise-separable graph, else its conv_W."""
+    if scope + "/depthwise_W" not in p:
+        return p[scope + "/conv_W"]
+    dw, pw = p[scope + "/depthwise_W"], p[scope + "/pointwise_W"]
+    return (dw[:, :, :, :1] * pw[0, 0][None, None]).astype(np.float32)
+
+
+def folded_image(p, kw, scope):
+    """The folded last upsampler's filter as build_fold / fold_kernel form it (tests/test_fold_cpu.py fold32)."""
+    from test_fold_cpu import fold32
+    wr = composed(p, "R-CNN1")
+    c = wr.shape[2]
+    if scope == "Up-TCNN":
+        import tconv_oracle as T
+        w = T.tconv_filter(p["Up-TCNN/Tconv_W"], kw["scale"])
+        return fold32(w, np.zeros(w.shape[-1], np.float32), wr, c)[0]
+    return fold32(composed(p, scope), p[scope + "/conv_B"], wr, c)[0]
+
+
+L12 = {2: "dcscn_L12_F196to48_NIN_A64_PS_R1F32", 4: "dcscn_L12_F196to48_Sc4_NIN_A64_PS_R1F32"}
+TCONV = dict(layers=4, filters=40, min_filters=24, filters_decay_gamma=1.5, nin_filters=32, nin_filters2=16,
+             transposed_upsampler=True)
+DS_WIDE = dict(scale=2, layers=3, filters=12, min_filters=6, nin_filters=32, nin_filters2=16, pixel_shuffler_filters=1,
+               depthwise_separable=True)
+_GC = {c[0]: c for c in GRADIENT_CASES}
+REFRESH_CASES = [
+    # id, config, weights
+    ("x2", SMALL, "he"), ("x4", SMALL4, "he"), ("x3", SMALL3, "he"), ("k5-x2", K5, "he"), ("cdcscn-x3", None, CDCSCN[3]),
+    ("L12-x2-fold", None, L12[2]), ("L12-x4-fold", None, L12[4]),                    # the fold on Up-PS / Up-PS2
+    ("x8", dict(SMALL, scale=8), "he"),
+    ("tconv-x2", dict(TCONV, scale=2), "he"), ("tconv-x3", dict(TCONV, scale=3), "he"),
+    ("ds-narrow", DS2, "he"), ("ds-wide", DS_WIDE, "he"),
+    ("relu", dict(SMALL, activator="relu"), "he"), ("sigmoid", dict(SMALL, activator="sigmoid"), "he"),
+    ("cnn1-272", _GC["cnn1-272"][1], "he"), ("ps144", _GC["ps144-x2"][1], "he"),
+]
+# the fp32 tensors of the depthwise-separable step (train_ds.inc).  Its atomic kernels (ds_colsum, ds_dpw, ds_ddw) write
+# filter gradients only, so every one of these must be bit-identical too.
+DS_TENSORS = ("U:", "Z:", "H:", "E:", "dZ:", "dU:", "dH:")
+
+
+@pytest.mark.parametrize("kw,weights", [c[1:] for c in REFRESH_CASES], ids=[c[0] for c in REFRESH_CASES])
+def test_device_refresh_equals_host_repack(kw, weights):
+    """After an optimizer step the packed tensor-core weight images (forward layers and dgrad twins, the folded last
+    upsampler), fused bias / slope vectors, the CNN1 / R-CNN1 filters and the depthwise-separable filters are refreshed
+    on the device (repack_kernel, fold_kernel, gather_params_kernel, ds_compose) through index maps derived from the
+    host packing code.  A fresh engine that packs the same weights on the host must compute the same bits.
+
+    The step is gd (no clip, lr 1) from a chosen gradient: every weight moves by a random relative step of at most
+    1e-3 and no element grows past its variable's largest magnitude, whose own gradient is 0.  So no image's
+    power-of-two scale changes (asserted for the images formed from products: the fold and the composed wide
+    depthwise-separable filters), and the device images must equal the host's bit for bit: the forward output and one
+    capture step's y_, dY and every dZ / dH plane (non-atomic kernels) are compared with array_equal; the filter
+    gradients, summed by fp32 atomics in any order, keep a 1e-4 bar."""
+    from helper import engine as E
+    import tconv_oracle as T
+    if weights != "he":
+        kw = MODEL_FLAGS[weights]
+    n, h, w = 2, 10, 12
+    s = kw["scale"] if "scale" in kw else 2
+    ocfg = {k: v for k, v in kw.items() if k not in ("activator", "transposed_upsampler")}
+    if weights != "he":
+        src = load_golden_weights(weights)
+    elif kw.get("transposed_upsampler"):
+        src = T.random_weights(T.Config(**ocfg), seed=3)
+    else:
+        src = O.he_init_weights(O.OracleConfig(**ocfg), seed=3)
+
+    def engine():
+        return E.Engine(E.make_config(dropout_keep=0.8, clipping_norm=0.0, optimizer="gd", **kw))
+    eng = engine()
+    shapes = eng.param_shapes()
+    eng.set_params({k: src[k] for k in shapes})
+    g = np.random.RandomState(4)
+    x = (g.rand(n, h, w, 1) * 255).astype(np.float32)
+    x2 = (g.rand(n, s * h, s * w, 1) * 255).astype(np.float32)
+    y = np.clip(x2 + g.randn(n, s * h, s * w, 1) * 10, 0, 255).astype(np.float32)
+    eng.train_step_host(x, x2, y, lr=0.0, seed=1)                   # first update: host pack, then the refresh maps
+    eng.train_step_host(x, x2, y, lr=0.0, seed=2, apply_update=False)
+    before = {k: eng.get_param(k) for k in shapes}
+    r = np.random.RandomState(5)
+    grads = []
+    for k in shapes:
+        wv = before[k].ravel()
+        step = r.uniform(-1e-3, 1e-3, wv.size)
+        step = np.where(np.abs(wv) * (1 + 2e-3) > np.abs(wv).max(), -np.abs(step), step)   # never past the largest
+        gv = (-wv * step).astype(np.float32)
+        gv[np.argmax(np.abs(wv))] = 0.0
+        grads.append(gv)
+    gflat = np.concatenate(grads)
+    gt = eng.grad_tensor()
+    gt[:gflat.size] = torch.from_numpy(gflat).to(gt.device)
+    eng.apply_gradients(1.0)
+    torch.cuda.synchronize()
+    after = {k: eng.get_param(k) for k in shapes}
+    off = 0
+    for k in shapes:
+        m = after[k].size
+        assert np.array_equal(after[k].ravel(), before[k].ravel() - gflat[off:off + m]), k      # w - 1 * g, one rounding
+        assert np.abs(after[k]).max() == np.abs(before[k]).max(), k
+        off += m
+    assert any(not np.array_equal(after[k], before[k]) for k in shapes)
+    for k in shapes:                                            # images formed from products keep their scale too
+        if k.endswith("/depthwise_W"):
+            sc = k[:-len("/depthwise_W")]
+            assert scale_exponent(composed(after, sc)) == scale_exponent(composed(before, sc)), sc
+    eng.set_option("grad_capture", 1)
+    y_dev = eng.forward_host(x, x2)
+    folded = True
+    try:
+        eng.get_activation("R-CNN1/taps", (1, 9, n, s * h, s * w))
+    except E.EngineError:
+        folded = False
+    if folded:
+        up = "Up-TCNN" if kw.get("transposed_upsampler") else ("Up-PS2/Up-PS2_CNN" if s == 4 else "Up-PS/Up-PS_CNN")
+        assert scale_exponent(folded_image(after, kw, up)) == scale_exponent(folded_image(before, kw, up))
+    eng.train_step_host(x, x2, y, lr=0.0, seed=99, apply_update=False)
+    fresh = engine()
+    fresh.set_params(after)
+    fresh.set_option("grad_capture", 1)
+    # a step first makes the fresh handle a training one: a wide depthwise-separable graph then packs its composed
+    # filters, as the trained handle does
+    fresh.train_step_host(x, x2, y, lr=0.0, seed=99, apply_update=False)
+    y_host = fresh.forward_host(x, x2)
+    assert np.array_equal(y_dev, y_host), float(np.abs(y_dev - y_host).max())
+    scopes = [t[0] for t in O.layer_table(O.OracleConfig(**ocfg))]
+    scopes += [sc.split("/")[0] for sc in scopes] + ["A1+B1", "Up-TCNN"]
+    prefixes = ("dZ:", "dH:") + (DS_TENSORS if kw.get("depthwise_separable") else ())
+    names = ["y_", "dY"] + sorted({p + sc for p in prefixes for sc in scopes})
+    got, want = train_tensors(eng, names), train_tensors(fresh, names)
+    assert set(got) == set(want)
+    assert {"y_", "dY"} <= set(got) and sum(k.startswith("dZ:") for k in got) >= 3, sorted(got)
+    differ = [k for k in got if not np.array_equal(got[k], want[k])]
+    assert not differ, differ
+    for k in shapes:
+        gh, gd = fresh.get_grad(k), eng.get_grad(k)
+        assert np.abs(gh - gd).max() <= 1e-4 * np.abs(gh).max() + 1e-9, k   # fp32 atomics reorder sums
+    print("%d train tensors bit-identical: %s" % (len(got), " ".join(sorted(got))))
+    eng.close()
+    fresh.close()

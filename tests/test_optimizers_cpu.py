@@ -1,5 +1,5 @@
-"""The non-Adam optimizers without a GPU: the fp64 oracle (tests/optimizer_oracle.py) against torch.optim where torch has
-the same rule, rmsprop against its formula, the checkpoint slot names, and the --optimizer flag handling."""
+"""The optimizers without a GPU: the fp64 oracle (tests/optimizer_oracle.py) against torch.optim where torch has the same
+rule, rmsprop and adam against their formulas, the checkpoint slot names, and the --optimizer flag handling."""
 import numpy as np
 import pytest
 import torch
@@ -66,6 +66,45 @@ def test_rmsprop_follows_tf_formula_not_torch():
     assert np.abs(p.detach().numpy() - got).max() > 1e-3
 
 
+@pytest.mark.parametrize("betas", [(0.9, 0.999, 1e-8), (0.5, 0.9, 1e-3)], ids=["default", "custom"])
+def test_adam_follows_oracle_adam_step_and_tf_formula_not_torch(betas):
+    """TF's Adam: lr_t = lr sqrt(1 - b2^t) / (1 - b1^t), m = b1 m + (1 - b1) g, v = b2 v + (1 - b2) g^2,
+    w -= lr_t m / (sqrt(v) + eps), with eps outside the root and after the bias correction of lr_t.  The oracle's `update`
+    must take the steps `Oracle.adam_step` takes (whose t is the update number) and a literal loop takes.
+    torch.optim.Adam divides by sqrt(v_hat) + eps: a different optimizer wherever eps matters."""
+    import dcscn_oracle as O
+    b1, b2, eps = betas
+    grads, w0 = _grads(2)
+    w, slots = w0.copy(), [np.zeros_like(w0), np.zeros_like(w0)]
+    for t, g in enumerate(grads, start=1):
+        w, slots = OO.update("adam", w, g, slots, LR, t=t, beta1=b1, beta2=b2, epsilon=eps)
+    lw, m, v = w0.copy(), np.zeros_like(w0), np.zeros_like(w0)
+    for t, g in enumerate(grads, start=1):
+        lr_t = LR * np.sqrt(1 - b2 ** t) / (1 - b1 ** t)
+        for i in range(lw.size):
+            m[i] = b1 * m[i] + (1 - b1) * g[i]
+            v[i] = b2 * v[i] + (1 - b2) * g[i] * g[i]
+            lw[i] = lw[i] - lr_t * m[i] / (np.sqrt(v[i]) + eps)
+    np.testing.assert_allclose(w, lw, rtol=1e-14, atol=1e-15)
+    np.testing.assert_allclose(slots[0], m, rtol=1e-14, atol=1e-300)
+    np.testing.assert_allclose(slots[1], v, rtol=1e-14, atol=1e-300)
+    orc = O.Oracle(O.OracleConfig(beta1=b1, beta2=b2, epsilon=eps), {"a": w0.copy()}, torch.float64)
+    om, ov = {"a": np.zeros_like(w0)}, {"a": np.zeros_like(w0)}
+    for t, g in enumerate(grads, start=1):
+        orc.adam_step({"a": g}, om, ov, t, LR)
+    np.testing.assert_allclose(orc.w["a"], w, rtol=1e-14, atol=1e-15)
+    # resuming at update t: the bias correction of the t-th update, not of the first
+    w3, _ = OO.update("adam", w0, grads[0], [m, v], LR, t=3, beta1=b1, beta2=b2, epsilon=eps)
+    w1, _ = OO.update("adam", w0, grads[0], [m, v], LR, t=1, beta1=b1, beta2=b2, epsilon=eps)
+    assert np.abs(w3 - w1).max() > 1e-4 * LR
+    p = torch.tensor(w0, dtype=torch.float64, requires_grad=True)
+    opt = torch.optim.Adam([p], lr=LR, betas=(b1, b2), eps=eps)
+    for g in grads:
+        p.grad = torch.tensor(g, dtype=torch.float64)
+        opt.step()
+    assert np.abs(p.detach().numpy() - w).max() > 1e-6 * LR
+
+
 def test_adadelta_update_uses_the_old_accum_update():
     w, slots = OO.update("adadelta", np.zeros(1), np.ones(1), [np.zeros(1), np.full(1, 4.0)], lr=1.0)
     acc = 0.05
@@ -83,7 +122,7 @@ def test_slot_table_names_and_initial_values():
     assert E.OPTIMIZER_SLOTS["adagrad"] == (("/Adagrad", 0.1),)
     assert E.OPTIMIZER_SLOTS["adadelta"] == (("/Adadelta", 0.0), ("/Adadelta_1", 0.0))
     assert E.OPTIMIZER_SLOTS["rmsprop"] == (("/RMSProp", 1.0), ("/RMSProp_1", 0.0))
-    for kind in OO.KINDS:
+    for kind in OO.KINDS + ("adam",):
         assert tuple(v for _, v in E.OPTIMIZER_SLOTS[kind]) == OO.SLOT_INIT[kind]
     c = E.make_config(optimizer="rmsprop", momentum=0.5)
     assert (c.optimizer, c.momentum) == (5, 0.5)
