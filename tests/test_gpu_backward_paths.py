@@ -141,6 +141,28 @@ class Checker:
         return [(k, v) for k, v in self.worst.items() if not v <= 1.0]
 
 
+def output_gradient(cfg, scope, plane):
+    """The gradient reaching the output of activated layer `scope` in a captured train step, before dropout, from the
+    step's captured planes: `plane(tensor, channels)` returns "dH:Up-PS" (split into B2 | A1), "dH:B2", "dH:A1+B1" (the
+    concatenated CNN outputs) or "dH:CNN<j>" (the gradient CNN<j> passes back to CNN<j-1>) as an fp64 NCHW tensor."""
+    f = O.feature_filters(cfg)
+    nin2 = cfg.nin_filters2
+    if scope in ("A1", "B2"):
+        g = plane("dH:Up-PS", cfg.nin_filters + nin2)
+        return g[:, nin2:] if scope == "A1" else g[:, :nin2]
+    if scope == "B1":
+        return plane("dH:B2", nin2)
+    j = int(scope[3:])
+    offs = np.cumsum([0] + f)
+    g = plane("dH:A1+B1", sum(f))[:, offs[j - 1]:offs[j]]
+    return g + plane("dH:CNN%d" % (j + 1), f[j - 1]) if j < cfg.layers else g
+
+
+def after_dropout(g, mask, keep):
+    """g mask fp32(1 / keep): the gradient of an activated layer's output before its dropout (`mask` None at keep 1)."""
+    return g * (1.0 if mask is None else mask) * float(np.float32(1.0) / np.float32(keep))
+
+
 def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None, act="prelu"):
     """Every backward kernel of the last train step of `eng` (run with grad_capture = 1, activator `act`) against its
     isolated reference.  `get_grad(name)` returns a variable's gradient as get_grad does (default: eng.get_grad); a wide
@@ -239,10 +261,12 @@ def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None, act="prelu"
     chk.add("dgrad twin Up-PS", dnin, v, bar)
 
     # ---- activation gradients
-    def act_grad(scope, c, g):
-        mask = t64(eng.dropout_mask(scope, seed, n, h, wd, c).astype(np.float32)) if keep < 1.0 else 1.0
-        inv_keep = float(np.float32(1.0) / np.float32(keep))
-        gm = g * mask * inv_keep
+    captured = {}     # the captured planes output_gradient reads, as they are fetched below
+
+    def act_grad(scope, c):
+        g = output_gradient(cfg, scope, lambda name, _: captured[name])
+        gm = after_dropout(g, t64(eng.dropout_mask(scope, seed, n, h, wd, c).astype(np.float32)) if keep < 1.0 else None,
+                           keep)
         chk.gm[scope] = gm
         got = T("dZ:" + scope, (n, h, wd, c))
         if act in ("prelu", "leaky_relu"):    # the slope below zero, decided by the min(z, 0) plane
@@ -280,8 +304,9 @@ def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None, act="prelu"
         return got
 
     nin2 = cfg.nin_filters2
-    dz_a1 = act_grad("A1", cfg.nin_filters, dnin[:, nin2:])
-    dz_b2 = act_grad("B2", nin2, dnin[:, :nin2])
+    captured["dH:Up-PS"] = dnin
+    dz_a1 = act_grad("A1", cfg.nin_filters)
+    dz_b2 = act_grad("B2", nin2)
     b1 = plane("B1", nin2)
     ref, bar = wgrad_tc("B2/conv_W", b1, dz_b2, 3, nin2, nin2, h, wd)
     chk.add("wgrad_tc B2", grad("B2/conv_W"), ref, bar, signed=True)
@@ -289,7 +314,8 @@ def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None, act="prelu"
     v, bar = twin("B2", dz_b2, wq, b1w, 3)
     db1 = T("dH:B2", (n, h, wd, nin2))
     chk.add("dgrad twin B2", db1, v, bar)
-    dz_b1 = act_grad("B1", nin2, db1)
+    captured["dH:B2"] = db1
+    dz_b1 = act_grad("B1", nin2)
     feats = [plane("CNN%d" % (i + 1), f[i]) for i in range(L)]
     concat = torch.cat(feats, dim=1)
     feat_pitch = sum(pad16(c) for c in f)
@@ -301,16 +327,12 @@ def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None, act="prelu"
     v, bar = twin("A1+B1", torch.cat([dz_a1, dz_b1], dim=1), np.concatenate([wa, wb], axis=3), a1w + b1w, 1)
     dcat = T("dH:A1+B1", (n, h, wd, sum(f)))
     chk.add("dgrad twin A1+B1", dcat, v, bar)
+    captured["dH:A1+B1"] = dcat
 
     # ---- feature-extraction stack
-    offs = np.cumsum([0] + f)
-    dnext = None
     for i in range(L - 1, -1, -1):
         sc = "CNN%d" % (i + 1)
-        g = dcat[:, offs[i]:offs[i + 1]]
-        if dnext is not None:
-            g = g + dnext
-        dz = act_grad(sc, f[i], g)
+        dz = act_grad(sc, f[i])
         if i == 0:
             a = t64(x)
             ssum, sabs = wgrad(a, dz, k), wgrad(a.abs(), dz.abs(), k)
@@ -321,8 +343,8 @@ def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None, act="prelu"
             chk.add("wgrad_tc CNN", grad(sc + "/conv_W"), ref, bar, signed=True)
             (wq,) = quantise([w[sc + "/conv_W"]], 2)
             v, bar = twin(sc, dz, wq, pad16(f[i]), k)
-            dnext = T("dH:" + sc, (n, h, wd, f[i - 1]))
-            chk.add("dgrad twin CNN", dnext, v, bar)
+            captured["dH:" + sc] = T("dH:" + sc, (n, h, wd, f[i - 1]))
+            chk.add("dgrad twin CNN", captured["dH:" + sc], v, bar)
     return chk
 
 

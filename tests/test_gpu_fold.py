@@ -11,13 +11,14 @@ folded filter W' (s*s*9 columns) and writes one set of tap planes, served by get
 import numpy as np
 import pytest
 import torch
+import torch.nn.functional as F
 
 import dcscn_oracle as O
 import tconv_oracle as T
 from conftest import MODEL_FLAGS, load_golden_weights
 from test_fold_cpu import fold32
 from test_gpu_forward import assert_stress, gpu_forward, make_engine
-from test_gpu_forward_paths import U23, U24, conv, nchw, pad16, quantise, tc_units
+from test_gpu_forward_paths import U23, U24, col, conv, nchw, pad16, quantise, tc_units
 from test_gpu_train import CDCSCN, SMALL, SMALL3, SMALL4, assert_kernels_ran, launched_kernels, setup
 
 pytestmark = pytest.mark.gpu
@@ -35,14 +36,65 @@ def tap_planes(eng, parts, n, hr_h, hr_w):
 
 
 def gather9(v):
-    """conv_last_gather: the sum over taps t of plane t at the pixel shifted by (t / 3 - 1, t % 3 - 1), zero outside."""
-    y = np.zeros(v.shape[1:])
+    """conv_last_gather of tap planes [9, n, H, W] (a torch tensor, on its device): the sum over taps t of plane t at
+    the pixel shifted by (t / 3 - 1, t % 3 - 1), zero outside."""
+    y = torch.zeros(v.shape[1:], dtype=v.dtype, device=v.device)
     hr_h, hr_w = v.shape[2:]
+    p = F.pad(v, (1, 1, 1, 1))
     for t in range(9):
         dy, dx = t // 3 - 1, t % 3 - 1
-        p = np.pad(v[t], ((0, 0), (1, 1), (1, 1)))
-        y += p[:, 1 + dy:1 + dy + hr_h, 1 + dx:1 + dx + hr_w]
+        y += p[t, :, 1 + dy:1 + dy + hr_h, 1 + dx:1 + dx + hr_w]
     return y
+
+
+def folded_filter(cfg, w):
+    """(W' quantised as pack_tc_layer packs it in f16x3, b') of the last upsampler folded with R-CNN1 (build_fold)."""
+    scope = "Up-PS2/Up-PS2_CNN" if cfg.scale == 4 else "Up-PS/Up-PS_CNN"
+    wf, bf = fold32(w[scope + "/conv_W"], w[scope + "/conv_B"], w["R-CNN1/conv_W"], cfg.pixel_shuffler_filters or
+                    cfg.nin_filters + cfg.nin_filters2)
+    (wq,) = quantise([wf], 2)
+    return wq, bf
+
+
+def folded_launch_ratios(eng, cfg, folded, x2, y, seg, device=None, chunk=None):
+    """{"taps": max err / bar, "y": max err / bar} of a folded forward whose activations `eng` still holds: the tap
+    planes against conv(input, W') + b' in fp64 from the GPU's own input to the folded launch (`folded` =
+    folded_filter(cfg, w)), at the tensor-core bar of test_gpu_forward_paths.py, and y against their gather + x2.
+    Formed on `device`, `chunk` images at a time (default: all at once)."""
+    wq, bf = folded
+    n, hr_h, hr_w = y.shape[:3]
+    r = 2 if cfg.scale == 4 else cfg.scale          # x4: the 2x second stage
+    hh, ww = hr_h // r, hr_w // r                   # the folded launch's pixel grid
+    h, wd = hr_h // cfg.scale, hr_w // cfg.scale
+    cps = cfg.nin_filters + cfg.nin_filters2
+    if cfg.scale == 4:
+        srcs, cin_pad = [("Up-PS", (n, hh, ww, cps))], pad16(cps)
+    else:
+        srcs = [("B2", (n, h, wd, cfg.nin_filters2)), ("A1", (n, h, wd, cfg.nin_filters))]
+        cin_pad = pad16(cfg.nin_filters2) + pad16(cfg.nin_filters)
+    src = [eng.get_activation(name, shape) for name, shape in srcs]
+    taps = tap_planes(eng, 1, n, hr_h, hr_w)[0]
+    bfc = col(bf, device)
+    out = {"taps": 0.0, "y": 0.0}
+    for i0 in range(0, n, chunk or n):
+        sl = slice(i0, min(n, i0 + (chunk or n)))
+        m = sl.stop - sl.start
+        a = torch.cat([nchw(p[sl], device) for p in src], dim=1)
+        s_abs = conv(a.abs(), np.abs(wq))
+        bar = tc_units(3, cin_pad, seg, 2) * U23 * s_abs + U23 * (s_abs + bfc.abs())
+        v = conv(a, wq) + bfc
+
+        def planes(t):   # [m, s*s*9, hh, ww] -> tap planes [9, m, r*hh, r*ww] (EPI_D2S_TAPS)
+            return t.reshape(m, r, r, 9, hh, ww).permute(3, 0, 4, 1, 5, 2).reshape(9, m, r * hh, r * ww)
+        got = torch.from_numpy(np.ascontiguousarray(taps[:, sl], dtype=np.float64)).to(device)
+        out["taps"] = max(out["taps"], float(((got - planes(v)).abs() / planes(bar)).max()))
+        # the gather + x2 of the reference planes: their bar carried through, plus the gather's ten fp32 adds
+        x2d = torch.from_numpy(np.ascontiguousarray(x2[sl, ..., 0], dtype=np.float64)).to(device)
+        y_ref = gather9(planes(v)) + x2d
+        bar_y = gather9(planes(bar)) + 10 * U24 * (gather9(planes(v).abs()) + x2d.abs())
+        got_y = torch.from_numpy(np.ascontiguousarray(y[sl, ..., 0], dtype=np.float64)).to(device)
+        out["y"] = max(out["y"], float(((got_y - y_ref).abs() / bar_y).max()))
+    return out
 
 
 @pytest.mark.parametrize("scale", [2, 4])
@@ -56,39 +108,14 @@ def test_folded_launch_isolated(scale):
     n, h, wd = 2, 13, 17
     x, x2 = noise(scale, n, h, wd, seed=5)
     eng = make_engine(kw, w)
-    cps = cfg.nin_filters + cfg.nin_filters2
-    scope, r = ("Up-PS2/Up-PS2_CNN", 2) if scale == 4 else ("Up-PS/Up-PS_CNN", scale)   # x4: the 2x second stage
-    wf, bf = fold32(w[scope + "/conv_W"], w[scope + "/conv_B"], w["R-CNN1/conv_W"], cps)
-    (wq,) = quantise([wf], 2)
+    folded = folded_filter(cfg, w)
     bad = []
     for seg in (0, 1):
         eng.set_option("seg_chunks", seg)
         y = gpu_forward(eng, x, x2)
-        if scale == 4:
-            a, cin_pad, m = nchw(eng.get_activation("Up-PS", (n, 2 * h, 2 * wd, cps))), pad16(cps), 2
-        else:
-            a = torch.cat([nchw(eng.get_activation("B2", (n, h, wd, cfg.nin_filters2))),
-                           nchw(eng.get_activation("A1", (n, h, wd, cfg.nin_filters)))], dim=1)
-            cin_pad, m = pad16(cfg.nin_filters2) + pad16(cfg.nin_filters), 1
-        s_abs = conv(a.abs(), np.abs(wq)).numpy()
-        bar = tc_units(3, cin_pad, seg, 2) * U23 * s_abs + U23 * (s_abs + np.abs(bf).reshape(1, -1, 1, 1))
-        v = conv(a, wq).numpy() + bf.astype(np.float64).reshape(1, -1, 1, 1)
-        hh, ww = m * h, m * wd
-
-        def planes(t):   # [n, s*s*9, hh, ww] -> tap planes [9, n, r*hh, r*ww] (EPI_D2S_TAPS)
-            return t.reshape(n, r, r, 9, hh, ww).transpose(3, 0, 4, 1, 5, 2).reshape(9, n, r * hh, r * ww)
-        got = tap_planes(eng, 1, n, r * hh, r * ww)[0]
-        ratio = float((np.abs(got - planes(v)) / planes(bar)).max())
-        if not ratio <= 1.0:
-            bad.append(("taps", seg, ratio))
-        # the gather + x2 of the reference planes: their bar carried through, plus the gather's ten fp32 adds
-        x2d = x2[..., 0].astype(np.float64)
-        y_ref = gather9(planes(v)) + x2d
-        bar_y = gather9(planes(bar)) + 10 * U24 * (gather9(np.abs(planes(v))) + np.abs(x2d))
-        ratio_y = float((np.abs(y[..., 0] - y_ref) / bar_y).max())
-        if not ratio_y <= 1.0:
-            bad.append(("y", seg, ratio_y))
-        print("x%d seg_chunks=%d: taps error / bar %.3f, y error / bar %.3f" % (scale, seg, ratio, ratio_y))
+        ratios = folded_launch_ratios(eng, cfg, folded, x2, y, seg)
+        bad += [(name, seg, ratio) for name, ratio in ratios.items() if not ratio <= 1.0]
+        print("x%d seg_chunks=%d: taps error / bar %.3f, y error / bar %.3f" % (scale, seg, ratios["taps"], ratios["y"]))
     eng.close()
     assert not bad, bad
 

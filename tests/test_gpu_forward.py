@@ -7,11 +7,14 @@ Tolerances (north_star: "1e-3 absolute (fp32)"):
   * uniform-noise / He-init stress inputs push activations to ~2e3, where ANY fp32 implementation sits up to ~2e-3
     from the exact result (the fp32 CPU oracle itself does).  Two settings are held to two bars there:
       - strict promotion (option seg_chunks = 1: every 16-channel K slice is added to the fp32 sum with round-to-nearest):
-        max(1e-3, 1.5 x the fp32 CPU oracle's own error) - on the L12 noise tiles plain 1e-3;
+        max(1e-3, 1.5 x the fp32 CPU oracle's own error) - on the 4 L12 noise tiles of test_l12_stress_noise_tiles
+        plain 1e-3, which does not extend to bench.py's whole 256-tile batch (test_gpu_work_items.py: 2.0e-3 there);
       - the default promotion periods (what bench.py's headline runs): 1.5e-3, and on
         the L12 noise tiles also below 0.75 x the fp32 CPU oracle's error.
     The tensor core truncates its fp32 accumulate on every wgmma; the promotion period trades that error for epilogue
-    work (DESIGN.md section 4).
+    work (DESIGN.md section 4).  Promoting every K slice is not more accurate in absolute terms: it adds one fp32
+    round-to-nearest sum per 16 channels instead of per segment, and on the L12 noise tiles its output lies further from
+    fp64 than the default periods' does.
 """
 import glob
 import os
@@ -149,8 +152,9 @@ DS2 = dict(scale=2, layers=3, filters=12, min_filters=6, filters_decay_gamma=1.5
            pixel_shuffler_filters=1, depthwise_separable=True)
 
 
-def check_depthwise_separable_layers(kw, w, n, h, wd):
-    """Output within 1e-3 of the fp64 oracle, and every layer's activation at fp32 level."""
+def check_depthwise_separable_layers(kw, w, n, h, wd, then=None, tag=None):
+    """Output within 1e-3 of the fp64 oracle, and every layer's activation at fp32 level.  `then(eng, x, x2, y)`, if
+    given, runs on the engine before it is closed; with `tag` every check's error / bar is printed under it."""
     cfg = O.OracleConfig(**kw)
     s = kw["scale"]
     g = torch.Generator().manual_seed(3)
@@ -160,12 +164,19 @@ def check_depthwise_separable_layers(kw, w, n, h, wd):
                                                          return_intermediates=True)
     eng = make_engine(kw, w)
     y = gpu_forward(eng, x, x2)
+    ratios = {"y": float(np.abs(y - y64).max()) / TOL}
     assert np.abs(y - y64).max() <= TOL
     for name, ref in inter.items():
         if name == "R-CNN":
             continue
         a = eng.get_activation(name, ref.shape)
-        assert np.abs(a - ref).max() <= 2e-6 * max(1.0, np.abs(ref).max()) + 1e-4, name
+        bar = 2e-6 * max(1.0, np.abs(ref).max()) + 1e-4
+        ratios[name] = float(np.abs(a - ref).max()) / bar
+        assert np.abs(a - ref).max() <= bar, name
+    if tag is not None:
+        print(tag, "error / bar:", " ".join("%s %.3f" % kv for kv in ratios.items()))
+    if then is not None:
+        then(eng, x, x2, y)
     eng.close()
 
 
@@ -234,9 +245,9 @@ def test_l12_stress_noise_tiles():
     # images, where the fp32 CPU forward itself is ~2.4e-3 from the exact result; the tensor-core path has to stay
     # clearly inside that - two fp32 evaluations cannot agree better than their own rounding noise.
     assert err <= max(TOL, 0.75 * err32), (err, err32)
-    # north_star's bar stated absolutely on this input distribution, 1e-3 against the exact (fp64) forward, is met by
-    # the strict setting: every 16-channel K slice promoted to the fp32 RN sum (seg_chunks = 1; bench.py's "strict" record
-    # carries its throughput).
+    # On these 4 tiles the strict setting (every 16-channel K slice promoted to the fp32 RN sum, seg_chunks = 1; bench.py's
+    # "strict" record carries its throughput) also meets 1e-3 against the exact (fp64) forward.  That does not hold for
+    # the whole 256-tile batch: there the worst tile is 2.0e-3 away (test_gpu_work_items.test_headline_batch).
     eng.set_option("seg_chunks", 1)
     y_strict = gpu_forward(eng, x, x2)
     eng.close()

@@ -120,14 +120,19 @@ DS_CASES = [
 
 
 # ------------------------------------------------------------------------------------ isolated per-layer reference ----
-def nchw(a):
-    return torch.from_numpy(np.ascontiguousarray(a, dtype=np.float64)).permute(0, 3, 1, 2)
+def nchw(a, device=None):
+    return torch.from_numpy(np.ascontiguousarray(a, dtype=np.float64)).to(device).permute(0, 3, 1, 2)
 
 
 def conv(a, w):
-    """tf.nn.conv2d(SAME) of an NCHW fp64 tensor with an HWIO filter."""
-    w = torch.from_numpy(np.ascontiguousarray(w, dtype=np.float64)).permute(3, 2, 0, 1)
+    """tf.nn.conv2d(SAME) of an NCHW fp64 tensor with an HWIO filter, on the tensor's device."""
+    w = torch.from_numpy(np.ascontiguousarray(w, dtype=np.float64)).to(a.device).permute(3, 2, 0, 1)
     return F.conv2d(a, w, padding=w.shape[-1] // 2)
+
+
+def col(v, device=None):
+    """A per-channel vector as an fp64 [1, C, 1, 1] tensor."""
+    return torch.from_numpy(np.asarray(v, dtype=np.float64)).to(device).view(1, -1, 1, 1)
 
 
 def quantise(ws, npl):
@@ -158,15 +163,23 @@ def tc_units(k, cin_pad, seg, npl):
 
 
 def stored_rounding(ref, npl):
-    r = np.abs(ref)
+    """Bar of storing the fp64 tensor `ref`: f16x1 one fp16 ulp of it (np.spacing of its fp16 value: 2^-24 below the
+    normal range, inf at 65504, NaN past it), f16x3 the hi / lo split.  A numpy `ref` gives a numpy bar."""
+    if isinstance(ref, np.ndarray):
+        return stored_rounding(torch.from_numpy(ref.astype(np.float64)), npl).numpy()
+    r = ref.abs()
     if npl == 1:
-        return np.spacing(r.astype(np.float16)).astype(np.float64)
+        r16 = r.to(torch.float16).to(torch.float64)
+        e = torch.frexp(r16)[1]
+        sp = torch.ldexp(torch.ones_like(r16), torch.clamp(e - 1, min=-14) - 10)
+        sp = torch.where(r16 == 0, 2.0 ** -24, sp)
+        sp = torch.where(r16 == 65504, float("inf"), sp)
+        return torch.where(torch.isinf(r16), float("nan"), sp)
     return 2.0 ** -22 * r + 2.0 ** -25
 
 
 def prelu(h, alpha):
-    a = torch.from_numpy(alpha.astype(np.float64)).view(1, -1, 1, 1)
-    return torch.where(h > 0, h, a * h)
+    return torch.where(h > 0, h, col(alpha, h.device) * h)
 
 
 # The kernels' fp32 constants (epilogue.cuh: kLeakySlope, kSeluScale, kSeluScaleAlpha).
@@ -204,109 +217,123 @@ def activation(act, z, bar, alpha=None):
     return v, d * bar + CURVE_U[act] * U24 * (v.abs() + d * bar) + floor
 
 
-def isolated_layers(eng, cfg, w, x, x2, y, npl, seg, fused, act="prelu", masks=None, keep=1.0, pre=None):
+def isolated_layers(eng, cfg, w, x, x2, y, npl, seg, fused, act="prelu", masks=None, keep=1.0, pre=None, device=None,
+                    chunk=None):
     """{layer: max err / bar} of one forward whose activations `eng` still holds (see module docstring), for activator
     `act`.  With `masks` ({layer: dropout_mask}, the train step's forward) a kept element's reference is
     f(z) fp32(1 / keep), one more 2^-24 rounding, and a dropped element must be exactly 0.  `pre`, if given, receives
-    {activated layer: (fp64 pre-activation z, bar of the GPU's fp32 z)}."""
+    {activated layer: (fp64 pre-activation z, bar of the GPU's fp32 z)}, or is called as pre(layer, z, bar, images)
+    once per slice of images.
+
+    The references are formed on `device` (default: the CPU), `chunk` images at a time (default: all at once).  Images
+    are independent, so the slices give the same maxima as one pass.  Each slice fetches the activations it reads and
+    keeps only its images of them, so host memory stays at one whole activation at a time."""
     n, h, wd = x.shape[:3]
     f = O.feature_filters(cfg)
     k = cfg.cnn_size
     cps = cfg.nin_filters + cfg.nin_filters2
     ps_out = cfg.pixel_shuffler_filters or cps
     inv_keep = float(np.float32(1.0) / np.float32(keep))
+    if isinstance(pre, dict) and chunk is not None and chunk < n:
+        raise ValueError("a pre-activation dict holds one slice: pass a callable with chunk")
     out = {}
 
-    def plane(name, c, r=1):
-        return nchw(eng.get_activation(name, (n, r * h, r * wd, c)))
-
     def check(name, got, ref, bar, dropped=None):
-        ratio = np.abs(got - ref) / (bar + 1e-300)     # the floor keeps an exact zero (bar 0) from giving 0 / 0
+        ratio = (got - ref).abs() / (bar + 1e-300)     # the floor keeps an exact zero (bar 0) from giving 0 / 0
         if dropped is not None:
-            ratio = np.where(dropped, np.where(got == 0, 0.0, np.inf), ratio)
-        out[name] = float(ratio.max())
+            ratio = torch.where(dropped, torch.where(got == 0, 0.0, float("inf")), ratio)
+        out[name] = max(out.get(name, 0.0), float(ratio.max()))
 
-    def tc_layer(a, wq, b, kk, cin_pad):
-        """(pre-activation, accumulation + epilogue bar) of one tensor-core layer on the GPU's input `a`."""
-        v = conv(a, wq) + torch.from_numpy(b.astype(np.float64)).view(1, -1, 1, 1)
-        s = conv(a.abs(), np.abs(wq))
-        bar = tc_units(kk, cin_pad, seg, npl) * U23 * s + U23 * (s + torch.from_numpy(np.abs(b).astype(np.float64)).view(1, -1, 1, 1))
-        return v, bar
+    for i0 in range(0, n, chunk or n):
+        sl = slice(i0, min(n, i0 + (chunk or n)))
 
-    def activated(scope, z, bar):
-        """(stored value, bar, dropped elements or None) of an activated layer from its pre-activation."""
-        if pre is not None:
-            pre[scope] = (z, bar)
-        alpha = w["%s/prelu/%s_prelu" % (scope, scope)] if act == "prelu" else None
-        v, bar = activation(act, z, bar, alpha)
-        if masks is None:
-            return v, bar, None
-        m = nchw(masks[scope])
-        v = v * inv_keep
-        return v * m, bar * inv_keep + U24 * v.abs(), (m == 0).numpy()
+        def plane(name, c, r=1):
+            return nchw(eng.get_activation(name, (n, r * h, r * wd, c))[sl], device)
 
-    def store_check(name, got, v, bar, dropped=None):
-        vn = v.numpy()
-        check(name, got.numpy(), vn, bar.numpy() + stored_rounding(vn, npl), dropped)
+        def tc_layer(a, wq, b, kk, cin_pad):
+            """(pre-activation, accumulation + epilogue bar) of one tensor-core layer on the GPU's input `a`."""
+            v = conv(a, wq) + col(b, device)
+            s = conv(a.abs(), np.abs(wq))
+            bar = tc_units(kk, cin_pad, seg, npl) * U23 * s + U23 * (s + col(np.abs(b), device))
+            return v, bar
 
-    # CNN1 (fp32 CUDA cores on x)
-    a = nchw(x)
-    w1 = w["CNN1/conv_W"].astype(np.float64)
-    s = conv(a.abs(), np.abs(w1))
-    b1 = w["CNN1/conv_B"].astype(np.float64)
-    v, bar, dropped = activated("CNN1", conv(a, w1) + torch.from_numpy(b1).view(1, -1, 1, 1),
-                                k * k * U24 * s + U23 * (s + torch.from_numpy(np.abs(b1)).view(1, -1, 1, 1)))
-    feats = [plane("CNN1", f[0])]
-    store_check("CNN1", feats[0], v, bar, dropped)
-    for i in range(1, cfg.layers):
-        sc = "CNN%d" % (i + 1)
-        (wq,) = quantise([w[sc + "/conv_W"]], npl)
-        v, bar, dropped = activated(sc, *tc_layer(feats[-1], wq, w[sc + "/conv_B"], k, pad16(f[i - 1])))
-        feats.append(plane(sc, f[i]))
-        store_check(sc, feats[-1], v, bar, dropped)
-    # A1 and B1: one packed layer over the concat, one scale
-    hc = torch.cat(feats, dim=1)
-    wa, wb = quantise([w["A1/conv_W"], w["B1/conv_W"]], npl)
-    cin_pad = sum(pad16(c) for c in f)
-    a1 = plane("A1", cfg.nin_filters)
-    b1g = plane("B1", cfg.nin_filters2)
-    v, bar, dropped = activated("A1", *tc_layer(hc, wa, w["A1/conv_B"], 1, cin_pad))
-    store_check("A1", a1, v, bar, dropped)
-    v, bar, dropped = activated("B1", *tc_layer(hc, wb, w["B1/conv_B"], 1, cin_pad))
-    store_check("B1", b1g, v, bar, dropped)
-    (wq,) = quantise([w["B2/conv_W"]], npl)
-    v, bar, dropped = activated("B2", *tc_layer(b1g, wq, w["B2/conv_B"], 3, pad16(cfg.nin_filters2)))
-    b2 = plane("B2", cfg.nin_filters2)
-    store_check("B2", b2, v, bar, dropped)
-    # pixel shuffler(s): the last one is fp32 (EPI_D2S_F32) or feeds the fused R-CNN1
-    src, cin_pad = torch.cat([b2, a1], dim=1), pad16(cfg.nin_filters2) + pad16(cfg.nin_filters)
-    stages = [("Up-PS", "Up-PS/Up-PS_CNN", 2, cps), ("Up-PS2", "Up-PS2/Up-PS2_CNN", 2, ps_out)] if cfg.scale == 4 else \
-        [("Up-PS", "Up-PS/Up-PS_CNN", cfg.scale, ps_out)]
-    mult = 1
-    for si, (name, scope, r, c) in enumerate(stages):
-        (wq,) = quantise([w[scope + "/conv_W"]], npl)
-        v, bar = tc_layer(src, wq, w[scope + "/conv_B"], k, cin_pad)
-        v, bar = O.depth_to_space(v, r), O.depth_to_space(bar, r)
-        mult *= r
-        if si + 1 < len(stages):            # x4 Up-PS: fp16 planes
-            src, cin_pad = plane(name, c, mult), pad16(c)
-            store_check(name, src, v, bar)
-        elif not fused:
-            up = plane(name, c, mult)
-            check(name, up.numpy(), v.numpy(), bar.numpy())
-    # R-CNN1 + x2 (fp32)
-    wr = w["R-CNN1/conv_W"].astype(np.float64)
-    kr = wr.shape[0]
-    x2t = nchw(x2)
-    gpu_y = nchw(y).numpy()
-    if fused:
-        yr = conv(v, wr) + x2t
-        bar_y = conv(bar, np.abs(wr)) + kr * kr * ps_out * U24 * conv(v.abs(), np.abs(wr)) + U24 * yr.abs()
-        check("R-CNN1 (fused)", gpu_y, yr.numpy(), bar_y.numpy())
-    else:
-        yr = conv(up, wr) + x2t
-        bar_y = kr * kr * ps_out * U24 * conv(up.abs(), np.abs(wr)) + U24 * yr.abs()
-        check("R-CNN1", gpu_y, yr.numpy(), bar_y.numpy())
+        def activated(scope, z, bar):
+            """(stored value, bar, dropped elements or None) of an activated layer from its pre-activation."""
+            if callable(pre):
+                pre(scope, z, bar, sl)
+            elif pre is not None:
+                pre[scope] = (z, bar)
+            alpha = w["%s/prelu/%s_prelu" % (scope, scope)] if act == "prelu" else None
+            v, bar = activation(act, z, bar, alpha)
+            if masks is None:
+                return v, bar, None
+            m = nchw(masks[scope][sl], device)
+            v = v * inv_keep
+            return v * m, bar * inv_keep + U24 * v.abs(), m == 0
+
+        def store_check(name, got, v, bar, dropped=None):
+            check(name, got, v, bar + stored_rounding(v, npl), dropped)
+
+        # CNN1 (fp32 CUDA cores on x)
+        a = nchw(x[sl], device)
+        w1 = w["CNN1/conv_W"].astype(np.float64)
+        s = conv(a.abs(), np.abs(w1))
+        b1 = w["CNN1/conv_B"].astype(np.float64)
+        v, bar, dropped = activated("CNN1", conv(a, w1) + col(b1, device),
+                                    k * k * U24 * s + U23 * (s + col(np.abs(b1), device)))
+        feats = [plane("CNN1", f[0])]
+        store_check("CNN1", feats[0], v, bar, dropped)
+        for i in range(1, cfg.layers):
+            sc = "CNN%d" % (i + 1)
+            (wq,) = quantise([w[sc + "/conv_W"]], npl)
+            v, bar, dropped = activated(sc, *tc_layer(feats[-1], wq, w[sc + "/conv_B"], k, pad16(f[i - 1])))
+            feats.append(plane(sc, f[i]))
+            store_check(sc, feats[-1], v, bar, dropped)
+        # A1 and B1: one packed layer over the concat, one scale
+        hc = torch.cat(feats, dim=1)
+        del feats
+        wa, wb = quantise([w["A1/conv_W"], w["B1/conv_W"]], npl)
+        cin_pad = sum(pad16(c) for c in f)
+        a1 = plane("A1", cfg.nin_filters)
+        b1g = plane("B1", cfg.nin_filters2)
+        v, bar, dropped = activated("A1", *tc_layer(hc, wa, w["A1/conv_B"], 1, cin_pad))
+        store_check("A1", a1, v, bar, dropped)
+        v, bar, dropped = activated("B1", *tc_layer(hc, wb, w["B1/conv_B"], 1, cin_pad))
+        store_check("B1", b1g, v, bar, dropped)
+        del hc
+        (wq,) = quantise([w["B2/conv_W"]], npl)
+        v, bar, dropped = activated("B2", *tc_layer(b1g, wq, w["B2/conv_B"], 3, pad16(cfg.nin_filters2)))
+        b2 = plane("B2", cfg.nin_filters2)
+        store_check("B2", b2, v, bar, dropped)
+        # pixel shuffler(s): the last one is fp32 (EPI_D2S_F32) or feeds the fused R-CNN1
+        src, cin_pad = torch.cat([b2, a1], dim=1), pad16(cfg.nin_filters2) + pad16(cfg.nin_filters)
+        stages = [("Up-PS", "Up-PS/Up-PS_CNN", 2, cps), ("Up-PS2", "Up-PS2/Up-PS2_CNN", 2, ps_out)] if cfg.scale == 4 \
+            else [("Up-PS", "Up-PS/Up-PS_CNN", cfg.scale, ps_out)]
+        mult = 1
+        for si, (name, scope, r, c) in enumerate(stages):
+            (wq,) = quantise([w[scope + "/conv_W"]], npl)
+            v, bar = tc_layer(src, wq, w[scope + "/conv_B"], k, cin_pad)
+            v, bar = O.depth_to_space(v, r), O.depth_to_space(bar, r)
+            mult *= r
+            if si + 1 < len(stages):            # x4 Up-PS: fp16 planes
+                src, cin_pad = plane(name, c, mult), pad16(c)
+                store_check(name, src, v, bar)
+            elif not fused:
+                up = plane(name, c, mult)
+                check(name, up, v, bar)
+        # R-CNN1 + x2 (fp32)
+        wr = w["R-CNN1/conv_W"].astype(np.float64)
+        kr = wr.shape[0]
+        x2t = nchw(x2[sl], device)
+        gpu_y = nchw(y[sl], device)
+        if fused:
+            yr = conv(v, wr) + x2t
+            bar_y = conv(bar, np.abs(wr)) + kr * kr * ps_out * U24 * conv(v.abs(), np.abs(wr)) + U24 * yr.abs()
+            check("R-CNN1 (fused)", gpu_y, yr, bar_y)
+        else:
+            yr = conv(up, wr) + x2t
+            bar_y = kr * kr * ps_out * U24 * conv(up.abs(), np.abs(wr)) + U24 * yr.abs()
+            check("R-CNN1", gpu_y, yr, bar_y)
     return out
 
 

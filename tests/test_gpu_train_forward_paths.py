@@ -26,7 +26,7 @@ import dcscn_oracle as O
 from conftest import MODEL_FLAGS
 from test_gpu_backward_paths import L12, Checker, check_step, dev, real_engine, real_patches, release_reference_memory  # noqa: F401
 from test_gpu_forward import SMALL, gpu_forward, make_engine
-from test_gpu_forward_paths import FIRST3, TC_CASES, isolated_layers, nchw
+from test_gpu_forward_paths import FIRST3, TC_CASES, isolated_layers, nchw, stored_rounding
 from test_gpu_train import FAST, GRADIENT_CASES, SMALL as TSMALL, assert_kernels_ran, launched_kernels, setup
 
 pytestmark = pytest.mark.gpu
@@ -41,50 +41,67 @@ def masks_of(eng, cfg, seed, n, h, w):
             for scope, k, cin, cout, bias, _ in O.layer_table(cfg) if A.activated(scope)}
 
 
+def zneg_ratio(zn, z, bz):
+    """max err / bar of one layer's min(z, 0) plane `zn` against the isolated pre-activation z (bar bz of the GPU's z),
+    all fp64 NCHW tensors on one device (module docstring)."""
+    half_ulp = 0.5 * stored_rounding(torch.clamp(z.abs() + bz, max=65504.0), 1)
+    tiny = (z < bz) & (z > -(U24 + bz))          # the fp32 z may lie in (-2^-24, 0): stored as -2^-24
+    ratio = (zn - z).abs() / (half_ulp + bz + torch.where(tiny, U24, 0.0))
+    ratio = torch.where(z > bz, torch.where(zn == 0, 0.0, float("inf")), ratio)
+    ratio = torch.where((zn > 0) | ((z < -bz) & (zn >= 0)), float("inf"), ratio)
+    return float(ratio.max())
+
+
 def zneg_ratios(eng, pre, n, h, wd):
-    """{zneg <layer>: max err / bar} of the min(z, 0) planes against the isolated pre-activations (module docstring)."""
-    out = {}
-    for scope, (z, bz) in pre.items():
-        zn = nchw(eng.get_train_tensor("zneg:" + scope, (n, h, wd, z.shape[1]))).numpy()
-        z, bz = z.numpy(), bz.numpy()
-        half_ulp = 0.5 * np.spacing(np.minimum(np.abs(z) + bz, 65504.0).astype(np.float16)).astype(np.float64)
-        tiny = (z < bz) & (z > -(U24 + bz))          # the fp32 z may lie in (-2^-24, 0): stored as -2^-24
-        ratio = np.abs(zn - z) / (half_ulp + bz + np.where(tiny, U24, 0.0))
-        ratio = np.where(z > bz, np.where(zn == 0, 0.0, np.inf), ratio)
-        ratio = np.where((zn > 0) | ((z < -bz) & (zn >= 0)), np.inf, ratio)
-        out["zneg " + scope] = float(ratio.max())
-    return out
+    """{zneg <layer>: max err / bar} of the min(z, 0) planes against the isolated pre-activations."""
+    return {"zneg " + scope: zneg_ratio(nchw(eng.get_train_tensor("zneg:" + scope, (n, h, wd, z.shape[1])), z.device), z, bz)
+            for scope, (z, bz) in pre.items()}
+
+
+class SlopeSums:
+    """Per-channel sums over images of the PReLU slope gradient's reference: sum g z over the isolated z < 0 and its
+    bar terms, added one slice of images at a time (add), then compared with the GPU's gradients (ratios)."""
+
+    def __init__(self):
+        self.sums = {}
+
+    def add(self, scope, gm, z, bz):
+        gz = torch.where(z < 0, gm * z, torch.zeros_like(gm))
+        terms = (gz.sum(dim=(0, 2, 3)), gz.abs().sum(dim=(0, 2, 3)), (gm.abs() * (bz + U24) * (z < bz)).sum(dim=(0, 2, 3)))
+        old = self.sums.get(scope)
+        self.sums[scope] = terms if old is None else tuple(a + b for a, b in zip(old, terms))
+
+    def ratios(self, eng, n, h, wd, scale):
+        """{slope <layer>: (max err / bar, max err / (sum |g z| / G))}.  The GPU sums g zneg in fp32 ((npx + 4) 2^-24
+        sum |g z|); zneg is the fp32 z (within B_z, and the sign is open where |z| <= B_z) stored in fp16 (2^-11 |z|, or
+        -2^-24 for z in (-2^-24, 0))."""
+        G = 2.0 ** round(math.log2(n * scale * h * scale * wd / 2.0))
+        npx = n * h * wd
+        out = {}
+        for scope, (sgzs, sgz, extra) in self.sums.items():
+            bar = (npx + 4) * U24 * sgz + 2.0 ** -11 * sgz + extra
+            ref = sgzs / G
+            bar = bar / G + U24 * ref.abs() + 1e-45
+            got = torch.from_numpy(eng.get_grad("%s/prelu/%s_prelu" % (scope, scope))).to(sgz.device, torch.float64)
+            err = (got - ref).abs()
+            out["slope " + scope] = (float((err / bar).max()), float((err / (sgz / G + 1e-45)).max()))
+        return out
 
 
 def slope_ratios(eng, pre, chk, n, h, wd, scale):
-    """{slope <layer>: (max err / bar, max err / (sum |g z| / G))} of the PReLU slope gradients against sum g z over the
-    isolated z < 0.  The GPU sums g zneg in fp32 ((npx + 4) 2^-24 sum |g z|); zneg is the fp32 z (within B_z, and the
-    sign is open where |z| <= B_z) stored in fp16 (2^-11 |z|, or -2^-24 for z in (-2^-24, 0))."""
-    G = 2.0 ** round(math.log2(n * scale * h * scale * wd / 2.0))
-    npx = n * h * wd
-    out = {}
+    """SlopeSums.ratios of the whole batch, with the output gradients check_step formed."""
+    sums = SlopeSums()
     for scope, (z, bz) in pre.items():
-        gm = chk.gm[scope]
-        z, bz = z.to(dev()), bz.to(dev())
-        gz = torch.where(z < 0, gm * z, torch.zeros_like(gm))
-        sgz = gz.abs().sum(dim=(0, 2, 3))
-        bar = (npx + 4) * U24 * sgz + 2.0 ** -11 * sgz + (gm.abs() * (bz + U24) * (z < bz)).sum(dim=(0, 2, 3))
-        ref = gz.sum(dim=(0, 2, 3)) / G
-        bar = bar / G + U24 * ref.abs() + 1e-45
-        got = torch.from_numpy(eng.get_grad("%s/prelu/%s_prelu" % (scope, scope))).to(dev(), torch.float64)
-        err = (got - ref).abs()
-        out["slope " + scope] = (float((err / bar).max()), float((err / (sgz / G + 1e-45)).max()))
-    return out
+        sums.add(scope, chk.gm[scope], z.to(dev()), bz.to(dev()))
+    return sums.ratios(eng, n, h, wd, scale)
 
 
-def train_case(kw, wts, act, keep, x, x2, y, kernels, tag):
-    """One captured train step (apply_update = False): the kernels it reached, then every forward layer, y_, the zneg
-    planes, the PReLU slope gradients and every backward kernel (check_step) against their isolated references.  All
-    violations are reported at once."""
+def captured_step(kw, wts, act, keep, x, x2, y, kernels):
+    """(engine, its dropout masks or None) after one captured train step (apply_update = False) that reached
+    `kernels`."""
     from helper import engine as E
     cfg = O.OracleConfig(**kw)
     n, h, wd = x.shape[:3]
-    s = cfg.scale
     eng = E.Engine(E.make_config(dropout_keep=keep, activator=act, **kw))
     eng.set_params({k: v.astype(np.float32) for k, v in wts.items()})
     eng.set_option("grad_capture", 1)
@@ -93,7 +110,17 @@ def train_case(kw, wts, act, keep, x, x2, y, kernels, tag):
     if any(k.startswith("conv_first3x3_kernel") for k in kernels):     # the min(z, 0) store is a template argument
         first = ["conv_first3x3_kernel<%s>" % ("true" if act in ("prelu", "leaky_relu") else "false")]
     assert_kernels_ran(names, kernels + first + ["loss_kernel", "act_grad8_kernel"])
-    masks = masks_of(eng, cfg, SEED, n, h, wd) if keep < 1.0 else None
+    return eng, (masks_of(eng, cfg, SEED, n, h, wd) if keep < 1.0 else None)
+
+
+def train_case(kw, wts, act, keep, x, x2, y, kernels, tag):
+    """One captured train step (apply_update = False): the kernels it reached, then every forward layer, y_, the zneg
+    planes, the PReLU slope gradients and every backward kernel (check_step) against their isolated references.  All
+    violations are reported at once."""
+    cfg = O.OracleConfig(**kw)
+    n, h, wd = x.shape[:3]
+    s = cfg.scale
+    eng, masks = captured_step(kw, wts, act, keep, x, x2, y, kernels)
     yp = eng.get_train_tensor("y_", (n, s * h, s * wd, 1))
     pre = {}
     ratios = isolated_layers(eng, cfg, wts, x, x2, yp, 2, 0, False, act=act, masks=masks, keep=keep, pre=pre)
