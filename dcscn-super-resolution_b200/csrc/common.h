@@ -93,6 +93,7 @@ struct ConvTCParams {
   int n_pad;             // columns per tile, multiple of 16, <= kMaxTileN (112)
   int seg_chunks;        // pipeline stages per accumulation segment (fp32 promotion period)
   const __half* wpack;   // packed weights [n_tile][tap][chunk][plane][n_pad x 64] (pre-swizzled)
+  int bias_smem;         // conv_tc_kernel keeps a copy of epi.bias / epi.alpha in shared memory (add_tc_launch)
   EpiParams epi;
 };
 

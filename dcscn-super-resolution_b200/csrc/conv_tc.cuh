@@ -26,10 +26,13 @@
 //     tiles (one per (tap, chunk), read from the packed image [n_tile][tap][chunk]).  The consumers commit one wgmma
 //     group per weight tile and release a slot as soon as `wgmma.wait_group 1` shows the group that last read it
 //     has completed, so both rings work purely as prefetch depth.  A weight tile arrives as one bulk copy.
-//   * Warp roles: warpgroup 0 = producer (warp 0 issues TMA), warpgroups 1 and 2 = consumers, one per 64-pixel half
-//     of the tile: they issue the wgmma of their rows, promote, and run the epilogue (bias/PReLU/split -> global) after
-//     an exchange through shared memory that gives every thread one pixel and a run of 16-column chunks.  Persistent
-//     CTAs (one per SM) stride over (pixel-tile, column-tile) work items.
+//   * Warp roles: warpgroups 1 and 2 = consumers, one per 64-pixel half of the tile: they issue the wgmma of their
+//     rows and promote.  At the end of an item they store the fp32 sums into a hand-off tile in shared memory and go
+//     on to the next item.  Warpgroup 0: thread 0 issues the TMA and bulk copies; warps 1-3 run the epilogue (bias /
+//     activation / split -> global, or the fused R-CNN1 dot products) from the hand-off tile, one pixel and a run of
+//     16-column chunks per work unit, while the consumers' wgmma of the next item run.  Two mbarriers pass the tile
+//     back and forth (stage_full, stage_empty).  Persistent CTAs (one per SM) stride over (pixel-tile, column-tile)
+//     work items.
 #pragma once
 #include "common.h"
 #include "epilogue.cuh"
@@ -39,16 +42,21 @@ namespace dcscn {
 
 constexpr int kConsumerWGs = 2;                    // one per 64-pixel half of the 128-pixel tile
 constexpr int kTcThreads = (1 + kConsumerWGs) * 128;
-constexpr int kRegsIssue = 40, kRegsEpilogue = 232;  // setmaxnreg budgets (128*40 + 256*232 <= 64K)
+// setmaxnreg budgets: the kernel starts at 168 registers a thread (65536 / 384, in steps of 8), a pool of 384 * 168;
+// 128 * 104 + 256 * 200 fills it exactly.  200 hold the three accumulator sets of a 112-column tile (168) without a
+// spill, now that the epilogue runs elsewhere; below 104 the epilogue warps spill inside their loop.
+constexpr int kRegsProducer = 104, kRegsConsumer = 200;
+constexpr int kRegsIssue = 40, kRegsEpilogue = 232;  // wgrad_tc_kernel's budgets (128*40 + 256*232 = 384 * 168)
+constexpr int kEpiWarps = 3;                       // warps 1-3 of the producer warpgroup run the tile epilogues
+constexpr int kEpiThreads = kEpiWarps * 32;
 constexpr int kMaxASlots = 4;                      // activation ring slots
 constexpr int kMaxWSlots = 12;                     // weight ring slots
-constexpr int kTcBarrierBytes = 2 * (kMaxASlots + kMaxWSlots) * 8;
+constexpr int kTcBarrierBytes = (2 * (kMaxASlots + kMaxWSlots) + 2) * 8;   // rings + stage_full / stage_empty
 constexpr int kMaxTileN = 112;                     // column tile cap: corr + dom + promoted sum = 3 N / 2 registers;
                                                    // at N = 128 (192 of them) ptxas spills inside the K loop
 constexpr int kRdotSmemBytes = 9 * 128 * 4;         // fused R-CNN1 filter taps (d2s_cout <= 128) staged in shared memory
-constexpr int kColSplit = 2;                       // epilogue threads per pixel, each owning a contiguous run of chunks
-constexpr int kXchgStride = 36;                    // floats per pixel row of the epilogue exchange buffer (2 chunks + pad)
-constexpr int kXchgBytes = kConsumerWGs * 64 * kXchgStride * 4;
+constexpr int kColSplit = 2;                       // epilogue work units per pixel, each a contiguous run of chunks
+
 constexpr int kTcKC = 64;                          // input channels per K chunk: an fp16 operand row is 128 bytes,
                                                    // one row of the SWIZZLE_128B layout
 
@@ -73,6 +81,21 @@ __host__ __device__ inline uint32_t tc_a_plane_bytes(int TW, int TH, int ksz) {
 __host__ __device__ inline uint32_t tc_w_tile_bytes(int nplanes, int n_pad) {
   return (uint32_t)nplanes * (uint32_t)n_pad * (uint32_t)kTcKC * 2u;
 }
+
+// The fp32 hand-off tile between the consumers and the epilogue warps: 128 pixel rows of an N-column tile.  A row holds
+// the first `per` 16-column chunks (the first epilogue unit of the pixel), 4 floats of gap, then the rest; the stride
+// N + 8 is 8 or 24 floats past a multiple of 32.  So the consumers' 8-byte stores (4 rows x 8 columns per half warp)
+// and the epilogue's 16-byte loads (4 pixels x both units per quarter warp) each touch every bank once.
+__host__ __device__ constexpr int tc_stage_stride(int n_pad) { return n_pad + 8; }
+__host__ __device__ constexpr uint32_t tc_stage_bytes(int n_pad) { return 128u * (uint32_t)tc_stage_stride(n_pad) * 4u; }
+
+#ifdef DCSCN_TC_PHASES
+// Diagnostic build only (-DDCSCN_TC_PHASES, scripts/tc_phases.py): clock64() cycles summed over the consumer warpgroups
+// of every CTA of a launch.  [0] K loop (item start to its last wgmma), [1] the consumers' epilogue, [2] items x
+// consumer warpgroups, [3] the epilogue warps' busy cycles (summed over the kEpiWarps warps).  The host reads and
+// clears them after each launch (tc_phase_report).
+__device__ unsigned long long g_tc_phase[4];
+#endif
 
 // One wgmma batch: the products of KS consecutive 16-channel K slices of a weight tile, committed as one group.
 // corr += a_lo*w_hi + a_hi*w_lo, dom += a_hi*w_hi; acc_on == 0 starts both from zero.
@@ -99,7 +122,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
                const ConvTCParams p, const int a_slots, const int w_slots) {
   static_assert(N % 16 == 0 && N >= 16 && N <= kMaxTileN, "column tile width");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [a_slots x (A_hi, A_lo)] [w_slots x (W_hi, W_lo)] then barriers, R-CNN1 taps, epilogue exchange
+  // carve: [a_slots x (A_hi, A_lo)] [w_slots x (W_hi, W_lo)] then barriers, the hand-off tile, the R-CNN1 taps
+  // (EPI_D2S_RDOT only) and, when p.bias_smem, the bias and slopes of all n_tiles * N columns
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const ConvGeom& g = p.g;
   const int ksz = p.ksz;
@@ -114,8 +138,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
   uint64_t* a_empty = a_full + kMaxASlots;
   uint64_t* w_full = a_empty + kMaxASlots;
   uint64_t* w_empty = w_full + kMaxWSlots;
-  float* s_rdot = reinterpret_cast<float*>(w_empty + kMaxWSlots);   // 16-byte aligned (barriers start 1024-aligned)
-  float* s_xchg = s_rdot + kRdotSmemBytes / 4;
+  uint64_t* stage_full = w_empty + kMaxWSlots;    // the consumers have stored an item's sums in the hand-off tile
+  uint64_t* stage_empty = stage_full + 1;          // the epilogue warps have read them
+  float* s_stage = reinterpret_cast<float*>(stage_empty + 1);   // 16-byte aligned (barriers start 1024-aligned)
+  float* s_rdot = s_stage + tc_stage_bytes(N) / 4;
+  constexpr int kStride = tc_stage_stride(N);
+  constexpr int nch = N >> 4;
+  constexpr int per = (nch + kColSplit - 1) / kColSplit;   // chunks of a pixel's first epilogue unit
 
   const int wg = threadIdx.x >> 7;
   const int lane = threadIdx.x & 31;
@@ -129,11 +158,25 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
       ptx::mbar_init(&w_full[s], 1);
       ptx::mbar_init(&w_empty[s], kConsumerWGs);
     }
+    ptx::mbar_init(stage_full, kConsumerWGs * 4);   // one arrival per consumer warp
+    ptx::mbar_init(stage_empty, kEpiWarps);         // one arrival per epilogue warp
     ptx::fence_barrier_init();
     ptx::fence_proxy_async();
   }
+  float* s_bias = s_rdot + (p.epi.mode == EPI_D2S_RDOT ? kRdotSmemBytes / 4 : 0);
+  float* s_alpha = s_bias + p.n_tiles * N;
   if (p.epi.mode == EPI_D2S_RDOT)
     for (int i = threadIdx.x; i < p.epi.rdot_taps * p.epi.d2s_cout; i += blockDim.x) s_rdot[i] = p.epi.rdot_w[i];
+  // epilogue_store16 reads them from here: an epilogue warp has few loads in flight, and an L1 miss on them is what it
+  // waits for longest
+  const bool bias_smem = p.bias_smem != 0;   // the host reserves them only in the EPI_PLANES / D2S plane modes
+  const float* bias_src = bias_smem ? s_bias : p.epi.bias;
+  const float* alpha_src = bias_smem ? s_alpha : p.epi.alpha;
+  if (bias_smem)
+    for (int i = threadIdx.x; i < p.n_tiles * N; i += blockDim.x) {
+      s_bias[i] = p.epi.bias[i];
+      s_alpha[i] = p.epi.alpha[i];
+    }
   __syncthreads();
 
   const int tiles_per_img = g.tiles_x * g.tiles_y;
@@ -142,7 +185,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
   const int chunks = p.chunks;
 
   if (wg == 0) {
-    ptx::setmaxnreg_dec<kRegsIssue>();
+    ptx::setmaxnreg_dec<kRegsProducer>();
     // ============================== TMA producer ==============================
     if (threadIdx.x == 0) {
       ptx::prefetch_tensormap(&tm_hi);
@@ -176,42 +219,105 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
           }
         }
       }
+    } else if (threadIdx.x >= 32) {
+      // ============================== epilogue warps ==========================
+      // Each item's sums arrive in the hand-off tile.  A work unit is one pixel and a contiguous run of 16-column chunks
+      // (the first `per` chunks, or the rest); unit u = 2 pixel + run, so a warp reads 16 pixels x both runs.  A
+      // thread's units all have the same run (kEpiThreads is even), so its bias and slopes stay the same.
+      const int e = threadIdx.x - 32;
+      const int n_total = p.n_tiles * N;
+      uint32_t st_ph = 0;
+#ifdef DCSCN_TC_PHASES
+      long long ph_w = 0;
+#endif
+      for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
+        const int n_tile = item % p.n_tiles;
+        const int tile = item / p.n_tiles;
+        const int img = tile / tiles_per_img;
+        const int t2 = tile - img * tiles_per_img;
+        const int ty = t2 / g.tiles_x, tx = t2 - ty * g.tiles_x;
+        ptx::mbar_wait(stage_full, st_ph);
+#ifdef DCSCN_TC_PHASES
+        const long long ph_t0 = clock64();
+#endif
+        // In the depth_to_space modes nothing is stored past n_valid: when the second runs of chunks lie wholly past it
+        // (the folded Up-PS: 36 of 96 columns), the units are the pixels' first runs alone.
+        const int runs = p.epi.mode != EPI_PLANES && n_tile * N + per * 16 >= p.epi.n_valid ? 1 : kColSplit;
+#pragma unroll 1
+        for (int u = e; u < 128 * runs; u += kEpiThreads) {
+          const int row = runs == kColSplit ? u >> 1 : u, grp = runs == kColSplit ? u & 1 : 0;
+          const int py = row / g.TW, px = row - py * g.TW;
+          const int y = ty * g.TH + py, x = tx * g.TW + px;
+          const bool valid = (y < g.H) && (x < g.W);
+          const int first_chunk = grp * per;
+          const int my_chunks = (nch - first_chunk) < per ? ((nch - first_chunk) > 0 ? nch - first_chunk : 0) : per;
+          const float4* src = reinterpret_cast<const float4*>(s_stage + row * kStride + grp * (per * 16 + 4));
+          float v9[9];
+#pragma unroll
+          for (int i = 0; i < 9; ++i) v9[i] = 0.f;
+#pragma unroll
+          for (int k = 0; k < per; ++k) {
+            if (k < my_chunks) {
+              float v[16];
+#pragma unroll
+              for (int q = 0; q < 4; ++q) {
+                const float4 f = src[4 * k + q];
+                v[4 * q] = f.x; v[4 * q + 1] = f.y; v[4 * q + 2] = f.z; v[4 * q + 3] = f.w;
+              }
+              const int cg = n_tile * N + (first_chunk + k) * 16;
+              if (p.epi.mode == EPI_D2S_RDOT) {
+                // the host guarantees that a unit's columns are whole sub-pixels (rdot_parts == 1) or an equal share of
+                // one sub-pixel (rdot_parts > 1: each share writes its own partial plane set)
+                if (cg < p.epi.n_valid) {
+                  const int ij = cg / p.epi.d2s_cout, cc = cg - ij * p.epi.d2s_cout;
+                  rdot_accumulate16(p.epi, s_rdot, cg, cc, v, v9);
+                  const bool last = p.epi.rdot_parts > 1 ? k + 1 == my_chunks : cc + 16 == p.epi.d2s_cout;
+                  if (last && valid) rdot_flush(p.epi, g, img, y, x, ij, p.epi.rdot_parts > 1 ? cc / (per * 16) : 0, v9);
+                }
+              } else if (valid) {
+                if (p.epi.mode == EPI_D2S_TAPS) taps_store16(p.epi, g, img, y, x, cg, v);
+                else epilogue_store16<true>(p.epi, g, n_total, img, y, x, cg, v, bias_src, alpha_src);
+              }
+            }
+          }
+        }
+        __syncwarp();
+        ptx::mbar_arrive_if(stage_empty, lane == 0);
+        st_ph ^= 1;
+#ifdef DCSCN_TC_PHASES
+        ph_w += clock64() - ph_t0;
+#endif
+      }
+#ifdef DCSCN_TC_PHASES
+      if (lane == 0) atomicAdd(&g_tc_phase[3], (unsigned long long)ph_w);
+#endif
     }
   } else {
-    ptx::setmaxnreg_inc<kRegsEpilogue>();
+    ptx::setmaxnreg_inc<kRegsConsumer>();
     // ============================== consumers ==================================
     const int cw = wg - 1;                   // which 64-pixel half of the tile
     const int t = threadIdx.x & 127;
     const int wq = t >> 5;                   // warp inside the warpgroup: accumulator rows 16 wq .. 16 wq + 15
-    constexpr int nch = N >> 4;
-    constexpr int per = (nch + kColSplit - 1) / kColSplit;
-    const int n_total = p.n_tiles * N;
     const bool strict = p.seg_chunks == 1;
     const uint32_t a_ring_u32 = ptx::smem_u32(a_ring);
     const uint32_t w_ring_u32 = ptx::smem_u32(w_ring);
     const uint32_t a_off = (uint32_t)(cw * 64 * TcSmem::kRowBytes);
     const uint32_t dy_step = (uint32_t)(g.TW * TcSmem::kRowBytes);   // one image row of the box: whole 8-row atoms
-    // epilogue ownership after the exchange: pixel `row`, chunks [grp * per, grp * per + my_chunks)
-    const int row = cw * 64 + (t >> 1);
-    const int grp = t & 1;
-    const int py = row / g.TW, px = row - py * g.TW;
-    const int first_chunk = grp * per;
-    const int my_chunks = (nch - first_chunk) < per ? ((nch - first_chunk) > 0 ? nch - first_chunk : 0) : per;
-    float* xchg = s_xchg + cw * 64 * kXchgStride;
+    // the wgmma layout gives a thread rows 16 wq + lane / 4 (+ 8) of its half and column pairs 8 j + 2 (lane % 4)
+    float* stage_row = s_stage + (cw * 64 + wq * 16 + (lane >> 2)) * kStride + 2 * (lane & 3);
+    uint32_t st_ph = 0;
     // a slot is released once the wgmma group that last read it has completed (one arrival per warpgroup, by thread 0)
     auto release_a = [&](int s) { ptx::mbar_arrive_if(&a_empty[s], t == 0); };
     auto release_w = [&](int s) { ptx::mbar_arrive_if(&w_empty[s], t == 0); };
     int as = 0, ws = 0;
     uint32_t a_ph = 0, w_ph = 0;
+#ifdef DCSCN_TC_PHASES
+    long long ph_k = 0, ph_e = 0, ph_n = 0;
+#endif
     for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-      const int n_tile = item % p.n_tiles;
-      const int tile = item / p.n_tiles;
-      const int img = tile / tiles_per_img;
-      const int t2 = tile - img * tiles_per_img;
-      const int ty = t2 / g.tiles_x, tx = t2 - ty * g.tiles_x;
-      const int y = ty * g.TH + py, x = tx * g.TW + px;
-      const bool valid = (y < g.H) && (x < g.W);
-
+#ifdef DCSCN_TC_PHASES
+      const long long ph_t0 = clock64();
+#endif
       float sum[N / 2], corr[N / 2], dom[N / 2];
 #pragma unroll
       for (int i = 0; i < N / 2; ++i) sum[i] = 0.f;
@@ -290,58 +396,39 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
         }
       }
       // the last weight tile ended a segment, so every group has completed; saying so here keeps ptxas from placing
-      // its own wait inside the loop, ahead of the exchange that reuses the accumulator registers
+      // its own wait inside the loop, ahead of the stores that read the accumulator registers
       ptx::wgmma_wait<0>();
+#ifdef DCSCN_TC_PHASES
+      const long long ph_t1 = clock64();
+#endif
 
-      // Exchange: the wgmma layout gives a thread rows 16 wq + lane / 4 (+ 8) and column pairs 8 j + 2 (lane % 4); the
-      // epilogue wants one pixel and 16 consecutive columns per thread.  Round k moves chunks k and per + k.
-      float v9[9];
+      // Hand-off: once the epilogue warps have read the previous item's tile, store the sums in it (8-byte stores, the
+      // second run of chunks 4 floats further on) and go on to the next item; the epilogue warps take it from here.
+      ptx::mbar_wait(stage_empty, st_ph ^ 1);
 #pragma unroll
-      for (int i = 0; i < 9; ++i) v9[i] = 0.f;
-      const int r0 = wq * 16 + (lane >> 2), cq = 2 * (lane & 3);
-#pragma unroll
-      for (int k = 0; k < per; ++k) {
-        ptx::named_bar_sync(1 + cw, 128);    // readers of the previous round are done
-#pragma unroll
-        for (int c = 0; c < nch; ++c) {
-          if (c == k || c == per + k) {
-            float* dst = xchg + (c == k ? 0 : 16);
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {      // 8-column halves of the chunk: accumulator group j = 2 c + h
-              const int j = 2 * c + h;
-              dst[r0 * kXchgStride + 8 * h + cq] = sum[4 * j];
-              dst[r0 * kXchgStride + 8 * h + cq + 1] = sum[4 * j + 1];
-              dst[(r0 + 8) * kXchgStride + 8 * h + cq] = sum[4 * j + 2];
-              dst[(r0 + 8) * kXchgStride + 8 * h + cq + 1] = sum[4 * j + 3];
-            }
-          }
-        }
-        ptx::named_bar_sync(1 + cw, 128);
-        if (k < my_chunks) {
-          float v[16];
-          const float4* srcp = reinterpret_cast<const float4*>(xchg + (t >> 1) * kXchgStride + grp * 16);
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const float4 f = srcp[q];
-            v[4 * q] = f.x; v[4 * q + 1] = f.y; v[4 * q + 2] = f.z; v[4 * q + 3] = f.w;
-          }
-          const int cg = n_tile * N + (first_chunk + k) * 16;
-          if (p.epi.mode == EPI_D2S_RDOT) {
-            // the host guarantees that a thread's columns are whole sub-pixels (rdot_parts == 1) or an equal share of
-            // one sub-pixel (rdot_parts > 1: each share writes its own partial plane set)
-            if (cg < p.epi.n_valid) {
-              const int ij = cg / p.epi.d2s_cout, cc = cg - ij * p.epi.d2s_cout;
-              rdot_accumulate16(p.epi, s_rdot, cg, cc, v, v9);
-              const bool last = p.epi.rdot_parts > 1 ? k + 1 == my_chunks : cc + 16 == p.epi.d2s_cout;
-              if (last && valid) rdot_flush(p.epi, g, img, y, x, ij, p.epi.rdot_parts > 1 ? cc / (per * 16) : 0, v9);
-            }
-          } else if (valid) {
-            if (p.epi.mode == EPI_D2S_TAPS) taps_store16(p.epi, g, img, y, x, cg, v);
-            else epilogue_store16(p.epi, g, n_total, img, y, x, cg, v);
-          }
-        }
+      for (int j = 0; j < N / 8; ++j) {
+        float* d = stage_row + 8 * j + (j / 2 >= per ? 4 : 0);
+        *reinterpret_cast<float2*>(d) = make_float2(sum[4 * j], sum[4 * j + 1]);
+        *reinterpret_cast<float2*>(d + 8 * kStride) = make_float2(sum[4 * j + 2], sum[4 * j + 3]);
       }
+      __syncwarp();
+      ptx::mbar_arrive_if(stage_full, lane == 0);
+      st_ph ^= 1;
+#ifdef DCSCN_TC_PHASES
+      ptx::named_bar_sync(1 + cw, 128);   // the warpgroup's slowest thread ends the epilogue
+      const long long ph_t2 = clock64();
+      ph_k += ph_t1 - ph_t0;
+      ph_e += ph_t2 - ph_t1;
+      ++ph_n;
+#endif
     }
+#ifdef DCSCN_TC_PHASES
+    if (t == 0) {
+      atomicAdd(&g_tc_phase[0], (unsigned long long)ph_k);
+      atomicAdd(&g_tc_phase[1], (unsigned long long)ph_e);
+      atomicAdd(&g_tc_phase[2], (unsigned long long)ph_n);
+    }
+#endif
   }
 
   __syncthreads();

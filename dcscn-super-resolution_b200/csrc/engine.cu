@@ -1088,9 +1088,13 @@ static int64_t workspace_bytes(const dcscn_handle* h) {
 }
 
 // --------------------------------------------------------------------------------------- plans ----
-// Shared memory of conv_tc_kernel left for its activation and weight rings (barriers, R-CNN1 taps and the epilogue
-// exchange take the rest).
-constexpr size_t kTcRingBudget = 227 * 1024 - 1024 - kTcBarrierBytes - kRdotSmemBytes - kXchgBytes;
+// Shared memory of conv_tc_kernel: at most kTcSmemMax per CTA, of which its barriers, 1 KB of alignment slack and the
+// fp32 hand-off tile of an n_pad-column tile leave the rest for the activation and weight rings.  The patch
+// (tc_patch_fits) and the ring depths (add_tc_launch) are both chosen against this budget.  The epilogue's copy of the
+// bias and slopes only takes what the rings leave over (add_tc_launch); the R-CNN1 taps of a launch that fuses R-CNN1
+// take it from there too, or from one weight tile (get_plan).
+constexpr size_t kTcSmemMax = 227 * 1024;
+static size_t tc_ring_budget(int n_pad) { return kTcSmemMax - 1024 - kTcBarrierBytes - tc_stage_bytes(n_pad); }
 
 // Whether a k x k layer (k > 1) can run on a TH x TW patch: its ky taps are read at row offsets of TW pixels inside one
 // activation box of TW x (TH + k - 1) pixels, which the swizzled operand descriptors allow only in whole 8-row atoms (TW
@@ -1099,7 +1103,7 @@ static bool tc_patch_fits(int nplanes, int n_pad, int ksz, int TH, int TW) {
   if (ksz == 1) return true;
   if (TW % 8 != 0) return false;
   return 2 * (size_t)nplanes * tc_a_plane_bytes(TW, TH, ksz) + 2 * (size_t)tc_w_tile_bytes(nplanes, n_pad) <=
-         kTcRingBudget;
+         tc_ring_budget(n_pad);
 }
 
 // 128-pixel rectangular patches; minimise padded area, prefer wide patches (contiguous TMA rows).  Returns false when no
@@ -1135,6 +1139,9 @@ static int encode_map(dcscn_handle* h, CUtensorMap* tm, const __half* base, int 
                 pitch, n, H, W, TH, TW);
   return 0;
 }
+
+// The epilogue's copy of a launch's bias and slopes (fp32, every column tile) in conv_tc_kernel's shared memory.
+static size_t tc_bias_bytes(const ConvTCParams& p) { return 2 * sizeof(float) * (size_t)p.n_tiles * p.n_pad; }
 
 static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, PlaneView src, int src_pitch, int n, int H, int W,
                          const EpiParams& epi) {
@@ -1182,7 +1189,7 @@ static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, PlaneView 
   // A 1x1 layer pairs one activation slot with one weight tile.
   const size_t a_slot = (size_t)planes(h) * tc_a_plane_bytes(TW, TH, t.ksz);
   const size_t w_tile = tc_w_tile_bytes(planes(h), t.n_pad);
-  const size_t budget = kTcRingBudget;
+  const size_t budget = tc_ring_budget(t.n_pad);
   int a_slots, w_slots;
   if (t.ksz == 1) {
     a_slots = w_slots = (int)std::min<size_t>(kMaxASlots, budget / (a_slot + w_tile));
@@ -1196,7 +1203,11 @@ static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, PlaneView 
                 t.name.c_str(), a_slot, w_tile);
   L.a_slots = a_slots;
   L.w_slots = w_slots;
-  L.smem = a_slots * a_slot + w_slots * w_tile + 1024 + kTcBarrierBytes + kRdotSmemBytes + kXchgBytes;
+  L.smem = a_slots * a_slot + w_slots * w_tile + 1024 + kTcBarrierBytes + tc_stage_bytes(t.n_pad);
+  // the epilogue warps read bias and slopes from shared memory when what the rings leave over holds them; a layer
+  // never gives up a ring slot for them (wide layers, e.g. the x5 ... x8 pixel shufflers, read them from global memory)
+  L.p.bias_smem = L.smem + tc_bias_bytes(L.p) <= kTcSmemMax;
+  if (L.p.bias_smem) L.smem += tc_bias_bytes(L.p);
   const long long tiles = (long long)n * g.tiles_x * g.tiles_y;
   const long long items = tiles * t.n_tiles;
   L.grid = (int)std::min<long long>(items, h->sm_count);
@@ -1340,6 +1351,10 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
     pl->unfused = L;
     pl->fused_index = (int)pl->tc.size() - 1;
     pl->fused_last = last_fuses(h, L.p.n_pad);
+    if (pl->fused_last && L.p.bias_smem) {   // the fused epilogues (EPI_D2S_TAPS / EPI_D2S_RDOT) read bias from global
+      L.smem -= tc_bias_bytes(L.p);
+      L.p.bias_smem = 0;
+    }
     if (pl->fused_last && h->fold.cout > 0) {
       // the folded layer (build_fold): same input, patch, rings and column-tile width, fewer column tiles
       const TcLayer& f = h->fold;
@@ -1362,6 +1377,13 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
       L.p.epi.rdot_w = h->d_last_w.get();
       L.p.epi.rdot_out = h->vbuf.get();
       L.p.epi.rdot_taps = klast * klast;
+      // the kernel stages the R-CNN1 taps behind the hand-off tile: weight tiles make room for them
+      const size_t w_tile = tc_w_tile_bytes(planes(h), L.p.n_pad);
+      for (L.smem += kRdotSmemBytes; L.smem > kTcSmemMax && L.w_slots > 2; L.smem -= w_tile) L.w_slots--;
+      if (L.smem > kTcSmemMax) {
+        fail("the fused R-CNN1 taps do not fit in shared memory beside two weight tiles (column tile %d)", L.p.n_pad);
+        return nullptr;
+      }
     }
     const int gparts = pl->fused_last ? L.p.epi.rdot_parts : 1;
     memset(&pl->gather, 0, sizeof(pl->gather));
@@ -1388,6 +1410,26 @@ static Plan* get_plan(dcscn_handle* h, int n, int H, int W) {
 }
 
 // ------------------------------------------------------------------------------------- forward ----
+#ifdef DCSCN_TC_PHASES
+// Diagnostic build: one stderr line per conv_tc_kernel launch with its phase cycles (g_tc_phase) and its plan; the launch
+// is waited for, so the timings of this build are not the product's.
+static int tc_phase_report(dcscn_handle* h, const TcLaunch& L, cudaStream_t st) {
+  unsigned long long c[4];
+  CUDA_TRY(cudaStreamSynchronize(st));
+  CUDA_TRY(cudaMemcpyFromSymbol(c, g_tc_phase, sizeof(c)));
+  const unsigned long long zero[4] = {};
+  CUDA_TRY(cudaMemcpyToSymbol(g_tc_phase, zero, sizeof(zero)));
+  std::string name = "?";
+  if (L.layer_fold) name = "Up-PS(fold)";
+  else if (L.layer_index >= 0 && !L.layer_bwd && L.layer_index < (int)h->tcl.size()) name = h->tcl[L.layer_index].name;
+  else if (L.layer_index >= 0 && L.layer_bwd && L.layer_index < (int)h->bwd.size()) name = "bwd:" + h->bwd[L.layer_index].name;
+  fprintf(stderr, "tc_phase %s mode=%d n_pad=%d n_tiles=%d patch=%dx%d a_slots=%d w_slots=%d smem=%zu k=%llu epi=%llu "
+          "items=%llu epw=%llu\n", name.c_str(), L.p.epi.mode, L.p.n_pad, L.p.n_tiles, L.p.g.TH, L.p.g.TW, L.a_slots,
+          L.w_slots, L.smem, c[0], c[1], c[2], c[3]);
+  return 0;
+}
+#endif
+
 template <int NPL, int N>
 static int launch_tc_inst(dcscn_handle* h, const TcLaunch& L, cudaStream_t st) {
   static bool attr_set_dev[64] = {};   // function attributes are per device
@@ -1398,7 +1440,11 @@ static int launch_tc_inst(dcscn_handle* h, const TcLaunch& L, cudaStream_t st) {
   }
   conv_tc_kernel<NPL, N><<<L.grid, kTcThreads, L.smem, st>>>(L.tm_hi, L.tm_lo, L.p, L.a_slots, L.w_slots);
   CUDA_TRY(cudaGetLastError());
+#ifdef DCSCN_TC_PHASES
+  return tc_phase_report(h, L, st);
+#else
   return 0;
+#endif
 }
 
 // The column-tile width is a template parameter of the kernel (the wgmma width is an immediate of the instruction).

@@ -99,16 +99,20 @@ __device__ __forceinline__ void store_planes16(__half* dst_hi, __half* dst_lo, s
 }
 
 // acc * out_scale + bias -> activation -> [inverted dropout] of 16 consecutive GEMM columns starting at `cg`; zn = fp16
-// pairs of min(z, 0), only formed when `want_zneg`.
-__device__ __forceinline__ void epilogue_values16(const EpiParams& e, const ConvGeom& g, int n_total, int img, int y, int x,
-                                                  int cg, const float (&acc)[16], float (&v)[16], uint32_t (&zn)[8],
+// pairs of min(z, 0), only formed when `want_zneg`.  `bias` / `alpha` are e.bias / e.alpha, read through the read-only
+// cache, or (kSmemBias) plain loads from copies in shared memory or, where the rings leave no room for those, from
+// e.bias / e.alpha.
+template <bool kSmemBias>
+__device__ __forceinline__ void epilogue_values16(const EpiParams& e, const float* bias, const float* alpha,
+                                                  const ConvGeom& g, int n_total, int img, int y, int x, int cg,
+                                                  const float (&acc)[16], float (&v)[16], uint32_t (&zn)[8],
                                                   bool want_zneg) {
-  const float4* b4 = reinterpret_cast<const float4*>(e.bias + cg);
-  const float4* a4 = reinterpret_cast<const float4*>(e.alpha + cg);
+  const float4* b4 = reinterpret_cast<const float4*>(bias + cg);
+  const float4* a4 = reinterpret_cast<const float4*>(alpha + cg);
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
-    float4 b = __ldg(b4 + q);
-    float4 a = __ldg(a4 + q);
+    float4 b = kSmemBias ? b4[q] : __ldg(b4 + q);
+    float4 a = kSmemBias ? a4[q] : __ldg(a4 + q);
     float t0 = fmaf(acc[4 * q + 0], e.out_scale, b.x);
     float t1 = fmaf(acc[4 * q + 1], e.out_scale, b.y);
     float t2 = fmaf(acc[4 * q + 2], e.out_scale, b.z);
@@ -137,13 +141,17 @@ __device__ __forceinline__ void epilogue_values16(const EpiParams& e, const Conv
   }
 }
 
-// One output pixel (img, y, x) of the LR grid, 16 consecutive GEMM columns starting at `cg`.
+// One output pixel (img, y, x) of the LR grid, 16 consecutive GEMM columns starting at `cg`.  kSmemBias: the bias and
+// slopes come from `bias` / `alpha` (conv_tc_kernel's epilogue warps: shared-memory copies when p.bias_smem).
+template <bool kSmemBias = false>
 __device__ __forceinline__ void epilogue_store16(const EpiParams& e, const ConvGeom& g, int n_total, int img, int y,
-                                                 int x, int cg, const float (&acc)[16]) {
+                                                 int x, int cg, const float (&acc)[16], const float* bias = nullptr,
+                                                 const float* alpha = nullptr) {
   float v[16];
   uint32_t zn[8];      // fp16 pairs of min(z, 0), only formed when a training segment asks for them
   const bool want_zneg = e.mode == EPI_PLANES && (e.seg[0].dst_zneg != nullptr || (e.num_seg > 1 && e.seg[1].dst_zneg != nullptr));
-  epilogue_values16(e, g, n_total, img, y, x, cg, acc, v, zn, want_zneg);
+  epilogue_values16<kSmemBias>(e, kSmemBias ? bias : e.bias, kSmemBias ? alpha : e.alpha, g, n_total, img, y, x, cg,
+                               acc, v, zn, want_zneg);
 
   if (e.mode == EPI_PLANES) {
 #pragma unroll
@@ -256,6 +264,8 @@ __device__ __forceinline__ void taps_store16(const EpiParams& e, const ConvGeom&
   const size_t HR_H = (size_t)g.H * r, HR_W = (size_t)g.W * r;
   const size_t plane = (size_t)g.n_img * HR_H * HR_W;
   const float4* b4 = reinterpret_cast<const float4*>(e.bias + cg);
+  // column cg + t is tap `tap` of sub-pixel (i, j): stepped from column to column instead of divided out of each
+  int tap = cg % taps, i = cg / taps / r, j = cg / taps % r;
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
     const float4 b = __ldg(b4 + q);
@@ -263,11 +273,13 @@ __device__ __forceinline__ void taps_store16(const EpiParams& e, const ConvGeom&
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       const int col = cg + 4 * q + u;
-      if (col >= e.n_valid) continue;
-      const int ij = col / taps, tap = col - ij * taps;
-      const int i = ij / r, j = ij - i * r;
+      if (col >= e.n_valid) return;
       const size_t pix = ((size_t)img * HR_H + (size_t)(y * r + i)) * HR_W + (size_t)(x * r + j);
       e.rdot_out[(size_t)tap * plane + pix] = fmaf(acc[4 * q + u], e.out_scale, bq[u]);
+      if (++tap == taps) {
+        tap = 0;
+        if (++j == r) { j = 0; ++i; }
+      }
     }
   }
 }
