@@ -128,6 +128,7 @@ class Checker:
     def __init__(self):
         self.worst, self.signed = {}, {}
         self.gm = {}      # per activated layer: the output gradient after dropout, g mask fp32(1 / keep) (check_step)
+        self.sums = {}    # per variable: (fp64 sum / G, its accumulation bar / G, L2 term) before finalized (check_step)
 
     def add(self, name, got, ref, bar, signed=False):
         got = torch.as_tensor(got).to(dev(), torch.float64) if not torch.is_tensor(got) else got.to(dev(), torch.float64)
@@ -163,13 +164,22 @@ def after_dropout(g, mask, keep):
     return g * (1.0 if mask is None else mask) * float(np.float32(1.0) / np.float32(keep))
 
 
-def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None, act="prelu"):
+def finalized(s, b, dec):
+    """get_grad of a variable whose fp32 sum over the batch, over G, is `s` with accumulation bar `b`, plus its L2 term
+    `dec`, rounded once: (reference, bar)."""
+    ref = s + dec
+    return ref, b + U24 * ref.abs() + U24 * dec.abs() + 1e-45
+
+
+def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None, act="prelu", bar_n=None):
     """Every backward kernel of the last train step of `eng` (run with grad_capture = 1, activator `act`) against its
     isolated reference.  `get_grad(name)` returns a variable's gradient as get_grad does (default: eng.get_grad); a wide
     depthwise-separable graph passes its composed filters as the conv_W entries of `w` and reads their gradients from
-    "dWc:"."""
+    "dWc:".  The bars of the filter, bias and slope sums are those of a batch of `bar_n` images (default: this step's):
+    a sub-batch of a larger step passes that step's n, and chk.sums then holds its share of the larger step's sums."""
     cfg = O.OracleConfig(**kw)
     n, h, wd = x.shape[:3]
+    nb = bar_n or n
     s = cfg.scale
     f = O.feature_filters(cfg)
     L = cfg.layers
@@ -194,8 +204,8 @@ def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None, act="prelu"
         """get_grad of a variable whose fp32 sum (scaled by G) is `ssum` with accumulation bar `bar_sum`."""
         wv = torch.from_numpy(w[name].astype(np.float32)).to(dev(), torch.float64)
         dec = float(l2) * wv if name.endswith("conv_W") else torch.zeros_like(wv)
-        ref = ssum / G + dec
-        return ref, bar_sum / G + U24 * ref.abs() + U24 * dec.abs() + 1e-45
+        chk.sums[name] = (ssum / G, bar_sum / G, dec)
+        return finalized(ssum / G, bar_sum / G, dec)
 
     # ---- loss
     yp = t64(eng.get_train_tensor("y_", (n, s * h, s * wd, 1)))
@@ -209,7 +219,7 @@ def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None, act="prelu"
     wr = w["R-CNN1/conv_W"]
     kr = wr.shape[0]
     ssum, sabs = wgrad(hr, dY, kr), wgrad(hr.abs(), dY.abs(), kr)
-    ref, bar = finalize("R-CNN1/conv_W", ssum, count * U24 * sabs)
+    ref, bar = finalize("R-CNN1/conv_W", ssum, nb * s * h * s * wd * U24 * sabs)
     chk.add("last_wgrad", grad("R-CNN1/conv_W"), ref, bar, signed=True)
     v = s2d(dgrad(dY, wr), r_last)
     sv = s2d(dgrad(dY.abs(), np.abs(wr)), r_last)
@@ -224,12 +234,12 @@ def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None, act="prelu"
         return v, (tc_units(kk, cin_pad, 0, 2) + 1) * U23 * sv + stored(v)
 
     def wgrad_tc(name, a, dz, kk, a_rows, dz_cols, hh, ww):
-        cpc, ksplit = wgrad_tc_chain(sm, n, hh, ww, kk, a_rows, dz_cols)
+        cpc, ksplit = wgrad_tc_chain(sm, nb, hh, ww, kk, a_rows, dz_cols)
         ssum, sabs = wgrad(a, dz, kk), wgrad(a.abs(), dz.abs(), kk)
         return finalize(name, ssum, ((6 * cpc) * 17 * U23 + U22 + (ksplit + 1) * U24) * sabs)
 
     def conv_b(name, dz):
-        ref, bar = finalize(name, dz.sum(dim=(0, 2, 3)), (dz[0, 0].numel() * n + 4) * U24 * dz.abs().sum(dim=(0, 2, 3)))
+        ref, bar = finalize(name, dz.sum(dim=(0, 2, 3)), (dz[0, 0].numel() * nb + 4) * U24 * dz.abs().sum(dim=(0, 2, 3)))
         chk.add("bias sums", grad(name), ref, bar)
 
     # ---- pixel shuffler(s)
@@ -299,7 +309,7 @@ def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None, act="prelu"
         if act == "prelu":
             term = torch.where(neg, gm * zn, torch.zeros_like(gm))
             pn = "%s/prelu/%s_prelu" % (scope, scope)
-            ref, bar = finalize(pn, term.sum(dim=(0, 2, 3)), (n * h * wd + 4) * U24 * term.abs().sum(dim=(0, 2, 3)))
+            ref, bar = finalize(pn, term.sum(dim=(0, 2, 3)), (nb * h * wd + 4) * U24 * term.abs().sum(dim=(0, 2, 3)))
             chk.add("act_grad slope sums", grad(pn), ref, bar)
         return got
 
@@ -336,7 +346,7 @@ def check_step(eng, kw, w, x, x2, y, keep, seed, chk, get_grad=None, act="prelu"
         if i == 0:
             a = t64(x)
             ssum, sabs = wgrad(a, dz, k), wgrad(a.abs(), dz.abs(), k)
-            ref, bar = finalize(sc + "/conv_W", ssum, n * h * wd * U24 * sabs)
+            ref, bar = finalize(sc + "/conv_W", ssum, nb * h * wd * U24 * sabs)
             chk.add("first_wgrad / wgrad (CNN1)", grad(sc + "/conv_W"), ref, bar, signed=True)
         else:
             ref, bar = wgrad_tc(sc + "/conv_W", feats[i - 1], dz, k, f[i - 1], f[i], h, wd)
