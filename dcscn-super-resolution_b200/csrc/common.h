@@ -92,6 +92,8 @@ struct ConvTCParams {
   int n_tiles;           // column tiles (N > kMaxTileN is split)
   int n_pad;             // columns per tile, multiple of 16, <= kMaxTileN (112)
   int seg_chunks;        // pipeline stages per accumulation segment (fp32 promotion period)
+  int chunk_box;         // k > 1: one (TW + k - 1) x (TH + k - 1) activation box per chunk serves all k x k taps (TW = 8);
+                         // 0: one TW x (TH + k - 1) box per (chunk, kx)
   const __half* wpack;   // packed weights [n_tile][tap][chunk][plane][n_pad x 64] (pre-swizzled)
   int bias_smem;         // conv_tc_kernel keeps a copy of epi.bias / epi.alpha in shared memory (add_tc_launch)
   EpiParams epi;

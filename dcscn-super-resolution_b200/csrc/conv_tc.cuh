@@ -5,11 +5,13 @@
 //
 // GEMM view:  D[M = 128 pixels (TH x TW patch), N = cout (padded to 16, <= 112 per column tile)]
 //             = sum over 64-channel input chunks, taps (kx, ky) of  A_tap[128 x 64] * W_tap[64 x N]
-//   * A tiles are fetched by TMA (4-D tiled tensor map over the NHWC fp16 plane).  A k x k layer (k = 3 or 5) loads ONE
-//     box of TW x (TH + k - 1) pixels per (chunk, kx), its origin shifted by (kx - k / 2, -k / 2); the k ky taps read it
-//     at row offsets 0, TW, ..., (k - 1) TW.  The host only picks patches with TW a multiple of 8, so every offset is a
-//     whole number of 8-row swizzle atoms and the operand descriptors stay valid.  TMA zero-fills out-of-image pixels, which IS TF's SAME padding - no halo handling in
-//     the kernel.  A 1x1 layer loads one TW x TH box per chunk.
+//   * A tiles are fetched by TMA (4-D tiled tensor map over the NHWC fp16 plane).  A k x k layer (k = 3 or 5) on a 16 x 8
+//     patch whose boxes fit (p.chunk_box) loads ONE box of W_box x (TH + k - 1) pixels per chunk, W_box = TW + k - 1,
+//     at origin (-k / 2, -k / 2): each 8-pixel patch row is one 8-row operand group, W_box rows apart, and tap (kx, ky)
+//     starts kx + ky W_box rows in - not a whole swizzle atom, which the address-based swizzle allows (make_smem_desc).
+//     Otherwise it loads one box of TW x (TH + k - 1) pixels per (chunk, kx), its origin shifted by (kx - k / 2, -k / 2);
+//     the k ky taps read it at row offsets 0, TW, ..., (k - 1) TW, with TW a multiple of 8.  TMA zero-fills out-of-image
+//     pixels, which IS TF's SAME padding - no halo handling in the kernel.  A 1x1 layer loads one TW x TH box per chunk.
 //   * fp32-equivalent precision from fp16 tensor cores:  a = a_hi + a_lo,  w*2^s = w_hi + w_lo
 //     (each 11-bit significands), D += a_hi*w_hi + a_lo*w_hi + a_hi*w_lo   (3 x m64nNk16 wgmma per 16 channels,
 //     fp32 accumulation in registers).  NPLANES == 1 is the single-pass fp16 "fast" mode.
@@ -22,7 +24,7 @@
 //     caps a column tile at 112 (kMaxTileN).
 //   * The column-tile width N is a template parameter: the wgmma width is an immediate of the instruction, and a
 //     straight-line run of same-width wgmma needs no per-instruction selection.
-//   * Two shared-memory rings with their own full/empty mbarriers: activation slots (one per (chunk, kx)) and weight
+//   * Two shared-memory rings with their own full/empty mbarriers: activation slots (one per chunk or (chunk, kx)) and weight
 //     tiles (one per (tap, chunk), read from the packed image [n_tile][tap][chunk]).  The consumers commit one wgmma
 //     group per weight tile and release a slot as soon as `wgmma.wait_group 1` shows the group that last read it
 //     has completed, so both rings work purely as prefetch depth.  A weight tile arrives as one bulk copy.
@@ -67,16 +69,22 @@ struct TcSmem {
 };
 
 // wgmma shared-memory matrix descriptor of a K-major swizzled operand tile: start address >> 4 in [0,14), leading
-// byte offset (unused for swizzled K-major, 1) in [16,30), stride byte offset >> 4 in [32,46), layout type in [62,64).
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(TcSmem::kSbo >> 4) << 32) |
+// byte offset (unused for swizzled K-major, 1) in [16,30), stride byte offset (between 8-row groups) >> 4 in [32,46),
+// base offset 0 in [49,52), layout type in [62,64).  The 128-byte swizzle is a function of the shared-memory address
+// itself, as TMA writes it (measured on H100, tests/test_gpu_wgmma_desc.py): a start any whole number of 128-byte rows
+// into an atom, with any multiple of 128 bytes as the stride, reads the rows TMA stored there with base offset 0.
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t sbo = TcSmem::kSbo) {
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(sbo >> 4) << 32) |
          (TcSmem::kLayout << 62);
 }
 
-// Bytes of one activation plane in a ring slot: the TMA box of TW x (TH + ksz - 1) pixels, rounded up to 1024 bytes
-// so that every slot and plane starts on a swizzle-atom boundary.
-__host__ __device__ inline uint32_t tc_a_plane_bytes(int TW, int TH, int ksz) {
-  return ((uint32_t)TW * (uint32_t)(TH + ksz - 1) * (uint32_t)kTcKC * 2u + 1023u) & ~1023u;
+// Width of a k x k layer's activation box: TW + k - 1 when one box per chunk serves all taps (chunk_box), else TW.
+__host__ __device__ inline int tc_box_w(int TW, int ksz, int chunk_box) { return chunk_box ? TW + ksz - 1 : TW; }
+
+// Bytes of one activation plane in a ring slot: the TMA box of box_w x (TH + ksz - 1) pixels, rounded up to 1024
+// bytes so that every slot and plane starts on a swizzle-atom boundary.
+__host__ __device__ inline uint32_t tc_a_plane_bytes(int box_w, int TH, int ksz) {
+  return ((uint32_t)box_w * (uint32_t)(TH + ksz - 1) * (uint32_t)kTcKC * 2u + 1023u) & ~1023u;
 }
 __host__ __device__ inline uint32_t tc_w_tile_bytes(int nplanes, int n_pad) {
   return (uint32_t)nplanes * (uint32_t)n_pad * (uint32_t)kTcKC * 2u;
@@ -95,6 +103,16 @@ __host__ __device__ constexpr uint32_t tc_stage_bytes(int n_pad) { return 128u *
 // consumer warpgroups, [3] the epilogue warps' busy cycles (summed over the kEpiWarps warps).  The host reads and
 // clears them after each launch (tc_phase_report).
 __device__ unsigned long long g_tc_phase[4];
+#endif
+
+// Diagnostic builds only (scripts/tc_bound.py), whose outputs are meaningless: -DDCSCN_TC_BOUND=1 (fill only) - the
+// consumers wait for every slot and release it without issuing wgmma; -DDCSCN_TC_BOUND=2 (math only) - once every
+// slot of a ring has been filled, the producer arrives on its full barrier without copying.  Their launch times bound
+// the K loop from the fill side and the wgmma side.
+#if defined(DCSCN_TC_BOUND) && DCSCN_TC_BOUND == 2
+#define DCSCN_TC_COPY(filled, slots) ((filled)++ < (slots))
+#else
+#define DCSCN_TC_COPY(filled, slots) ((void)(filled), true)
 #endif
 
 // One wgmma batch: the products of KS consecutive 16-channel K slices of a weight tile, committed as one group.
@@ -127,9 +145,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const ConvGeom& g = p.g;
   const int ksz = p.ksz;
-  const uint32_t A_PLANE = tc_a_plane_bytes(g.TW, g.TH, ksz);
+  const bool chunk_box = p.chunk_box != 0;
+  const int box_w = tc_box_w(g.TW, ksz, p.chunk_box);
+  const uint32_t A_PLANE = tc_a_plane_bytes(box_w, g.TH, ksz);
   const uint32_t A_SLOT = NPLANES * A_PLANE;
-  const uint32_t A_TX = (uint32_t)NPLANES * (uint32_t)g.TW * (uint32_t)(g.TH + ksz - 1) * kTcKC * 2u;  // bytes TMA delivers
+  const uint32_t A_TX = (uint32_t)NPLANES * (uint32_t)box_w * (uint32_t)(g.TH + ksz - 1) * kTcKC * 2u;  // bytes TMA delivers
   constexpr uint32_t B_BYTES = N * kTcKC * 2;
   constexpr uint32_t W_TILE = NPLANES * B_BYTES;
   uint8_t* a_ring = smem;
@@ -192,6 +212,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
       if (NPLANES == 2) ptx::prefetch_tensormap(&tm_lo);
       int as = 0, ws = 0;
       uint32_t a_ph = 0, w_ph = 0;
+      int a_filled = 0, w_filled = 0;   // DCSCN_TC_BOUND == 2 only
       for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
         const int n_tile = item % p.n_tiles;
         const int tile = item / p.n_tiles;
@@ -202,18 +223,28 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
         const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.wpack) + (size_t)n_tile * ksz * ksz * chunks * W_TILE;
         for (int ch = 0; ch < chunks; ++ch) {
           for (int dx = 0; dx < ksz; ++dx) {
-            ptx::mbar_wait(&a_empty[as], a_ph ^ 1);
-            uint8_t* ad = a_ring + (size_t)as * A_SLOT;
-            ptx::mbar_arrive_expect_tx(&a_full[as], A_TX);
-            ptx::tma_load_4d(ad, &tm_hi, &a_full[as], ch * kTcKC, x0 + dx, y0, img);
-            if (NPLANES == 2) ptx::tma_load_4d(ad + A_PLANE, &tm_lo, &a_full[as], ch * kTcKC, x0 + dx, y0, img);
-            if (++as == a_slots) { as = 0; a_ph ^= 1; }
+            if (!chunk_box || dx == 0) {   // a chunk box is loaded once, at origin (-k / 2, -k / 2)
+              ptx::mbar_wait(&a_empty[as], a_ph ^ 1);
+              uint8_t* ad = a_ring + (size_t)as * A_SLOT;
+              if (DCSCN_TC_COPY(a_filled, a_slots)) {
+                ptx::mbar_arrive_expect_tx(&a_full[as], A_TX);
+                ptx::tma_load_4d(ad, &tm_hi, &a_full[as], ch * kTcKC, x0 + dx, y0, img);
+                if (NPLANES == 2) ptx::tma_load_4d(ad + A_PLANE, &tm_lo, &a_full[as], ch * kTcKC, x0 + dx, y0, img);
+              } else {
+                ptx::mbar_arrive(&a_full[as]);
+              }
+              if (++as == a_slots) { as = 0; a_ph ^= 1; }
+            }
             for (int dy = 0; dy < ksz; ++dy) {
               ptx::mbar_wait(&w_empty[ws], w_ph ^ 1);
               uint8_t* wd = w_ring + (size_t)ws * W_TILE;
-              ptx::mbar_arrive_expect_tx(&w_full[ws], W_TILE);
-              const uint8_t* wtile = wsrc + (size_t)((dy * ksz + dx) * chunks + ch) * W_TILE;
-              ptx::bulk_load(wd, wtile, W_TILE, &w_full[ws]);
+              if (DCSCN_TC_COPY(w_filled, w_slots)) {
+                ptx::mbar_arrive_expect_tx(&w_full[ws], W_TILE);
+                const uint8_t* wtile = wsrc + (size_t)((dy * ksz + dx) * chunks + ch) * W_TILE;
+                ptx::bulk_load(wd, wtile, W_TILE, &w_full[ws]);
+              } else {
+                ptx::mbar_arrive(&w_full[ws]);
+              }
               if (++ws == w_slots) { ws = 0; w_ph ^= 1; }
             }
           }
@@ -301,8 +332,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
     const bool strict = p.seg_chunks == 1;
     const uint32_t a_ring_u32 = ptx::smem_u32(a_ring);
     const uint32_t w_ring_u32 = ptx::smem_u32(w_ring);
-    const uint32_t a_off = (uint32_t)(cw * 64 * TcSmem::kRowBytes);
-    const uint32_t dy_step = (uint32_t)(g.TW * TcSmem::kRowBytes);   // one image row of the box: whole 8-row atoms
+    // A chunk box holds the patch's 8-pixel rows W_box = TW + k - 1 pixels apart: each is one 8-row group of the operand
+    // (stride W_box rows), tap (kx, ky) starts kx + ky W_box rows in, and this half's rows start TH / 2 box rows on.
+    // A (chunk, kx) box is TW pixels wide: whole 8-row groups, 1024 bytes apart, and ky starts ky TW rows in.
+    const uint32_t a_off = (uint32_t)((chunk_box ? cw * (g.TH / 2) * box_w : cw * 64) * TcSmem::kRowBytes);
+    const uint32_t a_sbo = chunk_box ? (uint32_t)(box_w * TcSmem::kRowBytes) : (uint32_t)TcSmem::kSbo;
+    const uint32_t dy_step = (uint32_t)(box_w * TcSmem::kRowBytes);   // one image row of the box
     // the wgmma layout gives a thread rows 16 wq + lane / 4 (+ 8) of its half and column pairs 8 j + 2 (lane % 4)
     float* stage_row = s_stage + (cw * 64 + wq * 16 + (lane >> 2)) * kStride + 2 * (lane & 3);
     uint32_t st_ph = 0;
@@ -337,16 +372,24 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
         int ksteps = p.cin_pad - ch * kTcKC;
         ksteps = (ksteps > kTcKC ? kTcKC : ksteps) >> 4;
         for (int dx = 0; dx < ksz; ++dx) {
-          ptx::mbar_wait(&a_full[as], a_ph);
-          const uint32_t a_addr = a_ring_u32 + (uint32_t)as * A_SLOT + a_off;
+          if (!chunk_box || dx == 0) ptx::mbar_wait(&a_full[as], a_ph);
+          const uint32_t a_addr =
+              a_ring_u32 + (uint32_t)as * A_SLOT + a_off + (chunk_box ? (uint32_t)dx * TcSmem::kRowBytes : 0u);
           for (int dy = 0; dy < ksz; ++dy) {
             ptx::mbar_wait(&w_full[ws], w_ph);
             const uint32_t w_addr = w_ring_u32 + (uint32_t)ws * W_TILE;
-            const uint64_t a_hi = make_smem_desc(a_addr + (uint32_t)dy * dy_step);
-            const uint64_t a_lo = make_smem_desc(a_addr + (uint32_t)dy * dy_step + A_PLANE);
+            const uint64_t a_hi = make_smem_desc(a_addr + (uint32_t)dy * dy_step, a_sbo);
+            const uint64_t a_lo = make_smem_desc(a_addr + (uint32_t)dy * dy_step + A_PLANE, a_sbo);
             const uint64_t b_hi = make_smem_desc(w_addr);
             const uint64_t b_lo = make_smem_desc(w_addr + B_BYTES);
-            const bool a_done = dy == ksz - 1;   // last tap that reads this activation slot
+            // last tap that reads this activation slot
+            const bool a_done = dy == ksz - 1 && (!chunk_box || dx == ksz - 1);
+#if defined(DCSCN_TC_BOUND) && DCSCN_TC_BOUND == 1
+            release_w(ws);
+            if (a_done) release_a(as);
+            if (++ws == w_slots) { ws = 0; w_ph ^= 1; }
+            continue;
+#endif
             if (strict) {
               // every 16-channel K slice (its three products) is promoted on its own
 #pragma unroll 1
@@ -392,7 +435,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_hi, const __grid_constant_
             }
             if (++ws == w_slots) { ws = 0; w_ph ^= 1; }
           }
-          if (++as == a_slots) { as = 0; a_ph ^= 1; }
+          if ((!chunk_box || dx == ksz - 1) && ++as == a_slots) { as = 0; a_ph ^= 1; }
         }
       }
       // the last weight tile ended a segment, so every group has completed; saying so here keeps ptxas from placing

@@ -1096,27 +1096,45 @@ static int64_t workspace_bytes(const dcscn_handle* h) {
 constexpr size_t kTcSmemMax = 227 * 1024;
 static size_t tc_ring_budget(int n_pad) { return kTcSmemMax - 1024 - kTcBarrierBytes - tc_stage_bytes(n_pad); }
 
-// Whether a k x k layer (k > 1) can run on a TH x TW patch: its ky taps are read at row offsets of TW pixels inside one
-// activation box of TW x (TH + k - 1) pixels, which the swizzled operand descriptors allow only in whole 8-row atoms (TW
-// a multiple of 8), and two such boxes plus two weight tiles must fit in shared memory.
+// Whether a k x k layer (k > 1) can load one activation box of (TW + k - 1) x (TH + k - 1) pixels per 64-channel chunk
+// for all k x k taps (ConvTCParams::chunk_box): the patch's 8-pixel rows must each be one 8-row operand group (TW = 8),
+// and two such boxes must fit beside three weight tiles (with two, 112-column layers ran 17-20 % slower than with
+// (chunk, kx) boxes).  At k = 3 a chunk then fills 10 x 18 = 180 pixels instead of the 3 x 16 x 10 = 480 of an 8 x 16
+// patch's three (chunk, kx) boxes.
+static bool tc_chunk_box(int nplanes, int n_pad, int ksz, int TH, int TW) {
+  if (ksz == 1 || TW != 8) return false;
+  return 2 * (size_t)nplanes * tc_a_plane_bytes(tc_box_w(TW, ksz, 1), TH, ksz) +
+             3 * (size_t)tc_w_tile_bytes(nplanes, n_pad) <= tc_ring_budget(n_pad);
+}
+
+// Whether a k x k layer (k > 1) can run on a TH x TW patch: with a chunk box (tc_chunk_box), or else with one box of
+// TW x (TH + k - 1) pixels per (chunk, kx) whose ky taps are read at row offsets of TW pixels, which the swizzled
+// operand descriptors allow only in whole 8-row groups (TW a multiple of 8); two such boxes plus two weight tiles must
+// fit in shared memory.
 static bool tc_patch_fits(int nplanes, int n_pad, int ksz, int TH, int TW) {
-  if (ksz == 1) return true;
+  if (ksz == 1 || tc_chunk_box(nplanes, n_pad, ksz, TH, TW)) return true;
   if (TW % 8 != 0) return false;
   return 2 * (size_t)nplanes * tc_a_plane_bytes(TW, TH, ksz) + 2 * (size_t)tc_w_tile_bytes(nplanes, n_pad) <=
          tc_ring_budget(n_pad);
 }
 
-// 128-pixel rectangular patches; minimise padded area, prefer wide patches (contiguous TMA rows).  Returns false when no
-// patch suits the layer.
+// 128-pixel rectangular patches; minimise padded area, prefer wide patches (contiguous TMA rows).  A k x k layer
+// (k > 1) takes the 16 x 8 patch with a chunk box unless another patch pads less.  Returns false when no patch suits
+// the layer.
 static bool choose_patch(int H, int W, int nplanes, int n_pad, int ksz, int* TH, int* TW) {
   static const int cand[][2] = {{8, 16}, {4, 32}, {16, 8}, {2, 64}, {32, 4}, {1, 128}, {64, 2}, {128, 1}};
   long long best = -1;
+  auto area = [&](int th, int tw) { return (long long)((H + th - 1) / th) * th * ((W + tw - 1) / tw) * tw; };
+  if (tc_chunk_box(nplanes, n_pad, ksz, 16, 8)) {
+    best = area(16, 8);
+    *TH = 16;
+    *TW = 8;
+  }
   for (auto& c : cand) {
     const int th = c[0], tw = c[1];
     if (!tc_patch_fits(nplanes, n_pad, ksz, th, tw)) continue;
-    long long area = (long long)((H + th - 1) / th) * th * ((W + tw - 1) / tw) * tw;
-    if (best < 0 || area < best) {
-      best = area;
+    if (best < 0 || area(th, tw) < best) {
+      best = area(th, tw);
       *TH = th;
       *TW = tw;
     }
@@ -1150,19 +1168,23 @@ static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, PlaneView 
   int TH = 0, TW = 0;
   if (!choose_patch(H, W, planes(h), t.n_pad, t.ksz, &TH, &TW))
     return fail("layer %s: no pixel patch fits a %dx%d filter in shared memory", t.name.c_str(), t.ksz, t.ksz);
-  // the kernel's ky taps start TW pixels apart inside the box: whole 8-row swizzle atoms, or the operands are misread
-  if (t.ksz > 1 && TW % 8 != 0)
+  const int chunk_box = tc_chunk_box(planes(h), t.n_pad, t.ksz, TH, TW);
+  // without a chunk box the kernel's ky taps start TW pixels apart inside the box: whole 8-row operand groups, or the
+  // operands are misread
+  if (t.ksz > 1 && !chunk_box && TW % 8 != 0)
     return fail("internal: layer %s: patch width %d is not a whole number of swizzle atoms", t.name.c_str(), TW);
   ConvGeom g{n, H, W, (W + TW - 1) / TW, (H + TH - 1) / TH, TW, TH};
   const int box_rows = TH + t.ksz - 1;   // a k x k layer's box carries the rows of all k ky taps
-  if (encode_map(h, &L.tm_hi, src.hi, t.cin_pad, src_pitch, n, H, W, box_rows, TW)) return 1;
+  const int box_w = tc_box_w(TW, t.ksz, chunk_box);   // and with a chunk box the columns of all k kx taps
+  if (encode_map(h, &L.tm_hi, src.hi, t.cin_pad, src_pitch, n, H, W, box_rows, box_w)) return 1;
   if (planes(h) == 2) {
-    if (encode_map(h, &L.tm_lo, src.lo, t.cin_pad, src_pitch, n, H, W, box_rows, TW)) return 1;
+    if (encode_map(h, &L.tm_lo, src.lo, t.cin_pad, src_pitch, n, H, W, box_rows, box_w)) return 1;
   } else {
     L.tm_lo = L.tm_hi;
   }
   L.p.g = g;
   L.p.ksz = t.ksz;
+  L.p.chunk_box = chunk_box;
   L.p.cin_pad = t.cin_pad;
   L.p.chunks = (t.cin_pad + kTcKC - 1) / kTcKC;
   L.p.n_tiles = t.n_tiles;
@@ -1184,15 +1206,19 @@ static int add_tc_launch(dcscn_handle* h, Plan* pl, const TcLayer& t, PlaneView 
   }
   L.p.epi.n_valid = t.n_valid;
 
-  // Ring depths.  The consumers release a slot one weight tile late, so each ring needs at least two slots.  A k x k layer
-  // reads k weight tiles per activation slot: three activation slots when four weight tiles still fit, else two.
-  // A 1x1 layer pairs one activation slot with one weight tile.
-  const size_t a_slot = (size_t)planes(h) * tc_a_plane_bytes(TW, TH, t.ksz);
+  // Ring depths.  The consumers release a slot one weight tile late, so each ring needs at least two slots.  With a
+  // chunk box a k x k layer reads k x k weight tiles per activation slot: two activation slots (one chunk ahead) and
+  // the rest in weight tiles.  Without one it reads k weight tiles per activation slot: three activation slots when
+  // four weight tiles still fit, else two.  A 1x1 layer pairs one activation slot with one weight tile.
+  const size_t a_slot = (size_t)planes(h) * tc_a_plane_bytes(box_w, TH, t.ksz);
   const size_t w_tile = tc_w_tile_bytes(planes(h), t.n_pad);
   const size_t budget = tc_ring_budget(t.n_pad);
   int a_slots, w_slots;
   if (t.ksz == 1) {
     a_slots = w_slots = (int)std::min<size_t>(kMaxASlots, budget / (a_slot + w_tile));
+  } else if (chunk_box) {
+    a_slots = 2;
+    w_slots = (int)std::min<size_t>(kMaxWSlots, (budget - a_slots * a_slot) / w_tile);
   } else {
     a_slots = 3;
     if (budget < a_slots * a_slot + 4 * w_tile) a_slots = 2;
@@ -1424,8 +1450,8 @@ static int tc_phase_report(dcscn_handle* h, const TcLaunch& L, cudaStream_t st) 
   else if (L.layer_index >= 0 && !L.layer_bwd && L.layer_index < (int)h->tcl.size()) name = h->tcl[L.layer_index].name;
   else if (L.layer_index >= 0 && L.layer_bwd && L.layer_index < (int)h->bwd.size()) name = "bwd:" + h->bwd[L.layer_index].name;
   fprintf(stderr, "tc_phase %s mode=%d n_pad=%d n_tiles=%d patch=%dx%d a_slots=%d w_slots=%d smem=%zu k=%llu epi=%llu "
-          "items=%llu epw=%llu\n", name.c_str(), L.p.epi.mode, L.p.n_pad, L.p.n_tiles, L.p.g.TH, L.p.g.TW, L.a_slots,
-          L.w_slots, L.smem, c[0], c[1], c[2], c[3]);
+          "items=%llu epw=%llu chunk_box=%d\n", name.c_str(), L.p.epi.mode, L.p.n_pad, L.p.n_tiles, L.p.g.TH, L.p.g.TW,
+          L.a_slots, L.w_slots, L.smem, c[0], c[1], c[2], c[3], L.p.chunk_box);
   return 0;
 }
 #endif
